@@ -1,5 +1,5 @@
 /*
- * qrec.h -- C ABI of libqrec.so, the B200 (sm_100a) engine behind QRec's
+ * qrec.h -- C ABI of libqrec.so, the H100 (sm_90a) engine behind QRec's
  * embedding-training hot path.
  *
  * The reference (Coder-Yu/QRec) is pure Python and defines no FFI; its plugin
@@ -36,7 +36,7 @@ extern "C" {
 #define QREC_ERR_NOMEM (-4)
 
 const char* qrec_last_error(void);
-/* "qrec-b200 <semver> sm_100a" */
+/* "qrec-b200 <semver> sm_90a" */
 const char* qrec_version(void);
 /* number of kernels this library has launched in this process (bench `gpu_launches`) */
 int64_t qrec_launch_count(void);
@@ -215,10 +215,11 @@ int qrec_bpr_sgd_batch_tma_f32(float* dev_P, float* dev_Q, int32_t d, int64_t n,
  * user's positives in CSR order): a lane group keeps P[u] in registers across the user's triples, so
  * P[u] is updated sequentially inside a user -- as in the reference -- and read/written once per
  * user; the item rows are gathered and scatter-added per triple (atomic sum across users).
- * rowptr: int64[n_users+1]; i, j: int32[n], n = rowptr[n_users], in that order.  Work is split into
- * 32-triple chunks of the CSR order (balanced for any degree distribution); a user spanning several
- * chunks receives the sum of the chunks' P deltas.  d multiple of 4, <= 128. */
-int qrec_bpr_sgd_usermajor_f32(float* dev_P, float* dev_Q, int32_t d, int32_t n_users, int64_t n,
+ * rowptr: int64[n_users+1]; i, j: int32[n], n = rowptr[n_users], in that order; num_items = rows of Q.
+ * Every user is processed whole by one lane group; the stream is swept in waves, each reading the item
+ * table as the earlier waves left it, so the result does not depend on timing (up to the summation order
+ * of the scatter-adds).  d multiple of 4, <= 128. */
+int qrec_bpr_sgd_usermajor_f32(float* dev_P, float* dev_Q, int32_t d, int32_t n_users, int64_t n, int32_t num_items,
                                const int64_t* dev_rowptr, const int32_t* dev_i, const int32_t* dev_j,
                                float lr, float reg_u, float reg_i, double* dev_loss, void* stream);
 
@@ -246,9 +247,8 @@ int qrec_bpr_epoch_usermajor_tma_f32(float* dev_P, float* dev_Q, int32_t d, int3
 /* The fused epoch with a pre-test in the sampler: rated_sig holds 16 words per user, bit (c & 511) set
  * for every rated column c (qrec_rated_signature_build; static per data set).  A clear bit proves a
  * draw is not rated, so about 1 - deg/512 of the draws skip the binary search -- the dependent-load
- * chain that holds 20 % of the kernel's stall samples (profiles/README.md).  No false negatives:
- * the negatives, hence P and Q, are identical to qrec_bpr_epoch_usermajor_f32.  d in {16,32,64,128}.
- * STATUS: written after round 1's GPU budget was spent; compiled, not yet run on hardware. */
+ * chain of the sampler.  No false negatives:
+ * the negatives, hence P and Q, are identical to qrec_bpr_epoch_usermajor_f32.  d in {16,32,64,128}. */
 int qrec_rated_signature_build(int32_t n_users, const int64_t* dev_rated_rowptr, const int32_t* dev_rated_cols,
                                uint32_t* dev_sig, void* stream);
 int qrec_bpr_epoch_usermajor_sig_f32(float* dev_P, float* dev_Q, int32_t d, int32_t n_users, int64_t n,
@@ -302,9 +302,9 @@ int qrec_score_topn_f32(const float* dev_U, const float* dev_V, int32_t d, int32
                         const int32_t* dev_user_ids, int32_t n_rows, const int64_t* dev_rated_rowptr,
                         const int32_t* dev_rated_cols, float rated_value, int32_t N, int32_t* dev_out_ids,
                         float* dev_out_scores, void* stream);
-/* The same contract with the scores computed on the tensor cores: tcgen05.mma kind::tf32, error-compensated
- * (3xTF32: hi.hi + lo.hi + hi.lo of operands split into two TF32 values), fp32 accumulators in TMEM read back with
- * tcgen05.ld by the selection code -- fp32-level scores (2^-22 relative per product), ~20x the SIMT kernel's rate.
+/* The same contract with the scores computed on the tensor cores: wgmma TF32, error-compensated
+ * (3xTF32: hi.hi + lo.hi + hi.lo of operands split into two TF32 values), fp32 accumulators in registers parked in
+ * shared memory for the selection code -- fp32-level scores (2^-22 relative per product).
  * d <= 64 and a multiple of 4; tables 16-byte aligned.  csrc/topn_tc.cu. */
 int qrec_score_topn_tc_f32(const float* dev_U, const float* dev_V, int32_t d, int32_t n_items,
                            const int32_t* dev_user_ids, int32_t n_rows, const int64_t* dev_rated_rowptr,
@@ -540,7 +540,7 @@ int qrec_mul_f32(float* dev_dst, const float* dev_a, const float* dev_b, int64_t
 
 /* =====================================================================================
  * K5 building block -- tensor-core GEMM for NeuMF's MLP (model/ranking/NeuMF.py:39-50):
- *   C[M,N] = epilogue(A[M,K] * B), fp32 storage, TF32 tcgen05.mma with fp32 accumulation in TMEM.
+ *   C[M,N] = epilogue(A[M,K] * B), fp32 storage, TF32 wgmma with fp32 accumulation in registers.
  * b_is_nk = 0: B is [K,N] row-major (a weight matrix, forward pass);
  * b_is_nk = 1: B is [N,K] row-major (dX = dY * W^T uses W as stored).
  * epilogue: 0 none | 1 relu(x + bias[n]) | 2 x * (mask[m,n] > 0) (ReLU backward) | 3 x + bias[n].
@@ -552,10 +552,9 @@ int qrec_tc_gemm_tf32(int32_t b_is_nk, int32_t M, int32_t N, int32_t K, const fl
                       int32_t ldmask, void* stream);
 /* The same product through a persistent, warp-specialised pipeline: one CTA per SM keeps a 64-column
  * block of B resident in shared memory, A arrives by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B tensor
- * map) through a 4-stage mbarrier ring, one thread issues tcgen05.mma into two alternating TMEM
- * accumulators, four epilogue warps drain them.  Same arguments and epilogues; K <= 320, N <= 64 x #SMs.
- * A is consumed as raw fp32 bits (TF32 truncation, error <= 2^-10 per operand; v1 rounds to nearest).
- * STATUS: written after round 1's GPU budget was spent; compiled, not yet run on hardware. */
+ * map) through a 4-stage mbarrier ring, two consumer warpgroups take the row tiles in turn (wgmma,
+ * accumulators in registers) and write their epilogues while the other multiplies.  Same arguments and epilogues; K <= 320, N <= 64 x #SMs.
+ * A is consumed as raw fp32 bits (TF32 truncation, error <= 2^-10 per operand; v1 rounds to nearest). */
 int qrec_tc_gemm_tf32_v2(int32_t b_is_nk, int32_t M, int32_t N, int32_t K, const float* dev_A,
                          int32_t lda, const float* dev_B, int32_t ldb, float* dev_C, int32_t ldc,
                          int32_t epilogue, const float* dev_bias, const float* dev_mask,
@@ -612,8 +611,6 @@ int qrec_mask_rated_f32(float* dev_scores, int32_t n_rows, int64_t ld, const int
  *                                                    and Bu[u] += lr*(e-regB*Bu[u]), Bi[i] likewise
  * e = r - prediction; the item row is updated from the NEW user row (`p` is a view in the reference).
  * dev_loss: double[1], accumulates sum e^2.  Bias pointers may be null unless kind == 2.
- * STATUS: written in round 1 after the GPU budget was spent -- compiled for sm_100a and covered by
- * the oracle, not yet run on hardware (tests gated by QREC_TEST_UNVALIDATED=1).
  * ===================================================================================== */
 /* wait_u[k] / wait_i[k] = number of earlier entries touching P[u[k]] / Q[i[k]] (host, O(n)). */
 int qrec_mf_order_prepare(int64_t n, const int32_t* u, const int32_t* i, int32_t num_users,

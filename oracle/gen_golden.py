@@ -23,7 +23,7 @@ What is exercised (reference file:line):
 modules because the reference imports them at module level (model/ranking/BPR.py:7,
 QRec.py:6).  The numpy path never calls into either.
 
-Usage:  python oracle/gen_golden.py [bpr] [mf] [sbpr]   (default: all sections; writes tests/golden/*.npz)
+Usage:  python oracle/gen_golden.py [bpr] [mf] [sbpr] [reference]   (default: all sections; writes tests/golden/)
 """
 import os
 import sys
@@ -389,9 +389,49 @@ def gen_sbpr():
     print('sbpr: %d relations, %d users with social feedback, 8 batches of 512' % (len(relation), int((fp_sizes > 0).sum())))
 
 
+def gen_reference():
+    """tests/reference_cases.py run against the unmodified reference modules: the SHA-256 of each case's canonical
+    result (tests/golden/reference_digests.json), and FilmTrust's ratings.txt, gzipped, as the loader cases' input."""
+    import gzip
+    import importlib
+    import json
+    import shutil
+    with open(os.path.join(REF, 'dataset', 'FilmTrust', 'ratings.txt'), 'rb') as src, \
+            gzip.GzipFile(os.path.join(OUT, 'filmtrust_ratings.txt.gz'), 'wb', mtime=0) as dst:
+        shutil.copyfileobj(src, dst)
+    sys.path.insert(0, os.path.join(REPO, 'tests'))
+    import reference_cases as RC
+    names = ('util.config', 'util.measure', 'util.qmath', 'util.io', 'util.dataSplit', 'data.rating', 'util.log',
+             'base.recommender', 'base.iterativeRecommender', 'base.deepRecommender')
+    mods = {n: importlib.import_module(n) for n in names}
+    out = {}
+    for name, case in sorted(RC.CASES.items()):
+        work = tempfile.mkdtemp(prefix='qrec_ref_case_')
+        out[name] = RC.digest(case(mods, work))
+    # the SBPR class's social-feedback sets and sampler, on the data of tests/test_sbpr_cpu.py
+    sys.path.insert(0, REPO)
+    import test_sbpr_cpu as TS
+    R = importlib.import_module('model.ranking.SBPR').SBPR
+    golden_bpr = np.load(os.path.join(OUT, 'bpr_filmtrust_seed0.npz'))
+    out['sbpr_sampler'] = RC.digest(TS.reference_sampler_view(R, mods['util.config'].ModelConf, golden_bpr,
+                                                               tempfile.mkdtemp(prefix='qrec_ref_case_')))
+    # the TBPR class under string-hash seed 0 (its joint item set is iterated in set order), in a fresh interpreter
+    import test_tbpr_cpu as TT
+    TT.run_with_hash_seed_0('T.reference_result(__import__("importlib").import_module("model.ranking.TBPR").TBPR, '
+                            '__import__("importlib").import_module("util.config").ModelConf, golden_bpr, workdir)',
+                            TT.GOLDEN_TBPR,
+                            prelude='import types\nsys.modules["tensorflow"] = types.ModuleType("tensorflow")\n'
+                                    'sys.modules["mkl"] = types.ModuleType("mkl")\nsys.path.append(%r)\n' % REF)
+    with open(RC.DIGESTS, 'w') as f:
+        json.dump(out, f, indent=1, sort_keys=True)
+        f.write('\n')
+
+
 def main():
-    what = set(sys.argv[1:]) or {'bpr', 'mf', 'sbpr'}
+    what = set(sys.argv[1:]) or {'bpr', 'mf', 'sbpr', 'reference'}
     _enter_workdir()
+    if 'reference' in what:
+        gen_reference()
     if 'bpr' in what:
         gen_bpr()
     if 'mf' in what:

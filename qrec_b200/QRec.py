@@ -17,7 +17,7 @@ def _model_class(name):
         try:
             mod = importlib.import_module('qrec_b200.model.ranking.' + name)
         except ImportError as e:
-            print('model %s is not available on the B200 engine (%s)' % (name, e))
+            print('model %s is not available on the H100 engine (%s)' % (name, e))
             sys.exit(-1)
     return getattr(mod, name)
 

@@ -1,1 +1,1 @@
-"""qrec_b200: B200-native engine behind QRec's BPR / LightGCN / NeuMF hot path (see DESIGN.md)."""
+"""qrec_b200: H100-native engine behind QRec's BPR / LightGCN / NeuMF hot path (see README.md)."""

@@ -36,10 +36,9 @@ class DeviceCSR(object):
 
     def set_split_row(self, row):
         """The joint adjacency of a bipartite graph is two very different halves: `row` = num_users short user rows that
-        gather item rows (a table that lives in the L2) and long item rows that gather user rows.  One launch over all of
-        them measured 2.03-2.11 ms on the 1M x 100K x 50M-edge benchmark graph, the two halves launched one after the
-        other 0.78 + 0.92 ms (profiles/r2/s2/bench_spmm_blocks.jsonl): lane groups working on 50-entry and on 500-entry
-        rows at the same time keep neither table's rows in the L2.  With a split row `matmul` issues the row-split
+        gather item rows (a table that lives in the L2) and long item rows that gather user rows.  Lane groups working on
+        50-entry and on 500-entry rows at the same time keep neither table's rows in the L2, so the halves are launched one
+        after the other.  With a split row `matmul` issues the row-split
         kernel once per half; rows, arithmetic and results are those of the single launch."""
         import os
         n = self.shape[0]

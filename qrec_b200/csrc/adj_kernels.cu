@@ -156,7 +156,7 @@ scan_add_kernel(long long* __restrict__ x, long long n, const long long* __restr
 }
 
 int grid_rows(long long n_rows) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long blocks = (n_rows + 7) / 8;

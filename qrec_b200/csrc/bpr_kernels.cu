@@ -426,11 +426,13 @@ __device__ __forceinline__ float group_sum_masked(float v, unsigned gmask) {
   return v;
 }
 
-// Work is cut into chunks of CH consecutive triples of the CSR order (balanced for any degree
-// distribution, like the nnz-balanced SpMM); a lane group finds the user of its first triple with an
-// LPR-ary search of rowptr and walks forward, flushing the P[u] delta (one row RED) whenever the user
-// changes or the chunk ends.  Inside a user P[u] is register-resident and updated sequentially; a
-// user whose triples span several chunks gets the sum of the chunks' deltas.
+// Work is cut into chunks of CH consecutive triples of the CSR order; a chunk takes the users whose first
+// triple lies inside it, so every user is processed whole by one lane group (P[u] register-resident,
+// updated sequentially, one row RED at the end) -- except at the ends of the launch, which are cut
+// where the caller cut them.  The chunks run in waves (ch_begin..ch_end);
+// inside a wave the item rows are READ from Qr, the table as it was when the wave started, and
+// scatter-added into Q.  Nothing a triple reads depends on timing: the result is the same every run up
+// to the summation order of the float REDs, and an item row is read at most about one wave late.
 // SAMPLE: the negatives are drawn inside the kernel (lane l draws the negative of triple base+l with
 // the same Philox counter as the stand-alone sampler, so both give identical j) instead of being
 // read from j[]; they are optionally written to j_out.
@@ -445,8 +447,8 @@ struct FusedSampler {
 // SIG: the sampler pre-tests every draw against the user's 512-bit rated signature (philox.cuh).
 template <int LPR, int G, int CH, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>   // FULL: d == 4*LPR (every lane owns a slice)
 __global__ void __launch_bounds__(256, MINB)
-bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec, int n_users,
-                         long long n, const long long* __restrict__ rowptr,
+bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, int n_users,
+                         long long n, long long ch_begin, long long ch_end, const long long* __restrict__ rowptr,
                          const int* __restrict__ i, const int* __restrict__ j, float lr,
                          float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
                          const uint32_t* __restrict__ rated_sig) {
@@ -462,19 +464,16 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec,
   const bool act = FULL ? true : (l < nvec);
   const float a_u = lr * reg_u, a_i = lr * reg_i;
   const float one_m_au = 1.0f - a_u, one_m_ai = 1.0f - a_i;
-  const long long nchunks = (n + CH - 1) / CH;
   float lsum = 0.f;
-  for (long long ch = group; ch < nchunks; ch += ngroups) {
-    const long long lo = ch * CH;
-    const long long hi = (lo + CH) < n ? (lo + CH) : n;
-    // user of triple lo: smallest r with rowptr[r+1] > lo
+  // user of triple t: smallest r with rowptr[r+1] > t (LPR-ary search by the lane group)
+  auto user_of = [&](long long t) {
     int a = 0, b = n_users - 1;
     while (a < b) {
       const int len = b - a + 1;
       const int step = (len + LPR - 1) / LPR;
       int pp = a + (l + 1) * step - 1;
       if (pp > b) pp = b;
-      const bool pred = (__ldg(rowptr + pp + 1) - trip_off) > lo;
+      const bool pred = (__ldg(rowptr + pp + 1) - trip_off) > t;
       const unsigned bal = (__ballot_sync(gmask, pred) & gmask) >> (sub * LPR);
       const int f = __ffs(bal) - 1;
       int pf = a + (f + 1) * step - 1;
@@ -482,7 +481,26 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec,
       a = a + f * step;
       b = pf;
     }
-    int uu = a;
+    return a;
+  };
+  for (long long ch = ch_begin + group; ch < ch_end; ch += ngroups) {
+    // the users whose first triple lies in [ch * CH, ch * CH + CH): a user cut by the chunk edge belongs to the
+    // chunk it starts in (the launch's own ends stay where they are)
+    long long lo = ch * CH;
+    long long hi = (lo + CH) < n ? (lo + CH) : n;
+    int uu = user_of(lo);
+    if (lo > 0 && __ldg(rowptr + uu) - trip_off < lo) {
+      lo = __ldg(rowptr + uu + 1) - trip_off;
+      ++uu;
+    }
+    if (hi < n) {
+      const int ub = user_of(hi);
+      if (__ldg(rowptr + ub) - trip_off < hi) {
+        const long long e = __ldg(rowptr + ub + 1) - trip_off;
+        hi = e < n ? e : n;
+      }
+    }
+    if (lo >= hi) continue;
     long long uend = __ldg(rowptr + uu + 1) - trip_off;
     float* prow = P + (size_t)uu * d + l * 4;
     float4 p = act ? *reinterpret_cast<const float4*>(prow) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -520,8 +538,8 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec,
           ri[f] = __shfl_sync(gmask, mi, sub * LPR + ((t0 + f) & (LPR - 1)));
           rj[f] = __shfl_sync(gmask, mj, sub * LPR + ((t0 + f) & (LPR - 1)));
           if (t0 + f < m && act) {
-            qi[f] = *reinterpret_cast<const float4*>(Q + (size_t)ri[f] * d + l * 4);
-            qj[f] = *reinterpret_cast<const float4*>(Q + (size_t)rj[f] * d + l * 4);
+            qi[f] = __ldg(reinterpret_cast<const float4*>(Qr + (size_t)ri[f] * d + l * 4));
+            qj[f] = __ldg(reinterpret_cast<const float4*>(Qr + (size_t)rj[f] * d + l * 4));
           } else {
             qi[f] = qj[f] = make_float4(0.f, 0.f, 0.f, 0.f);
           }
@@ -615,10 +633,10 @@ sumsq_kernel(const T* __restrict__ x, long long n, double* out) {
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     cached[dev] = v;
   }
   return cached[dev];
@@ -725,7 +743,7 @@ int qrec_bpr_sgd_batch_tma_f32(float* P, float* Q, int32_t d, int64_t n, const i
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && j, "qrec_bpr_sgd_batch_tma_f32: null index pointer");
   constexpr int UN = 4;
-  // which rows use the bulk engine: P only by default (the measured optimum, DESIGN.md section 4);
+  // which rows use the bulk engine: P only by default (fewest bytes through the copy engine);
   // QREC_K1_TMA_MASK=7 sends all three rows through it, 6 the two item rows
   static int mask = -1;
   if (mask < 0) {
@@ -767,12 +785,10 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
   FusedSampler fs = {reinterpret_cast<const long long*>(rated_rowptr), rated_cols, num_items, (uint32_t)seed,
                      (uint32_t)(seed >> 32), epoch, j_out};
   const int nvec = d / 4;
-  // Grid = exactly the CTAs that are resident at once (occupancy API per instantiation), so that the launch is ONE
-  // sweep over the user-major stream: at any moment the lane groups work on a contiguous window of chunks
-  // (chunk = group + k * ngroups).  A larger grid makes later CTAs start again at the beginning of the stream --
-  // several interleaved sweeps, i.e. a much larger re-ordering against the reference loop (measured at config 2:
-  // P / Q error relative to the epoch's update 14.7 % / 37.6 % with 8 CTAs per SM vs a few % with one sweep;
-  // bench.py parity_check).  QREC_K1_UM_CAP=<CTAs per SM> overrides (experiment switch).
+  // Grid = exactly the CTAs that are resident at once (occupancy API per instantiation); the stream is swept in
+  // waves, each reading the item table as the previous waves left it (a snapshot copied on the stream).
+  // QREC_K1_UM_CAP=<CTAs per SM> overrides
+  // (experiment switch).
   static int cap_mult = -1;
   if (cap_mult < 0) {
     const char* e = getenv("QREC_K1_UM_CAP");
@@ -780,9 +796,8 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
     if (cap_mult < 0) cap_mult = 0;
   }
   constexpr int CH = 32;
-  // experiment switch (d = 64 only), measured on 50 M triples: 0 = 3 CTAs/SM, 4 triples in flight
-  // (default, 5.80 ms); 1 = 4 CTAs/SM at 64 registers (spills, 7.08 ms); 2 = 2 CTAs/SM, 8 triples in
-  // flight (5.75 ms) -- occupancy and load depth are not the limiter any more
+  // experiment switch (d = 64 only): 0 = 3 CTAs/SM, 4 triples in flight (default); 1 = 4 CTAs/SM at 64
+  // registers (spills); 2 = 2 CTAs/SM, 8 triples in flight
   static int variant = -1;
   if (variant < 0) {
     const char* e = getenv("QREC_K1_UM_VARIANT");
@@ -795,14 +810,20 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
     else if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, KERNEL, 256, 0) != cudaSuccess || occ < 1) occ = 3; \
     const long long cap = (long long)sm_count() * occ;                                           \
     if (blocks > cap) blocks = cap;                                                              \
-    KERNEL<<<(int)blocks, 256, 0, st>>>(P, Q, nvec, n_users, n, reinterpret_cast<const long long*>(rowptr), i, j, lr, \
-                                        reg_u, reg_i, loss, fs, trip_off, SIGPTR);               \
+    for (long long c0 = 0; c0 < nchunks; c0 += wave) {                                           \
+      QREC_CUDA(cudaMemcpyAsync(Qr, Q, q_bytes, cudaMemcpyDeviceToDevice, st));                  \
+      const long long c1 = (c0 + wave) < nchunks ? (c0 + wave) : nchunks;                        \
+      KERNEL<<<(int)blocks, 256, 0, st>>>(P, Q, Qr, nvec, n_users, n, c0, c1, reinterpret_cast<const long long*>(rowptr), \
+                                          i, j, lr, reg_u, reg_i, loss, fs, trip_off, SIGPTR);   \
+      QREC_CUDA(cudaGetLastError());                                                             \
+      if (c1 < nchunks) qrec::count_launch();                                                    \
+    }                                                                                            \
   }
 #define QREC_UM2(LPR, FULLV, SAMPLEV) QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<LPR, 4, CH, FULLV, SAMPLEV>), nullptr)
 #define QREC_UM(LPR)                                                                             \
   {                                                                                              \
     const long long per_block = 8 * (32 / LPR);                                                  \
-    long long blocks = ((n + CH - 1) / CH + per_block - 1) / per_block;                          \
+    long long blocks = (nchunks + per_block - 1) / per_block;                                    \
     if (nvec == LPR && sample && rated_sig != nullptr) {                                         \
       QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<LPR, 4, CH, true, true, 3, true>), rated_sig)     \
     } else if (nvec == LPR && LPR == 16 && variant == 1) {                                       \
@@ -815,13 +836,33 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
     if (nvec == LPR) { if (sample) QREC_UM2(LPR, true, true) else QREC_UM2(LPR, true, false) }   \
     else { if (sample) QREC_UM2(LPR, false, true) else QREC_UM2(LPR, false, false) }             \
   }
-  if (nvec <= 4) QREC_UM(4)
-  else if (nvec <= 8) QREC_UM(8)
-  else if (nvec <= 16) QREC_UM(16)
-  else QREC_UM(32)
+  if (n <= 0) return QREC_OK;
+  QREC_REQUIRE(num_items >= 1, "qrec user-major epoch: num_items=%d (the item table's rows) must be given", num_items);
+  const long long nchunks = (n + CH - 1) / CH;
+  const size_t q_bytes = (size_t)num_items * d * sizeof(float);
+  // Wave size in triples: no more than 4 x the item rows, so an item row is read only a few of its own updates late.
+  // On a small table (snapshot copy under 8 MB, about the cost of a launch) at least 64 waves per launch: on a small
+  // data set the hot items recur within a few hundred triples.  On a large one the wave is long enough that the
+  // copy stays under 1/8 of the wave's algorithmic bytes (24 d + 12 per triple).
+  const long long copy_bytes = 2 * (long long)q_bytes;
+  const long long copy_floor = copy_bytes > (8LL << 20) ? 8 * copy_bytes / (24LL * d + 12) : 0;
+  long long wave_triples = n / 64 > copy_floor ? n / 64 : copy_floor;
+  if (wave_triples > 4LL * num_items) wave_triples = 4LL * num_items;
+  const long long wave = wave_triples / CH > 1 ? wave_triples / CH : 1;      // in chunks
+  float* Qr = nullptr;                                // the item table as the current wave started (stream-ordered scratch)
+  QREC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&Qr), q_bytes, st));
+  const int rc = [&]() -> int {
+    if (nvec <= 4) QREC_UM(4)
+    else if (nvec <= 8) QREC_UM(8)
+    else if (nvec <= 16) QREC_UM(16)
+    else QREC_UM(32)
+    return QREC_OK;
+  }();
 #undef QREC_UM
 #undef QREC_UM2
 #undef QREC_UM_LAUNCH
+  QREC_CUDA(cudaFreeAsync(Qr, st));
+  if (rc != QREC_OK) return rc;
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -829,15 +870,15 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
 
 extern "C" {
 
-int qrec_bpr_sgd_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
-                               const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i,
+int qrec_bpr_sgd_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, int32_t num_items,
+                               const int64_t* rowptr, const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i,
                                double* loss, void* stream) {
   QREC_REQUIRE(P && Q && loss, "qrec_bpr_sgd_usermajor_f32: null pointer");
   QREC_REQUIRE(d >= 4 && d <= 128 && (d % 4) == 0, "qrec_bpr_sgd_usermajor_f32: d=%d unsupported (multiple of 4, 4..128)", d);
   QREC_REQUIRE(n_users >= 0 && n >= 0, "qrec_bpr_sgd_usermajor_f32: negative size");
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && j, "qrec_bpr_sgd_usermajor_f32: null index pointer");
-  return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, j, lr, reg_u, reg_i, loss, false, nullptr, nullptr, 0,
+  return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, j, lr, reg_u, reg_i, loss, false, nullptr, nullptr, num_items,
                                 0, 0, nullptr, 0, (cudaStream_t)stream, nullptr);
 }
 

@@ -220,7 +220,7 @@ extern "C" int qrec_bpr_epoch_usermajor_tma_f32(float* P, float* Q, int32_t d, i
     QREC_CUDA(cudaFuncSetAttribute(bpr_sgd_usermajor_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long blocks = ((n + CH - 1) / CH + GROUPS - 1) / GROUPS;

@@ -22,6 +22,6 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 extern "C" {
 const char* qrec_last_error(void) { return g_err; }
-const char* qrec_version(void) { return "qrec-b200 0.1.0 sm_100a"; }
+const char* qrec_version(void) { return "qrec-b200 0.1.0 sm_90a"; }
 int64_t qrec_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 }

@@ -23,8 +23,8 @@ __device__ __forceinline__ float sgn(float x) { return (x > 0.f) ? 1.f : ((x < 0
 
 int sm_count() {
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
   return v;
 }
 

@@ -44,8 +44,8 @@ __device__ __forceinline__ void fma4(float4& acc, float s, float4 x) {
 
 int sm_count() {
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
   return v;
 }
 
@@ -582,8 +582,7 @@ int qrec_spmm_csr_rowsplit_f32(int32_t n_rows, int64_t nnz, const int64_t* rowpt
   QREC_REQUIRE(rowptr && X && Y, "qrec_spmm_csr_rowsplit_f32: null pointer");
   QREC_REQUIRE(aligned16(X) && aligned16(Y) && aligned16(acc), "qrec_spmm_csr_rowsplit_f32: tables must be 16-byte aligned");
   QREC_REQUIRE(X != Y, "qrec_spmm_csr_rowsplit_f32: X and Y must not alias");
-  // d = 64: the width-specialised instantiation at 4 CTAs/SM (spmm_variants.cu, variant 0) -- bit-identical results,
-  // 2.15 ms instead of 2.49 ms on the 100 M-nnz benchmark graph (profiles/README.md, round 2)
+  // d = 64: the width-specialised instantiation at 4 CTAs/SM (spmm_variants.cu, variant 0) -- bit-identical results
   if (d == 64 && X != nullptr && Y != nullptr) {
     static int var = -1;                                  // QREC_SPMM_VARIANT: experiment switch (spmm_variants.cu)
     if (var < 0) {

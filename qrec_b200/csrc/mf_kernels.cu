@@ -245,8 +245,8 @@ mf_predict_pairs_kernel(const T* __restrict__ P, const T* __restrict__ Q, int d,
 
 int sm_count() {
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
   return v;
 }
 

@@ -62,7 +62,7 @@ extern "C" int qrec_ubench_row_ops_f32(float* dev_table, int64_t rows, int64_t n
   QREC_REQUIRE(rows > 0 && rows < (1LL << 32) && n_ops >= 0, "ubench_row_ops: bad sizes");
   QREC_REQUIRE(mode >= 0 && mode <= 2, "ubench_row_ops: mode must be 0 (gather), 1 (reduce) or 2 (both)");
   if (n_ops == 0) return QREC_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = sms * 8;                       // 8 CTAs of 256 threads per SM: full occupancy at <= 32 registers

@@ -31,7 +31,7 @@ extern "C" int qrec_sample_neg_philox(int64_t n, int32_t num_items, const int32_
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && rowptr && cols && out_j, "qrec_sample_neg_philox: null pointer");
   const long long blocks = (n + 255) / 256;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   sample_neg_philox_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(
       n, num_items, u, reinterpret_cast<const long long*>(rowptr), cols, (uint32_t)seed,
       (uint32_t)(seed >> 32), epoch, out_j);

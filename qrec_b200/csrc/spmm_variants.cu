@@ -1,7 +1,5 @@
 // K2 experiments (d = 64, row-split): the production kernel is spmm_csr_kernel<16,1> in
-// graph_kernels.cu -- 8 gathered rows in flight per lane group, issued and consumed in lock step, 61
-// registers, 44 % of the warps resident, 64 % of the stall samples on the first FMA after a batch of
-// gathers (profiles/README.md).  The variants here change only HOW MANY loads are outstanding and how
+// graph_kernels.cu -- 8 gathered rows in flight per lane group, issued and consumed in lock step.  The variants here change only HOW MANY loads are outstanding and how
 // many warps are resident, never the order of the floating-point operations, so every variant must
 // reproduce the production kernel bit for bit:
 //   0  G=8,  4 CTAs/SM   the production configuration (A/B control)
@@ -12,8 +10,7 @@
 //                                   current group is consumed (8 in flight continuously)
 //   5  G=8 x 2 buffers, 2 CTAs/SM   the same with 16 in flight
 //   6  variant 0 + L2 residency hints: (col, val) streamed (L2::evict_first, no L1 allocation), X rows evict_last
-// STATUS: written after round 1's GPU budget was spent -- compiled, not yet run on hardware; reached
-// only through qrec_spmm_csr_rowsplit_var_f32 (tests/test_gpu_spmm_variants.py, tools/bench_graph.py).
+// Reached only through qrec_spmm_csr_rowsplit_var_f32 (tests/test_gpu_spmm_variants.py, tools/bench_graph.py).
 #include "common.h"
 
 namespace {
@@ -200,8 +197,8 @@ spmm_rowsplit_pipe_kernel(int n_rows, const long long* __restrict__ rowptr, cons
 
 int sm_count() {
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
   return v;
 }
 

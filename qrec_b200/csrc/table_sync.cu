@@ -102,7 +102,7 @@ table_all_gather_kernel(PeerPtrs peers_S, int world, long long slice4, float4* _
 }
 
 int grid_for(long long n4) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long blocks = (n4 + 127) / 128;

@@ -1,19 +1,20 @@
 // K5 building block: the tensor-core GEMM of NeuMF's MLP (model/ranking/NeuMF.py:39-50),
-//     C[M,N] = epilogue( A[M,K] * B )          fp32 in HBM, TF32 tcgen05.mma, fp32 accumulate in TMEM
-// written directly against the sm_100a tensor-core path:
+//     C[M,N] = epilogue( A[M,K] * B )          fp32 in HBM, TF32 wgmma, fp32 accumulate in registers
+// written directly against the sm_90a tensor-core path:
 //   * operands are staged in shared memory in the canonical K-major SWIZZLE_128B layout
 //     (rows of 32 fp32 = 128 B, 8-row 1024 B atoms, 16-byte chunk index XOR row%8) -- the MLP's
 //     weight matrices are [K,N] row-major, so they are transposed on the way into shared memory;
-//   * one elected thread issues tcgen05.mma.cta_group::1.kind::tf32 (M=128, N=64, K=8 per
-//     instruction, 4 per 128-byte stage) with the 64-bit shared-memory matrix descriptors and the
-//     32-bit instruction descriptor built below; accumulators live in 64 TMEM columns;
-//   * stages are recycled through mbarriers signalled by tcgen05.commit (2-stage ring), the
-//     epilogue reads the accumulator with tcgen05.ld.32x32b.x16 (warp w owns TMEM lanes 32w..32w+31),
-//     applies bias / ReLU / ReLU-mask and writes fp32 rows.
+//   * the CTA is one warpgroup: per 8-wide k-step it issues two wgmma.mma_async m64n64k8 TF32
+//     (rows 0-63 and 64-127 of the tile) from shared-memory descriptors (csrc/wgmma.cuh); the
+//     128 x 64 fp32 accumulator lives in registers (64 per thread);
+//   * 2-stage ring: the MMAs of k-block kb run while the stores of k-block kb+1 wait only for the
+//     group of kb-1 (wgmma.wait_group 1 + a CTA barrier before a stage is rewritten);
 //   * global loads are register-staged one k-block ahead (their latency overlaps the MMAs), the
-//     epilogue is parked in shared memory and written as whole 256-byte rows.
+//     epilogue is parked in shared memory and written as whole 256-byte rows with bias / ReLU /
+//     ReLU-mask applied.
 // Tile: 128 x 64 per CTA, 128 threads.
 #include "common.h"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -21,53 +22,13 @@ constexpr int BM = 128, BN = 64, BK = 32;           // BK fp32 = 128 B = one swi
 constexpr int STAGE_A = BM * 128, STAGE_B = BN * 128;
 constexpr int SMEM_BYTES = 2 * (STAGE_A + STAGE_B) + 1024;   // + alignment slack
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-
-// K-major SWIZZLE_128B descriptor: start>>4 | LBO=0 | SBO=1024>>4 | version 1 | layout SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);           // bits 0-13  start address
-  d |= (uint64_t)0 << 16;                            // bits 16-29 leading byte offset (unused, K-major swizzled)
-  d |= (uint64_t)(1024 >> 4) << 32;                  // bits 32-45 stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                            // bits 46-47 descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                            // bits 61-63 layout type: SWIZZLE_128B
-  return d;
-}
-
-// instruction descriptor, kind::tf32: D=F32, A=B=TF32, both K-major, N=64, M=128
-__device__ __forceinline__ uint32_t make_idesc() {
-  uint32_t i = 0;
-  i |= 1u << 4;                 // D format F32
-  i |= 2u << 7;                 // A format TF32
-  i |= 2u << 10;                // B format TF32
-  i |= (uint32_t)(BN >> 3) << 17;
-  i |= (uint32_t)(BM >> 4) << 24;
-  return i;
-}
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-
 // byte offset of element (row, k) inside a K-major SWIZZLE_128B tile (k in [0,32) fp32)
 __device__ __forceinline__ uint32_t sw_off(int row, int k) {
   const int chunk = (k >> 2) ^ (row & 7);
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + chunk * 16 + (k & 3) * 4);
 }
 
-// tcgen05 kind::tf32 reads the top 19 bits of each fp32 operand, i.e. truncates.  Rounding to
+// The tensor cores read the top 19 bits of each fp32 operand, i.e. truncate.  Rounding to
 // nearest-away while staging removes the systematic toward-zero bias (2^-11 unbiased instead of up
 // to 2^-10 one-sided per operand), which matters over the 6-GEMM forward/backward chain of the MLP.
 __device__ __forceinline__ float to_tf32(float x) {
@@ -81,7 +42,6 @@ __device__ __forceinline__ float4 to_tf32(float4 v) {
 
 enum Epilogue { EPI_NONE = 0, EPI_BIAS_RELU = 1, EPI_RELU_MASK = 2, EPI_BIAS = 3 };
 
-// B_IS_NK: B is stored [N,K] row-major (already K-major); otherwise [K,N] row-major.
 template <bool B_IS_NK>
 __global__ void __launch_bounds__(128)
 tc_gemm_tf32_kernel(int M, int N, int K, const float* __restrict__ A, int lda,
@@ -89,28 +49,16 @@ tc_gemm_tf32_kernel(int M, int N, int K, const float* __restrict__ A, int lda,
                     int epi, const float* __restrict__ bias, const float* __restrict__ mask,
                     int ldmask) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t mma_done[2];
-  __shared__ uint32_t tmem_base_slot;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   // stage s: A tile at smem + s*(STAGE_A+STAGE_B), B tile right behind it (computed, not looked up:
   // a pointer array indexed by the stage lands in local memory)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-
-  if (tid == 0) {
-    mbar_init(&mma_done[0], 1);
-    mbar_init(&mma_done[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "n"(BN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_acc = tmem_base_slot;
-  const uint32_t idesc = make_idesc();
+  float acc[2][32];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int e = 0; e < 32; ++e) acc[h][e] = 0.f;
 
   const int nkb = (K + BK - 1) / BK;
   // Register-staged global loads, one k-block ahead: the loads of block kb+1 are issued before the
@@ -149,7 +97,7 @@ tc_gemm_tf32_kernel(int M, int N, int K, const float* __restrict__ A, int lda,
     const int s = kb & 1;
     uint8_t* const sA_s = smem + s * (STAGE_A + STAGE_B);
     uint8_t* const sB_s = sA_s + STAGE_A;
-    if (kb >= 2) mbar_wait(&mma_done[s], (uint32_t)(((kb >> 1) - 1) & 1));   // MMAs that read stage s are done
+    if (kb >= 2) __syncthreads();          // every warp has retired the MMAs of kb-2 (wait_group 1 below): stage s is free
 #pragma unroll
     for (int p = 0; p < 8; ++p) {
       const int row = (tid >> 3) + 16 * p, c = tid & 7;
@@ -169,55 +117,30 @@ tc_gemm_tf32_kernel(int M, int N, int K, const float* __restrict__ A, int lda,
       }
     }
     if (kb + 1 < nkb) load_block(kb + 1);                                        // in flight during the MMAs
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> async proxy (UMMA)
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> async proxy (wgmma)
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint64_t da = make_desc(smem_u32(sA_s)), db = make_desc(smem_u32(sB_s));
+    wg::fence();
+    const uint64_t da = wg::desc_sw128(wg::smem_u32(sA_s)), db = wg::desc_sw128(wg::smem_u32(sB_s));
 #pragma unroll
-      for (int k4 = 0; k4 < BK / 8; ++k4) {
-        const uint32_t acc = (kb > 0 || k4 > 0) ? 1u : 0u;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_acc),
-            "l"(da + (uint64_t)(k4 * 2)), "l"(db + (uint64_t)(k4 * 2)), "r"(idesc), "r"(acc)
-            : "memory");                                              // +2 = 32 bytes (8 tf32) along K
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mma_done[s]))
-                   : "memory");
+    for (int k4 = 0; k4 < BK / 8; ++k4) {                              // +2 = 32 bytes (8 tf32) along K
+      wg::mma_m64n64k8_tf32(acc[0], da + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), 1u);
+      wg::mma_m64n64k8_tf32(acc[1], da + (uint64_t)(STAGE_A / 2 >> 4) + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), 1u);
     }
+    wg::commit();
+    wg::wait<1>();
   }
-  // the last commit covers every earlier MMA (they retire in issue order)
-  {
-    const int last = nkb - 1;
-    mbar_wait(&mma_done[last & 1], (uint32_t)((last >> 1) & 1));
-  }
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  // ---- epilogue: TMEM -> registers -> shared memory (the operand stages are free now) -> coalesced
-  // global rows.  Warp w reads TMEM lanes [32w, 32w+32) (one accumulator row per thread) and parks
-  // them in a [128][64+4] fp32 tile (row pitch 272 B: conflict-free 16-byte stores); then every warp
-  // writes whole 256-byte rows.
+  wg::wait<0>();
+  __syncthreads();                                  // every warp's MMAs are done: the operand stages are free
+  // ---- epilogue: registers -> shared memory -> coalesced global rows.  The accumulator is parked in a
+  // [128][64+4] fp32 tile (row pitch 272 B); then every warp writes whole 256-byte rows.
   float* tile = reinterpret_cast<float*>(smem);
   constexpr int PITCH = BN + 4;
-  {
-    const int r_in_tile = warp * 32 + lane;
 #pragma unroll
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      uint32_t r[16];
-      const uint32_t taddr = tmem_acc + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-            "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int q = 0; q < 16; q += 4)
-        *reinterpret_cast<uint4*>(tile + r_in_tile * PITCH + c0 + q) = make_uint4(r[q], r[q + 1], r[q + 2], r[q + 3]);
-    }
-  }
+    for (int e = 0; e < 32; e += 2)
+      *reinterpret_cast<float2*>(tile + (64 * h + wg::frag_row(warp, lane, e)) * PITCH + wg::frag_col(lane, e)) =
+          make_float2(acc[h][e], acc[h][e + 1]);
   __syncthreads();
   {
     const int c4 = (tid & 15) * 4;                 // 16 threads cover one 64-float row
@@ -255,11 +178,6 @@ tc_gemm_tf32_kernel(int M, int N, int K, const float* __restrict__ A, int lda,
         if (col + 3 < N) dst[3] = v.w;
       }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(BN));
   }
 }
 

@@ -1,26 +1,25 @@
 // K5 v2: the same product as tc_gemm.cu,
-//     C[M,N] = epilogue( A[M,K] * B )          fp32 in HBM, TF32 tcgen05.mma, fp32 accumulate in TMEM
+//     C[M,N] = epilogue( A[M,K] * B )          fp32 in HBM, TF32 wgmma, fp32 accumulate in registers
 // rebuilt as a persistent, warp-specialised pipeline (model/ranking/NeuMF.py:39-50 is still the caller):
 //   * one CTA per SM keeps ONE 64-column block of B resident in shared memory for its whole life
 //     (all K/32 k-blocks, transposed / rounded to TF32 once) and walks the 128-row tiles of A that
 //     belong to that column block;
-//   * warp 0 (one lane): TMA producer -- cp.async.bulk.tensor.2d loads 128 x 32 fp32 boxes of A through
-//     a SWIZZLE_128B tensor map straight into the K-major layout the MMA descriptors expect, NSTAGE-deep
+//   * warp 4 (one lane): TMA producer -- cp.async.bulk.tensor.2d loads 128 x 32 fp32 boxes of A through
+//     a SWIZZLE_128B tensor map straight into the K-major layout the wgmma descriptors expect, NSTAGE-deep
 //     ring, mbarrier complete_tx; out-of-range rows / columns are zero-filled by the copy engine;
-//   * warp 1 (one lane): MMA issuer -- waits for a stage, issues 4 x tcgen05.mma.kind::tf32
-//     (M=128, N=64, K=8), tcgen05.commit frees the stage; the accumulator alternates between two
-//     64-column TMEM buffers so tile t+1 is multiplied while tile t is drained;
-//   * warps 2-5: epilogue -- tcgen05.ld the finished buffer, hand it back (tmem_empty), apply
-//     bias / ReLU / ReLU-mask and write whole 256-byte rows through a per-warp shared-memory transpose.
-// A reaches the tensor cores as raw fp32 bits (kind::tf32 drops the low 13 mantissa bits: truncation,
+//   * warps 0-3 (one warpgroup) consume the ring in order: per stage two wgmma.mma_async m64n64k8 TF32 per
+//     8-wide k-step (csrc/wgmma.cuh), accumulator in registers; the stage goes back to the producer once the
+//     group has retired, so the copy engine runs ahead into the next tile while the epilogue applies
+//     bias / ReLU / ReLU-mask and writes whole 256-byte rows through a shared-memory tile.
+//     (The ring is consumed strictly in order: an mbarrier parity wait cannot tell a phase two ahead from
+//     the one before, so a second consumer taking every other tile could not wait on the same ring.)
+// A reaches the tensor cores as raw fp32 bits (the TF32 MMA drops the low 13 mantissa bits: truncation,
 // error <= 2^-10 per operand instead of 2^-11 with the cvt.rna staging of v1); B is rounded (rna) while
-// it is staged.  K <= 320 (B block + 4-stage ring + epilogue tiles = 179 KB of the 227 KB).
-//
-// STATUS: written after round 1's GPU budget was spent -- compiles for sm_100a, NOT yet run on
-// hardware; reached only through qrec_tc_gemm_tf32_v2 (nothing in the product calls it yet).
+// it is staged.  K <= 320 (B block + 4-stage ring + epilogue tile = 178 KB of the 227 KB).
 #include <cuda.h>
 
 #include "common.h"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -29,33 +28,11 @@ constexpr int NSTAGE = 4;
 constexpr int STAGE_A = BM * 128;                   // 16 KB per A stage
 constexpr int KB_B = BN * 128;                      // 8 KB per resident B k-block
 constexpr int MAX_K = 320;
-constexpr int EPI_PITCH = BN + 4;                   // floats; 272-byte rows: conflict-free 16-byte stores
-constexpr int EPI_WARP_BYTES = 32 * EPI_PITCH * 4;  // per epilogue warp
-constexpr int NTHREADS = 192;
+constexpr int EPI_PITCH = BN + 4;                   // floats; 272-byte rows
+constexpr int EPI_BYTES = BM * EPI_PITCH * 4;
+constexpr int NTHREADS = 160;                       // the consumer warpgroup + the producer warp
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-
-// K-major SWIZZLE_128B descriptor (same encoding as tc_gemm.cu, validated there)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(1024 >> 4) << 32;                  // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                            // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                            // SWIZZLE_128B
-  return d;
-}
-
-__device__ __forceinline__ uint32_t make_idesc() {  // kind::tf32, D=F32, A=B=TF32 K-major, N=64, M=128
-  uint32_t i = 0;
-  i |= 1u << 4;
-  i |= 2u << 7;
-  i |= 2u << 10;
-  i |= (uint32_t)(BN >> 3) << 17;
-  i |= (uint32_t)(BM >> 4) << 24;
-  return i;
-}
+using wg::smem_u32;
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -82,6 +59,9 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
+__device__ __forceinline__ void group_sync() {     // the 128 threads of the consumer warpgroup
+  asm volatile("bar.sync 1, 128;" ::: "memory");
+}
 
 __device__ __forceinline__ uint32_t sw_off(int row, int k) {   // (row, k) inside a K-major SWIZZLE_128B tile
   const int chunk = (k >> 2) ^ (row & 7);
@@ -104,13 +84,12 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
                        const float* __restrict__ bias, const float* __restrict__ mask, int ldmask,
                        int n_blocks, int ctas_per_n) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t full_bar[NSTAGE], empty_bar[NSTAGE], tmem_full[2], tmem_empty[2];
-  __shared__ uint32_t tmem_base_slot;
+  __shared__ uint64_t full_bar[NSTAGE], empty_bar[NSTAGE];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int nkb = (K + BK - 1) / BK;
   uint8_t* sA = smem;                                // NSTAGE x 16 KB
   uint8_t* sB = smem + NSTAGE * STAGE_A;             // nkb x 8 KB, resident
-  uint8_t* sE = sB + nkb * KB_B;                     // 4 x EPI_WARP_BYTES
+  uint8_t* sE = sB + nkb * KB_B;                     // EPI_BYTES
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nb = blockIdx.x % n_blocks, first_tile = blockIdx.x / n_blocks;
   const int n0 = nb * BN;
@@ -119,18 +98,10 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
   if (tid == 0) {
     for (int s = 0; s < NSTAGE; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);                   // one arrival per warp of the consuming warpgroup
     }
-    mbar_init(&tmem_full[0], 1);
-    mbar_init(&tmem_full[1], 1);
-    mbar_init(&tmem_empty[0], 4);                    // one arrival per epilogue warp
-    mbar_init(&tmem_empty[1], 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "n"(2 * BN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   // resident B block: every thread stages a share of the nkb k-blocks, rounded to TF32, K-major
   for (int kb = 0; kb < nkb; ++kb) {
@@ -153,13 +124,10 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
       }
     }
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy writes -> async proxy (UMMA)
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy writes -> async proxy (wgmma)
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_acc = tmem_base_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ===== TMA producer =====
     if (lane == 0) {
       int stage = 0;
@@ -173,47 +141,10 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc();
-      int stage = 0;
-      uint32_t phase = 0;
-      int t = 0;
-      for (int mt = first_tile; mt < m_tiles; mt += ctas_per_n, ++t) {
-        const int buf = t & 1;
-        const uint32_t use = (uint32_t)(t >> 1);                     // how often this buffer was used before
-        mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);                  // epilogue drained it (passes on first use)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc_addr = tmem_acc + (uint32_t)(buf * BN);
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);                         // the copy engine has landed this stage
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = make_desc(smem_u32(sA + stage * STAGE_A));
-          const uint64_t db = make_desc(smem_u32(sB + kb * KB_B));
-#pragma unroll
-          for (int k4 = 0; k4 < BK / 8; ++k4) {
-            const uint32_t acc = (kb > 0 || k4 > 0) ? 1u : 0u;
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t"
-                "setp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(acc_addr),
-                "l"(da + (uint64_t)(k4 * 2)), "l"(db + (uint64_t)(k4 * 2)), "r"(idesc), "r"(acc)
-                : "memory");                                          // +2 = 32 bytes (8 tf32) along K
-          }
-          asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&empty_bar[stage]))
-                       : "memory");                                   // stage reusable once these MMAs retire
-          if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&tmem_full[buf]))
-                     : "memory");                                     // accumulator complete
-      }
-    }
   } else {
-    // ===== epilogue warps 2..5: TMEM lane quarter (warp % 4) =====
-    const int q = warp & 3;
-    float* tile = reinterpret_cast<float*>(sE + (warp - 2) * EPI_WARP_BYTES);
-    const int c4 = (lane & 15) * 4;                  // 16 lanes cover one 64-float row on the way out
+    // ===== consumer warpgroup =====
+    float* tile = reinterpret_cast<float*>(sE);
+    const int c4 = (tid & 15) * 4;                   // 16 threads cover one 64-float row on the way out
     const int col = n0 + c4;
     float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
     if ((epi == EPI_BIAS_RELU || epi == EPI_BIAS) && col < N) {
@@ -223,34 +154,38 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
       if (col + 3 < N) bv.w = bias[col + 3];
     }
     const bool vec_ok = (col + 3 < N) && ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
-    int t = 0;
-    for (int mt = first_tile; mt < m_tiles; mt += ctas_per_n, ++t) {
-      const int buf = t & 1;
-      const uint32_t use = (uint32_t)(t >> 1);
-      mbar_wait(&tmem_full[buf], use & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int mt = first_tile; mt < m_tiles; mt += ctas_per_n) {
+      float acc[2][32];
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);                           // the copy engine has landed this stage
+        __syncwarp();                                                  // wgmma is warp-aligned: reconverge after the spin
+        wg::fence();
+        const uint64_t da = wg::desc_sw128(smem_u32(sA + stage * STAGE_A));
+        const uint64_t db = wg::desc_sw128(smem_u32(sB + kb * KB_B));
 #pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t r[16];
-        const uint32_t taddr = tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN + c0);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-              "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int x = 0; x < 16; x += 4)
-          *reinterpret_cast<uint4*>(tile + lane * EPI_PITCH + c0 + x) = make_uint4(r[x], r[x + 1], r[x + 2], r[x + 3]);
+        for (int k4 = 0; k4 < BK / 8; ++k4) {                          // +2 = 32 bytes (8 tf32) along K
+          const uint32_t accumulate = (kb > 0 || k4 > 0) ? 1u : 0u;
+          wg::mma_m64n64k8_tf32(acc[0], da + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), accumulate);
+          wg::mma_m64n64k8_tf32(acc[1], da + (uint64_t)(STAGE_A / 2 >> 4) + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), accumulate);
+        }
+        wg::commit();
+        wg::wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);                 // this warp's share of the stage is read
+        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
       }
-      // the buffer is in registers / shared memory now: hand it back before the global stores
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-      const int row_base = mt * BM + q * 32;
-      for (int rr = lane >> 4; rr < 32; rr += 2) {   // two rows per pass, 256 B each
-        const int row = row_base + rr;
+      group_sync();                                  // the previous tile's rows are out of the staging tile
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 32; e += 2)
+          *reinterpret_cast<float2*>(tile + (64 * h + wg::frag_row(warp, lane, e)) * EPI_PITCH + wg::frag_col(lane, e)) =
+              make_float2(acc[h][e], acc[h][e + 1]);
+      group_sync();
+      for (int rr = tid >> 4; rr < BM; rr += 8) {    // eight rows per pass, 256 B each
+        const int row = mt * BM + rr;
         if (row >= M || col >= N) continue;
         float4 v = *reinterpret_cast<const float4*>(tile + rr * EPI_PITCH + c4);
         if (epi == EPI_BIAS_RELU) {
@@ -274,14 +209,7 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
           if (col + 3 < N) dst[3] = v.w;
         }
       }
-      __syncwarp();                                  // the staging tile is rewritten by the next tile
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(2 * BN));
   }
 }
 
@@ -304,8 +232,8 @@ EncodeTiledFn encode_tiled() {
 
 int sm_count() {
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
   return v;
 }
 
@@ -345,7 +273,7 @@ extern "C" int qrec_tc_gemm_tf32_v2(int32_t b_is_nk, int32_t M, int32_t N, int32
   if (ctas_per_n > m_tiles) ctas_per_n = m_tiles;
   if (ctas_per_n < 1) ctas_per_n = 1;
   const int nkb = (K + BK - 1) / BK;
-  const int smem = NSTAGE * STAGE_A + nkb * KB_B + 4 * EPI_WARP_BYTES + 1024;
+  const int smem = NSTAGE * STAGE_A + nkb * KB_B + EPI_BYTES + 1024;
   if (b_is_nk) QREC_CUDA(cudaFuncSetAttribute(tc_gemm_tf32_v2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   else QREC_CUDA(cudaFuncSetAttribute(tc_gemm_tf32_v2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = n_blocks * ctas_per_n;

@@ -8,34 +8,37 @@
 //     128-item tile as one contiguous block already in the shared-memory layout; the main kernel streams those blocks
 //     through a 2-stage ring with cp.async.bulk (one 64 KB bulk copy per tile, completion on an mbarrier) -- no
 //     thread touches the item operands;
-//   * one thread issues tcgen05.mma.cta_group::1.kind::tf32 (M=128, N=128, K=8) three times per k-step --
-//     hi.hi + lo.hi + hi.lo, the classical 3xTF32 error-compensated product: the dropped lo.lo term is 2^-22
-//     relative, i.e. fp32-level scores, which is what keeps the index lists equal to an fp32 GEMV's wherever
-//     scores are distinct (plain TF32's 10-bit mantissa reorders close scores) -- into one of two 128-column TMEM
-//     accumulators;
-//   * while the tensor cores work on tile t, 256 threads read tile t-1's accumulator with tcgen05.ld -- two threads
-//     per user row (warps w and w+4 own TMEM lanes 32 (w%4)..; one takes columns 0-63 of the tile, the other 64-127),
-//     each with its OWN candidate list and cut-off (the N best overall are among the N best of the two halves; the
-//     lists are merged at the end) -- and run the selection of topn_kernels.cu with the count and cut-off in
+//   * two warpgroups each multiply 64 of the users against the tile with wgmma.mma_async m64n128k8 TF32
+//     (csrc/wgmma.cuh) three times per k-step -- hi.hi + lo.hi + hi.lo, the classical 3xTF32 error-compensated
+//     product: the dropped lo.lo term is 2^-22 relative, i.e. fp32-level scores, which is what keeps the index lists
+//     equal to an fp32 GEMV's wherever scores are distinct (plain TF32's 10-bit mantissa reorders close scores) --
+//     into 64 accumulator registers per thread, and park the 64 x 128 scores in the warpgroup's own shared-memory tile;
+//   * every thread then owns one user row and one half of the tile (warps 4g + h and 4g + h + 2 of warpgroup g cover
+//     rows 32 (2g + h) ..; one takes columns 0-63 of the tile, the other 64-127), each with its OWN candidate list and
+//     cut-off (the N best overall are among the N best of the two halves; the lists are merged at the end) -- and runs
+//     the selection of topn_kernels.cu with the count and cut-off in
 //     REGISTERS: 16 scores are compared without a branch; the few that beat the cut-off look up the row's 512-bit
 //     rated-set signature (built in shared memory when the kernel starts), run the exact rated test (bisection) only
 //     on a signature hit, and are appended to the row's 512-key list (L2-resident scratch).  Whenever a list could
 //     overflow, its warp finds the list's N-th largest key by a bit-wise search (16 keys per lane in registers, one
 //     warp reduction per bit -- no sort) and keeps the N keys at or above it; rows are sorted once, at the end.
+//     The operand stage is handed back to the copy engine as soon as both warpgroups' MMAs have retired, so the next
+//     tile streams in during the selection.
 // Nothing of the [users x items] matrix is written.  d <= 64, a multiple of 4 (one or two 128-byte k-blocks, zero-padded).
 #include "common.h"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int CAP = 320;   // candidate slots per half-row list (>= N_max + TRIG_EXTRA + the 64 items a tile can add)
 constexpr int TRIG_EXTRA = 96;   // a list is cut back to its N best once it holds more than N + TRIG_EXTRA keys
 constexpr int SORTN = 256; // keys of the final per-row sort (two lists of at most N_max keys)
-constexpr int NT = 256;    // selecting threads per CTA: 8 warps, two per TMEM lane quarter (a 9th warp drives TMA and the MMAs)
-constexpr int NBUF = 4;    // TMEM accumulators of 128 columns: the tensor cores may run up to 3 tiles ahead of the slowest warp
+constexpr int NT = 256;    // multiplying and selecting threads per CTA: two warpgroups (a 9th warp drives the bulk copies)
 constexpr int SIGW = 16;   // 32-bit words of a row's rated-set signature (512 bits) kept in shared memory
 constexpr int NMAX = 100;  // base/recommender.py:131-134 clamps N to <= 100
 constexpr int TM = 128, TN = 128;
 constexpr int KBLK = TM * 128;                       // bytes of one k-block (32 fp32 = 128 B per row) of a 128-row operand
+constexpr int SP = TN + 4;                           // row pitch (floats) of a warpgroup's score tile: conflict-free row reads
 
 __device__ __forceinline__ uint32_t ord_of(float s) {          // monotone float -> uint
   const uint32_t u = __float_as_uint(s);
@@ -73,27 +76,8 @@ __device__ __forceinline__ void warp_sort_desc(unsigned long long* k, int lane) 
   __syncwarp();
 }
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+using wg::smem_u32;
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (csrc/tc_gemm.cu): start>>4 | SBO = 1024 B | version 1 | swizzle 128B
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// instruction descriptor, kind::tf32: D = F32, A = B = TF32, both K-major, N = 128, M = 128
-__device__ __forceinline__ uint32_t make_idesc() {
-  uint32_t i = 0;
-  i |= 1u << 4;
-  i |= 2u << 7;
-  i |= 2u << 10;
-  i |= (uint32_t)(TN >> 3) << 17;
-  i |= (uint32_t)(TM >> 4) << 24;
-  return i;
-}
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
@@ -119,6 +103,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void group_sync(int group) {     // the 128 threads of one warpgroup
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + group) : "memory");
 }
 // byte offset of element (row, k) inside one K-major SWIZZLE_128B k-block (k in [0,32) fp32)
 __device__ __forceinline__ uint32_t sw_off(int row, int k) {
@@ -161,8 +148,9 @@ split_items_kernel(const float* __restrict__ V, int d, int n_items, uint8_t* __r
   }
 }
 
-// KB = d / 32 k-blocks.  Shared memory: A hi | A lo (KB x 16 KB each), then two B stages (hi | lo, KB x 16 KB each),
-// then one 2 KB sort buffer per warp (8 warps) and the 128 rows' 512-bit rated-set signatures (8 KB).
+// KB = d / 32 k-blocks.  Shared memory: A hi | A lo (KB x 16 KB each), then NSB = 3 - KB operand stages (hi | lo,
+// KB x 16 KB each), one 2 KB sort buffer per warp (8 warps), the 128 rows' 512-bit rated-set signatures (8 KB) and
+// the two warpgroups' 64 x 128 score tiles (33 KB each).
 template <int KB>
 __global__ void __launch_bounds__(NT + 32, 1)
 score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ item_blocks, int d, int n_items,
@@ -172,23 +160,27 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
   constexpr int D = KB * 32;
   constexpr int OPER = KB * KBLK;                     // bytes of one 128-row operand (hi or lo)
   constexpr int APT = TM * D / 4 / NT;                // float4 per thread of the users' 128-row operand (4 or 8)
+  constexpr int NSB = 3 - KB;                         // operand stages: two at d <= 32, one at d <= 64 (227 KB)
   extern __shared__ uint8_t smem_raw[];
   __shared__ int cnt_sh[2][TM];
-  __shared__ uint64_t mma_done[NBUF];                 // accumulator b holds a finished tile (tcgen05.commit)
-  __shared__ uint64_t acc_free[NBUF];                 // all 8 selecting warps are done with accumulator b
-  __shared__ uint64_t full[2];                        // operand stage s holds a whole tile (bulk-copy bytes counted)
-  __shared__ uint32_t tmem_base_slot;
+  __shared__ uint64_t full[NSB];                      // operand stage s holds a whole tile (bulk-copy bytes counted)
+  __shared__ uint64_t empty[NSB];                     // the 8 warps' MMAs that read stage s have retired
   // 1024-byte alignment by an offset from the array itself (not an integer round trip): the compiler keeps the
   // shared address space, so the sort / rated buffers are read with LDS / written with STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* const sA_hi = smem;
   uint8_t* const sA_lo = smem + OPER;
   uint8_t* const sB = smem + 2 * OPER;                // stage s: hi at sB + s * 2 * OPER, lo right behind it
-  unsigned long long* const sort_buf = reinterpret_cast<unsigned long long*>(smem + 6 * OPER);
-  uint32_t* const sig = reinterpret_cast<uint32_t*>(smem + 6 * OPER + 8 * SORTN * sizeof(unsigned long long));   // [SIGW][TM], word-major
+  unsigned long long* const sort_buf = reinterpret_cast<unsigned long long*>(smem + (2 + 2 * NSB) * OPER);
+  uint32_t* const sig = reinterpret_cast<uint32_t*>(smem + (2 + 2 * NSB) * OPER + 8 * SORTN * sizeof(unsigned long long));   // [SIGW][TM], word-major
+  float* const scores_all = reinterpret_cast<float*>(sig + SIGW * TM);                 // [2][64][SP]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int wq = warp & 3, half = warp >> 2;          // TMEM lane quarter; which 64 columns of a tile this thread selects from
-  const int rowl = wq * 32 + lane;                    // the thread's user row inside the CTA (= its TMEM lane)
+  const int grp = warp >> 2;                          // warpgroup: users 64 grp .. 64 grp + 63 of the CTA
+  const bool selecting = warp < NT / 32;
+  // the thread's 32-row quarter and which 64 columns of a tile it selects from (the 9th warp selects nothing)
+  const int wq = selecting ? 2 * grp + (warp & 1) : 0, half = selecting ? (warp >> 1) & 1 : 2;
+  const int rowl = wq * 32 + lane;                    // the thread's user row inside the CTA
+  float* const scores = scores_all + (size_t)(grp & 1) * 64 * SP;                      // this warpgroup's score tile
   const int row0 = blockIdx.x * TM;
   const int my_row = row0 + rowl;
   const int u = (my_row < n_rows) ? __ldg(user_ids + my_row) : -1;
@@ -209,17 +201,11 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
   }
 
   if (tid == 0) {
-    for (int b = 0; b < NBUF; ++b) {
-      mbar_init(&mma_done[b], 1);
-      mbar_init(&acc_free[b], NT / 32);
+    for (int b = 0; b < NSB; ++b) {
+      mbar_init(&full[b], 1);
+      mbar_init(&empty[b], NT / 32);
     }
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "n"(NBUF * TN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   // ---- the users' rows, split and stored once: float4 number q of the tile is (row q / (D/4), columns 4 * (q % (D/4)))
 #pragma unroll
@@ -235,12 +221,8 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
     *reinterpret_cast<float4*>(sA_hi + off) = hi;
     *reinterpret_cast<float4*>(sA_lo + off) = lo;
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // the A operands: generic-proxy writes -> async proxy (UMMA)
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // the A operands: generic-proxy writes -> async proxy (wgmma)
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_acc = tmem_base_slot;
-  const uint32_t idesc = make_idesc();
 
   const int n_tiles = (n_items + TN - 1) / TN;
   int cnt = 0;                                        // this thread's row: candidates in its list, current cut-off
@@ -306,7 +288,8 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
     if (lane == src) { cnt = base; thr = low; }        // base == N; low = the N-th best key
     __syncwarp();
   };
-  // selection over one finished accumulator (tile t, TMEM buffer t & 1)
+  // tile t: this warpgroup's 64 users x 128 items on the tensor cores, parked in its score tile, then the selection
+  constexpr uint32_t TILE_BYTES = 2 * OPER;
   auto select_tile = [&](int t) {
     // a row that could overflow during this tile goes back to its N best first (its warp works on it together)
     unsigned need = __ballot_sync(0xffffffffu, cnt > N + TRIG_EXTRA);
@@ -315,27 +298,58 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
       need &= need - 1;
       compact_row(src);
     }
+    {
+      const int s = t % NSB;
+      mbar_wait(&full[s], (uint32_t)((t / NSB) & 1));                  // tile t has landed
+      __syncwarp();                                                      // wgmma is warp-aligned: reconverge after the spin
+      uint8_t* const sB_hi = sB + s * TILE_BYTES;
+      uint8_t* const sB_lo = sB_hi + OPER;
+      float acc[64];
+      wg::fence();
+      bool first = true;
+#pragma unroll
+      for (int kb = 0; kb < KB; ++kb) {
+        const int a_off = kb * KBLK + grp * (KBLK / 2);                 // this warpgroup's 64 rows of the k-block
+        const uint64_t a_hi = wg::desc_sw128(smem_u32(sA_hi + a_off)), a_lo = wg::desc_sw128(smem_u32(sA_lo + a_off));
+        const uint64_t b_hi = wg::desc_sw128(smem_u32(sB_hi + kb * KBLK)), b_lo = wg::desc_sw128(smem_u32(sB_lo + kb * KBLK));
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4) {
+          const uint64_t step = (uint64_t)(k4 * 2);   // +2 = 32 bytes (8 tf32) along K inside the 128-byte span
+#pragma unroll
+          for (int term = 0; term < 3; ++term) {      // small terms first: lo.hi, hi.lo, then hi.hi
+            const uint64_t da = (term == 0 ? a_lo : a_hi) + step;
+            const uint64_t db = (term == 1 ? b_lo : b_hi) + step;
+            wg::mma_m64n128k8_tf32(acc, da, db, first ? 0u : 1u);
+            first = false;
+          }
+        }
+      }
+      wg::commit();
+      wg::wait<0>();
+      __syncwarp();
+      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
+      group_sync(grp);                                // every warp of the group is done reading the previous tile's scores
+      const int w4 = warp & 3;
+#pragma unroll
+      for (int e = 0; e < 64; e += 2)
+        *reinterpret_cast<float2*>(scores + wg::frag_row(w4, lane, e) * SP + wg::frag_col(lane, e)) = make_float2(acc[e], acc[e + 1]);
+      group_sync(grp);
+    }
     // pre-filter for the 128 scores of this tile (the cut-off only moves in the compaction above): a score below the
     // cut-off's score cannot pass, unless the list is not full yet or a rated item's fixed value could pass
     const bool open_row = thr == 0ULL || (uint32_t)(thr >> 32) <= (uint32_t)(rated_key_hi >> 32);
     const float thr_f = open_row ? -INFINITY : score_of((uint32_t)(thr >> 32));
-    const int buf = t % NBUF;
-    mbar_wait(&mma_done[buf], (uint32_t)((t / NBUF) & 1));
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     const int c0 = t * TN + half * 64;                                // first item of this thread's 64 columns
     const int valid = n_items - c0;                                    // columns of them that are items (may be <= 0 or > 64)
+    const float* const my_scores = scores + (rowl - 64 * grp) * SP + half * 64;
 #pragma unroll 1
     for (int cc = 0; cc < 64; cc += 16) {
       uint32_t r[16];
-      __syncwarp();                                   // the rare path below diverges; tcgen05.ld is warp-collective
-      const uint32_t taddr = tmem_acc + ((uint32_t)(wq * 32) << 16) + (uint32_t)(buf * TN + half * 64 + cc);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-            "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+#pragma unroll
+      for (int q = 0; q < 16; q += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(my_scores + cc + q);
+        r[q] = __float_as_uint(v.x); r[q + 1] = __float_as_uint(v.y); r[q + 2] = __float_as_uint(v.z); r[q + 3] = __float_as_uint(v.w);
+      }
       // 16 compares without a branch: bit q of `pass` <=> score q is at or above the cut-off's score
       uint32_t pass = 0;
 #pragma unroll
@@ -362,55 +376,19 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
         }
       }
     }
-    // the accumulator may be overwritten once all 8 warps are past their loads: each warp says so on acc_free
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncwarp();
-    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_free[buf])) : "memory");
   };
 
-  // ---- main loop.  The 9th warp's lane 0 drives the two engines -- bulk copies (tile j into the operand stage that
-  // MMA(j-2) has released) and the 24 MMAs of tile j into accumulator j % 4 once the 8 selecting warps have released
-  // it -- and never selects; the selecting warps follow at their own pace (no CTA-wide barrier per tile: a warp that
-  // compacts a list only holds back the accumulator it has not released yet).
-  constexpr uint32_t TILE_BYTES = 2 * OPER;
+  // ---- main loop.  The 9th warp's lane 0 streams the item tiles in (tile j into the operand stage that the MMAs of
+  // tile j - NSB have released) and never selects; the two warpgroups follow at their own pace (no CTA-wide barrier
+  // per tile: a warpgroup that compacts a list only holds back the stage its MMAs have not released yet).
   if (warp == NT / 32) {
     if (lane == 0) {
       for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1, b = j % NBUF;
-        if (j >= 2) mbar_wait(&mma_done[(j - 2) % NBUF], (uint32_t)(((j - 2) / NBUF) & 1));   // MMA(j-2) done: stage s is free
+        const int s = j % NSB;
+        if (j >= NSB) mbar_wait(&empty[s], (uint32_t)((j / NSB - 1) & 1));   // the MMAs of tile j - NSB have retired
         mbar_expect_tx(&full[s], TILE_BYTES);
         bulk_g2s(sB + s * TILE_BYTES, item_blocks + (size_t)j * TILE_BYTES, TILE_BYTES, &full[s]);
-        if (j >= NBUF) mbar_wait(&acc_free[b], (uint32_t)((j / NBUF - 1) & 1));              // select(j-4) done everywhere
-        mbar_wait(&full[s], (uint32_t)((j >> 1) & 1));                                        // tile j has landed
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint8_t* const sB_hi = sB + s * TILE_BYTES;
-        uint8_t* const sB_lo = sB_hi + OPER;
-        const uint32_t acc_addr = tmem_acc + (uint32_t)(b * TN);
-        bool first = true;
-#pragma unroll
-        for (int kb = 0; kb < KB; ++kb) {
-          const uint64_t a_hi = make_desc(smem_u32(sA_hi + kb * KBLK)), a_lo = make_desc(smem_u32(sA_lo + kb * KBLK));
-          const uint64_t b_hi = make_desc(smem_u32(sB_hi + kb * KBLK)), b_lo = make_desc(smem_u32(sB_lo + kb * KBLK));
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4) {
-            const uint64_t step = (uint64_t)(k4 * 2);   // +2 = 32 bytes (8 tf32) along K inside the 128-byte span
-#pragma unroll
-            for (int term = 0; term < 3; ++term) {      // small terms first: lo.hi, hi.lo, then hi.hi
-              const uint64_t da = (term == 0 ? a_lo : a_hi) + step;
-              const uint64_t db = (term == 1 ? b_lo : b_hi) + step;
-              const uint32_t accf = first ? 0u : 1u;
-              first = false;
-              asm volatile(
-                  "{\n\t.reg .pred p;\n\t"
-                  "setp.ne.b32 p, %4, 0;\n\t"
-                  "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(acc_addr), "l"(da), "l"(db), "r"(idesc),
-                  "r"(accf)
-                  : "memory");
-            }
-          }
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mma_done[b]))
-                     : "memory");
       }
     }
   } else {
@@ -447,17 +425,13 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
     }
     __syncwarp();
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(NBUF * TN));
-  }
 }
 
 template <int KB>
 int launch_tc(const float* U, const float* V, int d, int n_items, const int* user_ids, int n_rows, const long long* rowptr,
               const int* cols, float rated_value, int N, int* out_ids, float* out_scores, cudaStream_t st) {
-  constexpr int SMEM = 6 * KB * KBLK + 8 * SORTN * (int)sizeof(unsigned long long) + SIGW * TM * (int)sizeof(uint32_t) + 1024;   // operands + sort buffers + signatures + alignment
+  constexpr int SMEM = (2 + 2 * (3 - KB)) * KB * KBLK + 8 * SORTN * (int)sizeof(unsigned long long) + SIGW * TM * (int)sizeof(uint32_t) +
+                       2 * 64 * SP * (int)sizeof(float) + 1024;   // operands + sort buffers + signatures + score tiles + alignment
   static bool attr_set = false;
   if (!attr_set) {
     QREC_CUDA(cudaFuncSetAttribute(score_topn_tc_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));

@@ -2,7 +2,7 @@
 
 Tables and index arrays on the device are torch CUDA tensors (torch is plumbing: allocation,
 streams, torch.distributed); every compute call below goes through ctypes into the hand-written
-sm_100a kernels.  There is no CPU path here: device entry points raise if a tensor is not on a
+sm_90a kernels.  There is no CPU path here: device entry points raise if a tensor is not on a
 CUDA device.
 """
 import ctypes as C
@@ -323,7 +323,7 @@ def bpr_sgd_usermajor(P, Q, rowptr, i, j, lr, reg_u, reg_i, loss):
     n_users = rowptr.shape[0] - 1
     assert i.shape[0] == j.shape[0]
     check(lib.qrec_bpr_sgd_usermajor_f32(_dev(P, torch.float32, 'P'), _dev(Q, torch.float32, 'Q'), P.shape[1], n_users,
-                                         int(i.shape[0]),
+                                         int(i.shape[0]), Q.shape[0],
                                          _dev(rowptr, torch.int64, 'rowptr'), _dev(i, torch.int32, 'i'),
                                          _dev(j, torch.int32, 'j'), float(lr), float(reg_u), float(reg_i),
                                          _dev(loss, torch.float64, 'loss'), _stream()), 'qrec_bpr_sgd_usermajor_f32')
@@ -458,7 +458,7 @@ SCORE_TOPN_TENSOR_CORES = True       # default of score_topn(tensor_cores=None) 
 def score_topn(U, V, user_ids, rated_rowptr, rated_cols, N, rated_value=0.0, out_ids=None, out_scores=None, tensor_cores=None):
     """K8: the N best items of every listed user in one kernel (scores, rated -> rated_value, top-N; nothing
     materialised).  Returns (ids int32 [n, N], scores fp32 [n, N]), best first, ties by ascending item id.
-    tensor_cores: True = the tcgen05 3xTF32 kernel (csrc/topn_tc.cu; d <= 64, multiple of 4), False = the fp32 SIMT kernel
+    tensor_cores: True = the wgmma 3xTF32 kernel (csrc/topn_tc.cu; d <= 64, multiple of 4), False = the fp32 SIMT kernel
     (csrc/topn_kernels.cu), None = the module default where the width allows it."""
     torch = _torch()
     if tensor_cores is None:
@@ -873,7 +873,7 @@ def _ld(t):
 
 def tc_gemm(A, B, C, b_is_nk=False, epilogue=EPI_NONE, bias=None, mask=None):
     """C = epilogue(A @ B) (b_is_nk=False, B [K,N]) or epilogue(A @ B.T) (b_is_nk=True, B [N,K]) on the
-    tcgen05 TF32 tensor-core path."""
+    wgmma TF32 tensor-core path."""
     torch = _torch()
     M, K = A.shape
     N = B.shape[0] if b_is_nk else B.shape[1]

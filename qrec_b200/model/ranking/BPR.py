@@ -1,4 +1,4 @@
-"""BPR-MF on the B200 engine -- drop-in for model/ranking/BPR.py of the reference.
+"""BPR-MF on the H100 engine -- drop-in for model/ranking/BPR.py of the reference.
 
 `trainModel` replaces the numpy loop (BPR.py:19-43): every epoch the (u,i,j) stream is produced
 by the bit-exact C clone of Python's MT19937 sampler (continuing from the interpreter's global

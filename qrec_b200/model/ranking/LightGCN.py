@@ -1,4 +1,4 @@
-"""LightGCN on the B200 engine -- drop-in for model/ranking/LightGCN.py of the reference.
+"""LightGCN on the H100 engine -- drop-in for model/ranking/LightGCN.py of the reference.
 
 The reference re-runs the whole n-layer propagation, its backward pass and a dense Adam update
 for EVERY minibatch (LightGCN.py:35-39: one sess.run per batch).  The same computation here:

@@ -1,4 +1,4 @@
-"""NGCF on the B200 engine -- drop-in for model/ranking/NGCF.py of the reference.
+"""NGCF on the H100 engine -- drop-in for model/ranking/NGCF.py of the reference.
 
 Two propagation layers (hard-coded in the reference, NGCF.py:19); per layer
     side = A ego                                   K2 SpMM
@@ -27,7 +27,7 @@ class NGCF(GraphRecommender):
         super(NGCF, self).initModel()
         import torch
         if self.emb_size % 4:
-            raise ValueError('NGCF on the B200 engine needs num.factors to be a multiple of 4 (got %d)' % self.emb_size)
+            raise ValueError('NGCF on the H100 engine needs num.factors to be a multiple of 4 (got %d)' % self.emb_size)
         dev, d = self.device, self.emb_size
         self.n_layers = 2
         n = self.num_users + self.num_items

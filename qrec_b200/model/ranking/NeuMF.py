@@ -1,4 +1,4 @@
-"""NeuMF on the B200 engine -- drop-in for model/ranking/NeuMF.py of the reference.
+"""NeuMF on the H100 engine -- drop-in for model/ranking/NeuMF.py of the reference.
 
 GMF head + 3-layer MLP (2d -> 5d -> 2d -> d, ReLU) + fused head, trained in the reference's three
 phases (GMF `maxEpoch` epochs, MLP `maxEpoch//2`, fused `maxEpoch//5`; NeuMF.py:77-100), each with
@@ -7,7 +7,7 @@ Batches come from next_batch_pointwise (1 positive + 4 sampled negatives per int
 
 Engine mapping (one minibatch of B = 5*batch_size samples):
   gather      qrec_gather_rows_f32 -> UG, IG and the concatenated MLP input [B, 2d]
-  MLP fwd     3 x qrec_tc_gemm_tf32 (tcgen05 TF32, bias+ReLU fused in the TMEM epilogue)
+  MLP fwd     3 x qrec_tc_gemm_tf32 (wgmma TF32, bias+ReLU fused in the epilogue)
   head        qrec_neumf_head_f32: sigmoid, BCE(+1e-9), dz, GMF-side gradients, ReLU-masked dH3
   MLP bwd     dX = dY W^T on the tensor cores (ReLU mask fused); dW = X^T dY and the bias/h-vector
               column sums on the split-K fp32 path (K = B is the long dimension there)
@@ -30,7 +30,7 @@ class NeuMF(DeepRecommender):
         super(NeuMF, self).initModel()
         import torch
         if self.emb_size % 4:
-            raise ValueError('NeuMF on the B200 engine needs num.factors to be a multiple of 4 (got %d)' % self.emb_size)
+            raise ValueError('NeuMF on the H100 engine needs num.factors to be a multiple of 4 (got %d)' % self.emb_size)
         dev, d = self.device, self.emb_size
         # MLP widths after the 2d-wide input: the reference hard-codes 5d -> 2d -> d (NeuMF.py:39-49); BASELINE.json's
         # config 4 names [256,128,64].  The attribute `mlp_widths` overrides; the last width feeds the fused head

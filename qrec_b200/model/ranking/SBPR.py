@@ -1,4 +1,4 @@
-"""SBPR (social BPR, Zhao et al. CIKM'14) on the B200 engine -- drop-in for model/ranking/SBPR.py.
+"""SBPR (social BPR, Zhao et al. CIKM'14) on the H100 engine -- drop-in for model/ranking/SBPR.py.
 
 What the reference class does, path by path:
 

@@ -1,4 +1,4 @@
-"""SGL (self-supervised graph learning) on the B200 engine -- drop-in for model/ranking/SGL.py of the reference.
+"""SGL (self-supervised graph learning) on the H100 engine -- drop-in for model/ranking/SGL.py of the reference.
 
 Per epoch the reference rebuilds two augmented views of the interaction graph on the host with scipy
 (`_create_adj_mat`, SGL.py:113-155; aug_type 0 node dropout, 1 edge dropout, 2 "random walk" = a fresh edge

@@ -1,4 +1,4 @@
-"""SimGCL on the B200 engine -- drop-in for model/ranking/SimGCL.py of the reference.
+"""SimGCL on the H100 engine -- drop-in for model/ranking/SimGCL.py of the reference.
 
 Per minibatch the reference runs three LightGCN encoders over the whole graph (one clean, two with
 fresh uniform-noise perturbation after every layer), BPR + batch L2 on the clean one, InfoNCE

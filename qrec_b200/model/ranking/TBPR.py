@@ -1,4 +1,4 @@
-"""TBPR (social BPR with strong / weak ties) on the B200 engine -- drop-in for model/ranking/TBPR.py.
+"""TBPR (social BPR with strong / weak ties) on the H100 engine -- drop-in for model/ranking/TBPR.py.
 
 The reference's inner step `optimization(u, i, j)` (TBPR.py:44-52) is BPR.optimization statement for statement, so
 the engine's K1 kernels run it unchanged; what is specific to TBPR is the HOST side, kept here with the

@@ -1,4 +1,4 @@
-"""BasicMF on the B200 engine -- drop-in for model/rating/BasicMF.py of the reference (kind 0 of K9):
+"""BasicMF on the H100 engine -- drop-in for model/rating/BasicMF.py of the reference (kind 0 of K9):
 P[u] += lr*e*Q[i]; Q[i] += lr*e*P[u]; loss = sum e^2, no regulariser (BasicMF.py:13-23)."""
 from ._pointwise import PointwiseMF
 

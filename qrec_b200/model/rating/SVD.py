@@ -1,4 +1,4 @@
-"""SVD (biased MF) on the B200 engine -- drop-in for model/rating/SVD.py of the reference (kind 2 of
+"""SVD (biased MF) on the H100 engine -- drop-in for model/rating/SVD.py of the reference (kind 2 of
 K9): PMF's step with e taken against P[u].Q[i] + globalMean + Bi[i] + Bu[u], plus the two bias
 updates and their regB penalty (SVD.py:17-34); training runs all epochs (SVD.py:36 ignores the
 convergence flag)."""

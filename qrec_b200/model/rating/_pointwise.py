@@ -1,4 +1,4 @@
-"""Shared trainer of the rating-prediction MF family (BasicMF / PMF / SVD) on the B200 engine.
+"""Shared trainer of the rating-prediction MF family (BasicMF / PMF / SVD) on the H100 engine.
 
 The reference visits `self.data.trainingData` entry by entry in list order and `isConverged`
 reshuffles the list after every epoch (model/rating/PMF.py:13-22, base/iterativeRecommender.py:101).
@@ -12,8 +12,6 @@ Here an epoch is one launch over the id-mapped (u, i, r) arrays of the list's cu
                           in-flight window is bounded to (0.25/lr) / (share of the most frequent row)
                           entries: 33 750 user-sorted FilmTrust entries applied as one stale step
                           diverge.
-STATUS: the kernels behind this module were written after round 1's GPU budget was spent; they
-compile for sm_100a and the oracle is pinned, but no hardware run has validated them yet.
 """
 import numpy as np
 

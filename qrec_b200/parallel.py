@@ -602,8 +602,8 @@ class UserShardedLightGCN(object):
         z = lambda n: torch.zeros(n, d, device=dev)           # noqa: E731
         self.bu, self.bi = [z(nu), z(nu)], [z(ni), z(ni)]
         # the item-side partial sums of a layer are written straight into peer-mapped buffers and summed over
-        # NVLink by our own kernels (PeerAllReduce) when QREC_PEER_ALLREDUCE=1 -- validated, but at N=2 NCCL's all-reduce
-        # of the 25.6 MB block was the faster of the two at B=2048 (5.7 vs 7.1 ms/step), so NCCL is the default;
+        # NVLink by our own kernels (PeerAllReduce) when QREC_PEER_ALLREDUCE=1; NCCL's all-reduce of the 25.6 MB
+        # block is the default;
         # gloo / world 1: plain tensors
         self.peer = None
         import os as _os
@@ -757,9 +757,8 @@ class UserShardedLightGCN(object):
         return self.loss
 
     # ---- the same step replayed from a CUDA graph ---------------------------------------------------------------
-    # At N = 8 a rank's share of a step is ~1 ms of device work issued through ~80 launches (kernels, the sort / where
-    # ops of the row lists, the NCCL calls): the host could not issue them that fast and the 8-GPU step was bound by
-    # the CPU (2.3 ms).  The step has no host read-back and a fixed launch sequence for a given batch size, so it is
+    # At large N a rank's share of a step is little device work issued through ~80 launches (kernels, the sort / where
+    # ops of the row lists, the NCCL calls), so the host's issue rate can bound the step.  The step has no host read-back and a fixed launch sequence for a given batch size, so it is
     # captured once -- kernels on torch's capture stream, the all-reduces on NCCL's stream with the captured event
     # dependencies, so the overlap of an exchange with the neighbouring products survives -- and replayed per minibatch
     # after three small device copies into the graph's input buffers.
@@ -806,9 +805,8 @@ _CAPTURED_GRAPHS = [0]
 
 
 def captured_graphs():
-    """How many CUDA graphs with NCCL collectives inside this process has captured.  Measured on 2 GPUs
-    (profiles/r2/s2): while such a graph (or its executable) is alive, tearing the NCCL communicator down --
-    dist.destroy_process_group(), or the interpreter's own shutdown -- does not return.  A program that used
+    """How many CUDA graphs with NCCL collectives inside this process has captured.  While such a graph (or its
+    executable) is alive, tearing the NCCL communicator down -- dist.destroy_process_group(), or the interpreter's own shutdown -- does not return.  A program that used
     train_step_graphed under NCCL therefore ends with `finish_process()` instead of destroy_process_group()."""
     return _CAPTURED_GRAPHS[0]
 

@@ -27,7 +27,7 @@ def test_every_declared_symbol_is_exported_and_bound():
 def test_version_and_error_channel():
     from qrec_b200 import engine as E
     from qrec_b200._lib import lib
-    assert 'sm_100a' in E.version()
+    assert 'sm_90a' in E.version()
     rc = lib.qrec_mt_seed(None, 0)
     assert rc == -1 and b'null' in lib.qrec_last_error()
 
@@ -43,8 +43,8 @@ def test_product_does_not_touch_oracle():
                 assert 'liboracle' not in txt, f
 
 
-def test_sm100a_only_and_blackwell_sass():
-    """The cubin inside libqrec.so targets sm_100a and uses the 128-bit vector reduction."""
+def test_sm90a_only_and_hopper_sass():
+    """The cubin inside libqrec.so targets sm_90a and uses the 128-bit vector reduction."""
     import shutil
     import subprocess
     from qrec_b200 import _lib
@@ -53,7 +53,7 @@ def test_sm100a_only_and_blackwell_sass():
         import pytest
         pytest.skip('cuobjdump not available')
     out = subprocess.run([cuobjdump, '-lelf', _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert 'sm_100a' in out and 'sm_90' not in out and 'sm_80' not in out
+    assert 'sm_90a' in out and 'sm_100' not in out and 'sm_80' not in out
     sass = subprocess.run([cuobjdump, '-sass', _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert 'REDG.E.ADD.F32x4' in sass          # red.global.add.v4.f32 scatter-add
     assert 'LDG.E.128' in sass                 # 128-bit row gathers

@@ -447,6 +447,31 @@ def test_usermajor_empty_and_bad_args(torch, E):
                             torch.zeros(5, dtype=torch.int64, device='cuda'), z, z, 0.1, 0.1, 0.1, loss)
 
 
+def test_usermajor_epoch_is_the_same_every_run(torch, E):
+    """Two fused epochs from the same tables and stream agree up to the summation order of the scatter-adds: what a
+    triple reads does not depend on timing (each user whole in one lane group; item rows read from the snapshot of
+    the wave).  Reads that raced with other lane groups' scatter-adds made runs differ by a fifth of the update."""
+    from qrec_b200 import synthetic
+    dev = torch.device('cuda', 0)
+    users, items, deg, d = 200_000, 20_000, 20, 64
+    data = synthetic.make_interactions(users, items, deg, device=dev, seed=5)
+    sig = E.rated_signature(data['sorted_rowptr'], data['sorted_cols'])
+    runs = []
+    for _ in range(2):
+        P, Q = synthetic.init_tables(users, items, d, seed=6, device=dev)
+        loss = torch.zeros(1, dtype=torch.float64, device=dev)
+        E.bpr_epoch_usermajor_sig(P, Q, data['sorted_rowptr'], data['i'], data['sorted_rowptr'], data['sorted_cols'], sig,
+                                  items, 77, 0, LR, REG, REG, loss)
+        torch.cuda.synchronize()
+        runs.append((P.cpu(), Q.cpu(), loss.item()))
+    P0, Q0 = synthetic.init_tables(users, items, d, seed=6, device=dev)
+    for k, X0 in ((0, P0.cpu()), (1, Q0.cpu())):
+        update = float((runs[0][k] - X0).abs().max())
+        assert update > 0
+        assert float((runs[0][k] - runs[1][k]).abs().max()) <= 1e-4 * update
+    assert abs(runs[0][2] - runs[1][2]) <= 1e-9 * abs(runs[0][2])
+
+
 def test_fused_epoch_equals_sampler_plus_kernel(torch, E, bpr_ids):
     """qrec_bpr_epoch_usermajor_f32 (sampling fused into the user-major kernel) draws exactly the
     negatives qrec_sample_neg_philox draws (same Philox counters) and then does the same updates."""

@@ -1,7 +1,6 @@
 """The signature pre-test in the fused sampler (qrec_bpr_epoch_usermajor_sig_f32): the 512-bit rated-set
 signature has no false negatives, so the sampled negatives must be bit-identical to the plain fused
-kernel and to the stand-alone Philox sampler.  Needs a GPU.
-First run on a B200 in round 2 (6.27 vs 6.59 ms per 50 M triples; the bench's default sampler since)."""
+kernel and to the stand-alone Philox sampler.  Needs a GPU."""
 import os
 
 import numpy as np

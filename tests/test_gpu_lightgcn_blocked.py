@@ -1,7 +1,6 @@
 """Column-blocked item-side SpMM of parallel.UserShardedLightGCN (item_side_blocks > 1) against the
 unblocked step on the reference's FilmTrust graph: same losses, gradients and tables up to the fp32
-regrouping of each item row's sum.  Measured in round 2: 11.8 ms/step with 3 blocks against 11.9 ms
-with one -- no gain on the benchmark graph, the option stays off by default."""
+regrouping of each item row's sum.  The option stays off by default."""
 import contextlib
 import io
 import os

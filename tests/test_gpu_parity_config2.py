@@ -16,7 +16,6 @@ pytestmark = pytest.mark.gpu
 
 LOSS_REL = 1e-3            # sum of -ln(sigmoid) over the epoch
 P_RMS, Q_RMS = 0.10, 0.15  # ||X - X_ref||_F / ||X_ref - X_0||_F : error relative to what the epoch moved
-#                            measured on a B200 (one sweep over the stream): loss 7.5e-6, P 0.048, Q 0.058
 
 
 def _run(users, items, zipf, loss_rel, p_rms, q_rms):

@@ -1,6 +1,5 @@
 """Parity tests for K9 (the rating-prediction MF family, SURVEY.md §8 f-4): the CUDA path through the C
-ABI against the pinned oracle and the golden runs of the reference's BasicMF / PMF / SVD.  Needs a GPU.
-First run on a B200 in round 2 (8.3-9.4 G entries/s, tools/bench_rating.py)."""
+ABI against the pinned oracle and the golden runs of the reference's BasicMF / PMF / SVD.  Needs a GPU."""
 import os
 
 import numpy as np

@@ -1,7 +1,6 @@
 """Experimental row-split SpMM configurations (csrc/spmm_variants.cu) against the production kernel:
 they change the number of outstanding gathers and the occupancy, not the floating-point order, so the
-outputs must be bit-identical.  Needs a GPU.  First run on a B200 in round 2: variant 0
-(width-specialised, 4 CTAs/SM) is 2.15 ms against 2.49 ms and now serves d = 64."""
+outputs must be bit-identical.  Needs a GPU."""
 import os
 
 import numpy as np

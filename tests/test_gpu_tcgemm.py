@@ -1,4 +1,4 @@
-"""K5 building block: the tcgen05 TF32 GEMM against an fp64 product.  TF32 keeps 10 mantissa
+"""K5 building block: the wgmma TF32 GEMM against an fp64 product.  TF32 keeps 10 mantissa
 bits of each operand, so the tolerance is 2^-10-ish relative to |A||B| row/column norms."""
 import pytest
 

@@ -1,7 +1,6 @@
-"""K5 v2 (persistent, TMA-fed, warp-specialised tcgen05 GEMM) against an fp64 product and against v1.
+"""K5 v2 (persistent, TMA-fed, warp-specialised wgmma GEMM) against an fp64 product and against v1.
 A is consumed as raw fp32 bits (TF32 truncation: up to 2^-10 per operand, one-sided), so the bound is
-twice v1's.  Needs a GPU.
-First run on a B200 in round 2: 131-169 TFLOP/s at M = 327 680 (v1: 94-100), slower than v1 at M = 10 240."""
+twice v1's.  Needs a GPU."""
 import os
 
 import pytest
@@ -28,7 +27,7 @@ def _bound(A, B_kn):
 
 def test_exact_on_tf32_representable_inputs(torch, E):
     """Small integers are exact in TF32: the product must be bit exact, which pins the tensor map, the
-    swizzle, the descriptors, the stage ring, the two TMEM buffers and the epilogue transpose (any
+    swizzle, the descriptors, the stage ring and the epilogue transpose (any
     misplaced element is a wrong integer).  Sizes cover several row tiles per CTA and ragged edges."""
     g = torch.Generator(device='cuda'); g.manual_seed(0)
     for M, N, K in ((384, 192, 160), (128, 64, 32), (100000, 320, 128), (129, 65, 68), (1, 1, 4), (4097, 130, 320)):

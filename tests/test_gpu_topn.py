@@ -46,7 +46,7 @@ def _csr(rng, nu, ni, max_deg):
 
 @pytest.mark.parametrize('nu,ni,d,N,signed,tc', [(130, 1000, 64, 10, False, False), (77, 333, 52, 100, True, False), (5, 150, 8, 50, True, False),
                                                  (300, 20000, 64, 20, False, False), (64, 129, 128, 100, True, False),
-                                                 # the tcgen05 3xTF32 kernel (d <= 64): same bounds -- fp32-level scores
+                                                 # the wgmma 3xTF32 kernel (d <= 64): same bounds -- fp32-level scores
                                                  (130, 1000, 64, 10, False, True), (77, 333, 32, 100, True, True), (5, 150, 64, 50, True, True),
                                                  (300, 20000, 64, 20, False, True), (129, 257, 32, 100, True, True), (90, 700, 52, 30, True, True), (40, 300, 8, 20, False, True),
                                                  (1000, 5000, 64, 100, True, True)])

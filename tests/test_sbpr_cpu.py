@@ -1,8 +1,8 @@
 """SBPR drop-in (f-4 sibling model: model/ranking/SBPR.py mirror) on the CPU.
 
-(1) the item sets and the minibatch sampler against the UNMODIFIED reference class in the same process (TensorFlow
-    stubbed: `initModel` and `next_batch` never touch it): same PositiveSet / FPSet, same (u, i, k, j, S_uk) batches
-    from the same `random` state, same generator state afterwards;
+(1) the item sets and the minibatch sampler against the UNMODIFIED reference class (its result recorded by
+    oracle/gen_golden.py in tests/golden/reference_digests.json): same PositiveSet / FPSet, same (u, i, k, j, S_uk)
+    batches from the same `random` state, same generator state afterwards;
     and (portable: no reference checkout needed) against the golden record oracle/gen_golden.py made from the unmodified
     reference class on FilmTrust with its real trust network (tests/golden/sbpr_filmtrust_seed77.npz);
 (2) the numpy path stops where the reference's does (SBPR.py:47, TypeError);
@@ -12,8 +12,6 @@ import contextlib
 import io
 import os
 import random
-import sys
-import types
 
 import numpy as np
 import pytest
@@ -22,7 +20,6 @@ from qrec_b200.util.config import ModelConf
 from test_bpr_model_cpu import _stub_engine
 from test_tbpr_cpu import _data
 
-REF = '/root/reference'
 CONF = '''ratings=x
 social=x
 ratings.setup=-columns 0 1 2
@@ -86,47 +83,42 @@ def test_sbpr_item_sets_and_numpy_path_error(golden_bpr, monkeypatch, tmp_path):
         assert (w == 0 and len(m.FPSet[user]) == 0) or m.FPSet[user][id2item[k]] == w
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='reference checkout not mounted')
+def sampler_view(m):
+    """What the sampler comparison looks at, for an SBPR object after initModel(): the social-feedback sets, the key
+    order of FPSet (`choice(list(keys))` depends on it), the minibatches of next_batch() at batch size 700 from
+    random.seed(77), and the generator state afterwards."""
+    m.batch_size = 700
+    random.seed(77)
+    batches = [[list(x) for x in b] for b in m.next_batch()]
+    return [{u: dict(v) for u, v in m.PositiveSet.items() if v}, {u: dict(v) for u, v in m.FPSet.items() if v},
+            {u: list(v.keys()) for u, v in m.FPSet.items()}, batches, random.getstate()]
+
+
+def reference_sampler_view(R, RConf, golden_bpr, workdir):
+    """sampler_view of the reference class R on the same data (oracle/gen_golden.py records its digest)."""
+    train, test, rel = _data(golden_bpr, 3000)
+    conf_file = os.path.join(workdir, 'sbpr.conf')
+    with open(conf_file, 'w') as f:
+        f.write(CONF)
+    np.random.seed(1)
+    ref = R(RConf(conf_file), [list(r) for r in train], [list(r) for r in test], [list(r) for r in rel])
+    with contextlib.redirect_stdout(io.StringIO()):
+        ref.readConfiguration()
+        ref.initModel()
+    return sampler_view(ref)
+
+
 def test_sbpr_sampler_equals_unmodified_reference_class(golden_bpr, monkeypatch, tmp_path):
+    """The drop-in's sets, FPSet key order, minibatches and generator state equal those of the reference's SBPR
+    class on the same data (its result recorded in tests/golden/reference_digests.json)."""
+    import reference_cases
     calls = []
     _stub_engine(monkeypatch, calls)
     monkeypatch.chdir(tmp_path)
     m, train, test, rel = _model(golden_bpr)
-    before = set(sys.modules)
-    tf = types.ModuleType('tensorflow')
-    for name, mod in (('tensorflow', tf), ('mkl', types.ModuleType('mkl'))):
-        sys.modules.setdefault(name, mod)
-    sys.path.insert(0, REF)
-    try:
-        import importlib
-        R = importlib.import_module('model.ranking.SBPR').SBPR
-        RConf = importlib.import_module('util.config').ModelConf
-        conf_file = tmp_path / 'sbpr.conf'
-        conf_file.write_text(CONF)
-        np.random.seed(1)
-        ref = R(RConf(str(conf_file)), [list(r) for r in train], [list(r) for r in test], [list(r) for r in rel])
-        with contextlib.redirect_stdout(io.StringIO()):
-            ref.readConfiguration()
-            ref.initModel()
-        ref.batch_size = 700
-        assert {u: dict(v) for u, v in ref.PositiveSet.items() if v} == {u: dict(v) for u, v in m.PositiveSet.items() if v}
-        assert {u: dict(v) for u, v in ref.FPSet.items() if v} == {u: dict(v) for u, v in m.FPSet.items() if v}
-        for u in ref.FPSet:
-            assert list(ref.FPSet[u].keys()) == list(m.FPSet[u].keys())         # `choice(list(keys))` depends on the order
-        random.seed(77)
-        ref_batches = [tuple(list(x) for x in b) for b in ref.next_batch()]
-        ref_state = random.getstate()
-    finally:
-        sys.path.remove(REF)
-        for k in set(sys.modules) - before:
-            del sys.modules[k]
-    random.seed(77)
-    m.batch_size = 700
-    ours = [tuple(list(x) for x in b) for b in m.next_batch()]
-    assert random.getstate() == ref_state
-    assert len(ours) == len(ref_batches) == 5
-    for a, b in zip(ours, ref_batches):
-        assert a == b
+    view = sampler_view(m)
+    assert len(view[3]) == 5
+    assert reference_cases.digest(view) == reference_cases.recorded('sbpr_sampler')
 
 
 def test_sbpr_trainModel_tf_composition_equals_autograd_restatement(golden_bpr, monkeypatch, tmp_path):

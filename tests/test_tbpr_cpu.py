@@ -3,16 +3,15 @@ kernels are replaced by the pinned oracle, so what is checked is the HOST side t
 strengths, the per-epoch strong / weak / joint item sets, the preference chains and their draw order from Python's
 `random`, the per-user regulariser quirk of the loss, the learning-rate bookkeeping.
 
-(1) differential against the UNMODIFIED reference class run in the same process (only where /root/reference is
-    mounted: the joint set is iterated in Python set order, which depends on the interpreter's string-hash seed, so
-    a recorded golden stream would not be portable -- a same-process differential is);
+(1) differential against the UNMODIFIED reference class: its run was recorded with the string-hash seed 0
+    (tests/golden/tbpr_reference_hashseed0.npz; the joint set is iterated in Python set order, which depends on that
+    seed), and the drop-in runs in a fresh interpreter with the same seed;
 (2) self-consistency that also runs on the GPU box's CPU suite."""
 import contextlib
 import io
 import os
 import random
 import sys
-import types
 
 import numpy as np
 import pytest
@@ -20,7 +19,6 @@ import pytest
 from qrec_b200.util.config import ModelConf
 from test_bpr_model_cpu import _stub_engine
 
-REF = '/root/reference'
 CONF = '''ratings=x
 social=x
 ratings.setup=-columns 0 1 2
@@ -117,42 +115,72 @@ def test_tbpr_host_logic_self_consistency(golden_bpr, monkeypatch, tmp_path):
     assert len(seen['rowptr']) == m.num_users + 1 and seen['rowptr'][-1] == seen['n'] and np.all(np.diff(seen['rowptr']) >= 0)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='reference checkout not mounted')
-def test_tbpr_equals_unmodified_reference_class(golden_bpr, monkeypatch, tmp_path):
-    """Same seeds, same process: epoch losses, learning rates, theta, the final tables and the ranking measures of
-    the drop-in equal those of the reference's TBPR (numpy path) -- K1 being the oracle here."""
+GOLDEN_TBPR = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'tbpr_reference_hashseed0.npz')
+
+
+def _result(m, losses, measure):
+    return dict(theta=m.theta, t_s=m.t_s, t_w=m.t_w, lrates=np.array([l[1] for l in losses]),
+                losses=np.array([l[0] for l in losses]), P=np.asarray(m.P), Q=np.asarray(m.Q),
+                measure=np.array([x.strip() for x in measure]))
+
+
+def mine_result(golden_bpr, workdir):
+    """The drop-in's TBPR run (K1 replaced by the pinned oracle) under the seeds of the reference run."""
     from qrec_b200.model.ranking.TBPR import TBPR
     train, test, rel = _data(golden_bpr)
-    # ---- the reference, under a private import context
-    before = set(sys.modules)
-    for name in ('tensorflow', 'mkl'):
-        sys.modules.setdefault(name, types.ModuleType(name))
-    sys.path.insert(0, REF)
+    with pytest.MonkeyPatch.context() as mp:
+        _stub_engine(mp, [])
+        mp.chdir(workdir)
+        return _result(*_run(TBPR, train, test, rel, CONF))
+
+
+def reference_result(R, RConf, golden_bpr, workdir):
+    """The reference's TBPR class (numpy path) on the same data and seeds (oracle/gen_golden.py records it)."""
+    train, test, rel = _data(golden_bpr)
+    conf_file = os.path.join(workdir, 'tbpr.conf')
+    with open(conf_file, 'w') as f:
+        f.write(CONF)
+    cwd = os.getcwd()
+    os.chdir(workdir)
     try:
-        import importlib
-        R = importlib.import_module('model.ranking.TBPR').TBPR
-        RConf = importlib.import_module('util.config').ModelConf
-        conf_file = tmp_path / 'tbpr.conf'
-        conf_file.write_text(CONF)
-        monkeypatch.chdir(tmp_path)
         random.seed(11); np.random.seed(11)
-        ref = R(RConf(str(conf_file)), [list(r) for r in train], [list(r) for r in test], [list(r) for r in rel])
+        ref = R(RConf(conf_file), [list(r) for r in train], [list(r) for r in test], [list(r) for r in rel])
         ref_losses = []
         orig = R.isConverged
         R.isConverged = lambda self, epoch: (ref_losses.append((self.loss, self.lRate)), orig(self, epoch))[1]
         with contextlib.redirect_stdout(io.StringIO()):
             ref_measure = ref.execute()
     finally:
-        sys.path.remove(REF)
-        for k in set(sys.modules) - before:
-            del sys.modules[k]
-    # ---- the drop-in
-    calls = []
-    _stub_engine(monkeypatch, calls)
-    m, losses, measure = _run(TBPR, train, test, rel, CONF)
-    assert m.theta == ref.theta and m.t_s == ref.t_s and m.t_w == ref.t_w
-    assert [l[1] for l in losses] == [l[1] for l in ref_losses]
-    np.testing.assert_allclose([l[0] for l in losses], [l[0] for l in ref_losses], rtol=1e-12)
-    np.testing.assert_allclose(m.P, ref.P, rtol=1e-12, atol=1e-15)
-    np.testing.assert_allclose(m.Q, ref.Q, rtol=1e-12, atol=1e-15)
-    assert [x.strip() for x in measure] == [x.strip() for x in ref_measure]
+        os.chdir(cwd)
+    return _result(ref, ref_losses, ref_measure)
+
+
+def run_with_hash_seed_0(call, out_path, prelude=''):
+    """Runs `call` (source of an expression over golden_bpr and workdir) in a fresh interpreter with
+    PYTHONHASHSEED=0 -- the joint item set is iterated in set order -- and saves its result to out_path.  `prelude`
+    is source run first."""
+    import subprocess
+    here = os.path.dirname(os.path.abspath(__file__))
+    code = ('import os, sys, tempfile, numpy as np\n'
+            'sys.path[:0] = [%r, %r]\n'
+            + prelude +
+            'import test_tbpr_cpu as T\n'
+            'golden_bpr = np.load(os.path.join(%r, "golden", "bpr_filmtrust_seed0.npz"))\n'
+            'workdir = tempfile.mkdtemp()\n'
+            'np.savez(%r, **(%s))\n') % (here, os.path.dirname(here), here, out_path, call)
+    env = dict(os.environ, PYTHONHASHSEED='0')
+    subprocess.run([sys.executable, '-c', code], check=True, env=env, cwd=here)
+
+
+def test_tbpr_equals_unmodified_reference_class(tmp_path):
+    """Same seeds and string-hash seed: epoch losses, learning rates, theta, the final tables and the ranking
+    measures of the drop-in equal those the reference's TBPR (numpy path) recorded -- K1 being the oracle here."""
+    out = str(tmp_path / 'mine.npz')
+    run_with_hash_seed_0('T.mine_result(golden_bpr, workdir)', out)
+    m, ref = np.load(out), np.load(GOLDEN_TBPR)
+    assert float(m['theta']) == float(ref['theta']) and float(m['t_s']) == float(ref['t_s']) and float(m['t_w']) == float(ref['t_w'])
+    assert m['lrates'].tolist() == ref['lrates'].tolist()
+    np.testing.assert_allclose(m['losses'], ref['losses'], rtol=1e-12)
+    np.testing.assert_allclose(m['P'], ref['P'], rtol=1e-12, atol=1e-15)
+    np.testing.assert_allclose(m['Q'], ref['Q'], rtol=1e-12, atol=1e-15)
+    assert m['measure'].tolist() == ref['measure'].tolist()

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times the tcgen05 TF32 GEMM on NeuMF's MLP shapes (d=64): forward [B,128]x[128,320],
+"""Times the wgmma TF32 GEMM on NeuMF's MLP shapes (d=64): forward [B,128]x[128,320],
 [B,320]x[320,128], [B,128]x[128,64] and the backward-data products, B = 5*batch_size samples."""
 import json
 import os

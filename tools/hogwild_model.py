@@ -2,7 +2,7 @@
 """CPU model of the fused kernel's parallelism at BASELINE config 2 (what the GPU parity numbers should look like).
 
 Triples are visited in the order the kernel's 7104 lane groups retire them; the item rows of a WINDOW of 4 x 7104
-triples (the rows a lane group has in flight, DESIGN.md section 4) are read before any of the window's item deltas
+triples (the rows a lane group has in flight) are read before any of the window's item deltas
 land (stale reads), P[u] is sequential inside a lane group as in the kernel, item deltas are summed at the end of
 the window.  float64, so what is measured is the schedule, not rounding.  Build-container result (about 4 min):
     loss rel 4.7e-06 | P max-norm rel 1.6e-03, rms err / rms update 1.8 % | Q max-norm rel 6.3e-03, 2.4 %

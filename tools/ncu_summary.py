@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Condenses `ncu -i X.ncu-rep --page raw --csv` exports into the handful of numbers profiles/README.md quotes.
+"""Condenses `ncu -i X.ncu-rep --page raw --csv` exports into a handful of summary numbers.
     python tools/ncu_summary.py gpurun_out/r2/*_raw.csv [--json out.json]"""
 import csv
 import json
