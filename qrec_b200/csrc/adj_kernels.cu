@@ -155,14 +155,7 @@ scan_add_kernel(long long* __restrict__ x, long long n, const long long* __restr
   if (blockIdx.x > 0 && k < n) x[k] += block_sums[blockIdx.x - 1];
 }
 
-int grid_rows(long long n_rows) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long blocks = (n_rows + 7) / 8;
-  const long long cap = (long long)sms * 8;
-  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
-}
+int grid_rows(long long n_rows) { return qrec::capped_grid((n_rows + 7) / 8, 8); }
 
 }  // namespace
 

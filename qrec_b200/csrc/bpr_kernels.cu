@@ -21,36 +21,14 @@
 #include <cstdlib>
 
 #include "common.h"
+#include "device.cuh"
 #include "philox.cuh"
 #include "bpr_step.cuh"
 
 namespace {
 
+using namespace qrec;
 using namespace qrec::bpr;
-
-// ------------------------------------------------------------------------------------------
-// helpers
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
-  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y),
-               "f"(v.z), "f"(v.w)
-               : "memory");
-}
-
-template <typename T>
-__device__ __forceinline__ T warp_sum(T v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // ------------------------------------------------------------------------------------------
 // parity mode
@@ -130,23 +108,7 @@ bpr_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
 // ------------------------------------------------------------------------------------------
 // throughput mode
 // ------------------------------------------------------------------------------------------
-// Throughput kernels: sigmoid and -ln(s) on the SFU (ex2.approx / lg2.approx / rcp.approx).  The
-// relative error (~2^-21) is far below the fp32 rounding of the row update it scales; parity mode
-// keeps expf/logf.
-__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-__device__ __forceinline__ float fast_neg_log(float s) { return -__logf(s); }
-
-template <int LPR>
-__device__ __forceinline__ float group_sum(float v) {
-#pragma unroll
-  for (int o = LPR / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ float dot4(float4 a, float4 b) {
-  return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
-}
-
+// sigmoid and -ln(s) on the SFU (fast_sigmoid / fast_neg_log, device.cuh); parity mode keeps expf/logf.
 template <int LPR, int VPL, int UNROLL>
 __global__ void __launch_bounds__(256)
 bpr_sgd_batch_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec, long long n,
@@ -223,15 +185,7 @@ bpr_sgd_batch_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec, lon
     }
   }
   // block reduction of the loss: one double atomic per block
-  __shared__ float wsum[8];
-  lsum = warp_sum(lsum);
-  if (lane == 0) wsum[threadIdx.x >> 5] = lsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)wsum[w];
-    if (t != 0.0) atomicAdd(loss, t);
-  }
+  block_add_loss(lsum, loss);
 }
 
 
@@ -283,15 +237,7 @@ bpr_sgd_staged_kernel(float* __restrict__ P, int nvec, long long n, const int* _
       *reinterpret_cast<float4*>(D + oj) = dqj;
     }
   }
-  __shared__ float wsum[8];
-  lsum = warp_sum(lsum);
-  if (lane == 0) wsum[threadIdx.x >> 5] = lsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)wsum[w];
-    if (t != 0.0) atomicAdd(loss, t);
-  }
+  block_add_loss(lsum, loss);
 }
 
 
@@ -398,15 +344,7 @@ bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long
     }
   }
   if (l < 3) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all reductions performed
-  __shared__ float wsum[8];
-  lsum = warp_sum(lsum);
-  if (lane == 0) wsum[threadIdx.x >> 5] = lsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)wsum[w];
-    if (t != 0.0) atomicAdd(loss, t);
-  }
+  block_add_loss(lsum, loss);
 }
 
 
@@ -419,13 +357,6 @@ bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long
 // REDG.E.ADD.F32x4 as in the batch kernel.  Per triple: 2 row loads + 2 row REDs instead of 3 + 3.
 // Input: CSR over users (rowptr), i[] / j[] in that order.
 // ------------------------------------------------------------------------------------------
-template <int LPR>
-__device__ __forceinline__ float group_sum_masked(float v, unsigned gmask) {
-#pragma unroll
-  for (int o = LPR / 2; o > 0; o >>= 1) v += __shfl_xor_sync(gmask, v, o);
-  return v;
-}
-
 // Work is cut into chunks of CH consecutive triples of the CSR order; a chunk takes the users whose first
 // triple lies inside it, so every user is processed whole by one lane group (P[u] register-resident,
 // updated sequentially, one row RED at the end) -- except at the ends of the launch, which are cut
@@ -435,14 +366,7 @@ __device__ __forceinline__ float group_sum_masked(float v, unsigned gmask) {
 // to the summation order of the float REDs, and an item row is read at most about one wave late.
 // SAMPLE: the negatives are drawn inside the kernel (lane l draws the negative of triple base+l with
 // the same Philox counter as the stand-alone sampler, so both give identical j) instead of being
-// read from j[]; they are optionally written to j_out.
-struct FusedSampler {
-  const long long* rated_rowptr;   // rejection sets: CSR over users, sorted columns
-  const int* rated_cols;
-  int num_items;
-  uint32_t seed_lo, seed_hi, epoch;
-  int* j_out;                      // may be null
-};
+// read from j[] (FusedSampler, philox.cuh); they are optionally written to j_out.
 
 // SIG: the sampler pre-tests every draw against the user's 512-bit rated signature (philox.cuh).
 template <int LPR, int G, int CH, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>   // FULL: d == 4*LPR (every lane owns a slice)
@@ -559,7 +483,7 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const flo
               p0 = p;
             }
             float x = dot4(p, qi[f]) - dot4(p, qj[f]);
-            x = group_sum_masked<LPR>(x, gmask);
+            x = group_sum<LPR>(x, gmask);
             const float s = fast_sigmoid(x);
             const float g = lr * (1.0f - s);
             if (l == 0) lsum += fast_neg_log(s);
@@ -575,15 +499,7 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const flo
     }
     if (act) red_add_v4(prow, make_float4(p.x - p0.x, p.y - p0.y, p.z - p0.z, p.w - p0.w));
   }
-  __shared__ float wsum[8];
-  lsum = warp_sum(lsum);
-  if (lane == 0) wsum[threadIdx.x >> 5] = lsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)wsum[w];
-    if (t != 0.0) atomicAdd(loss, t);
-  }
+  block_add_loss(lsum, loss);
 }
 
 // one warp per user: bit (c & 511) of the user's 16-word signature for every rated column c
@@ -630,18 +546,6 @@ sumsq_kernel(const T* __restrict__ x, long long n, double* out) {
   }
 }
 
-int sm_count() {
-  static int cached[64] = {0};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-  if (cached[dev] == 0) {
-    int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
-    cached[dev] = v;
-  }
-  return cached[dev];
-}
-
 template <typename T>
 int launch_ordered(T* P, T* Q, int d, long long n, const int* u, const int* i, const int* j,
                    const int* wu, const int* wi, const int* wj, int* ver_p, int* ver_q,
@@ -659,12 +563,7 @@ int launch_ordered(T* P, T* Q, int d, long long n, const int* u, const int* i, c
   // n_warps > 0: the caller knows the width of the dependency DAG (qrec_bpr_order_depth) and asks
   // for about that many pollers -- thousands of idle warps hammering the version counters slow the
   // few that can make progress (1.4 independent triples per level on FilmTrust, ~25 at SYN scale)
-  int grid = sm_count() * 2;
-  if (n_warps > 0) {
-    grid = (n_warps + 7) / 8;
-    if (grid < 1) grid = 1;
-    if (grid > sm_count() * 2) grid = sm_count() * 2;
-  }
+  const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
 #define QREC_ORD(E)                                                                              \
   bpr_sgd_ordered_kernel<T, E><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, j, wu, wi, wj, ver_p,     \
                                                      ver_q, ticket, lr, reg_u, reg_i, loss)
@@ -691,9 +590,7 @@ int launch_bpr_batch(float* P, float* Q, int d, long long n, const int* u, const
   QREC_REQUIRE(u && i && j, "bpr_sgd_batch: null index pointer");
   const int nvec = d / 4;
   const long long warps_needed = (n + 31) / 32;
-  const long long blocks_needed = (warps_needed + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;  // 8 CTAs x 8 warps per SM, grid-stride beyond
-  const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
+  const int grid = capped_grid((warps_needed + 7) / 8, 8);  // 8 CTAs x 8 warps per SM, grid-stride beyond
 #define QREC_BATCH(LPR, VPL, UN)                                                                \
   bpr_sgd_batch_kernel<LPR, VPL, UN><<<grid, 256, 0, st>>>(P, Q, nvec, n, u, i, j, lr, reg_u,   \
                                                            reg_i, loss)
@@ -756,14 +653,8 @@ int qrec_bpr_sgd_batch_tma_f32(float* P, float* Q, int32_t d, int64_t n, const i
 #define QREC_TMA(MASK, ROWS, CTAS)                                                                \
   {                                                                                               \
     constexpr int smem = 8 * 2 * UN * 2 * ROWS * 64 * 4;                                          \
-    static bool attr_set = false;                                                                 \
-    if (!attr_set) {                                                                              \
-      QREC_CUDA(cudaFuncSetAttribute(bpr_sgd_batch_tma_kernel<UN, MASK>,                          \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, smem));         \
-      attr_set = true;                                                                            \
-    }                                                                                             \
-    const long long cap = (long long)sm_count() * CTAS;                                           \
-    const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);                            \
+    QREC_CUDA(allow_dynamic_smem((const void*)bpr_sgd_batch_tma_kernel<UN, MASK>, smem));         \
+    const int grid = capped_grid(blocks_needed, CTAS);                                            \
     bpr_sgd_batch_tma_kernel<UN, MASK><<<grid, 256, smem, st>>>(P, Q, n, u, i, j, lr, reg_u, reg_i, loss); \
   }
   if (mask == 7) QREC_TMA(7, 3, 2)
@@ -808,12 +699,11 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
     int occ = 3;                                                                                 \
     if (cap_mult > 0) occ = cap_mult;                                                            \
     else if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, KERNEL, 256, 0) != cudaSuccess || occ < 1) occ = 3; \
-    const long long cap = (long long)sm_count() * occ;                                           \
-    if (blocks > cap) blocks = cap;                                                              \
+    const int grid = capped_grid(blocks, occ);                                                   \
     for (long long c0 = 0; c0 < nchunks; c0 += wave) {                                           \
       QREC_CUDA(cudaMemcpyAsync(Qr, Q, q_bytes, cudaMemcpyDeviceToDevice, st));                  \
       const long long c1 = (c0 + wave) < nchunks ? (c0 + wave) : nchunks;                        \
-      KERNEL<<<(int)blocks, 256, 0, st>>>(P, Q, Qr, nvec, n_users, n, c0, c1, reinterpret_cast<const long long*>(rowptr), \
+      KERNEL<<<grid, 256, 0, st>>>(P, Q, Qr, nvec, n_users, n, c0, c1, reinterpret_cast<const long long*>(rowptr), \
                                           i, j, lr, reg_u, reg_i, loss, fs, trip_off, SIGPTR);   \
       QREC_CUDA(cudaGetLastError());                                                             \
       if (c1 < nchunks) qrec::count_launch();                                                    \
@@ -823,7 +713,7 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
 #define QREC_UM(LPR)                                                                             \
   {                                                                                              \
     const long long per_block = 8 * (32 / LPR);                                                  \
-    long long blocks = (nchunks + per_block - 1) / per_block;                                    \
+    const long long blocks = (nchunks + per_block - 1) / per_block;                              \
     if (nvec == LPR && sample && rated_sig != nullptr) {                                         \
       QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<LPR, 4, CH, true, true, 3, true>), rated_sig)     \
     } else if (nvec == LPR && LPR == 16 && variant == 1) {                                       \
@@ -902,10 +792,7 @@ int qrec_rated_signature_build(int32_t n_users, const int64_t* rated_rowptr, con
   QREC_REQUIRE(rated_rowptr && rated_cols && sig, "qrec_rated_signature_build: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   QREC_CUDA(cudaMemsetAsync(sig, 0, (size_t)n_users * qrec::RATED_SIG_WORDS * sizeof(uint32_t), st));
-  long long blocks = ((long long)n_users + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  rated_signature_kernel<<<(int)blocks, 256, 0, st>>>(n_users, reinterpret_cast<const long long*>(rated_rowptr),
+  rated_signature_kernel<<<capped_grid(((long long)n_users + 7) / 8, 8), 256, 0, st>>>(n_users, reinterpret_cast<const long long*>(rated_rowptr),
                                                      rated_cols, sig);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
@@ -933,15 +820,13 @@ int qrec_bpr_sgd_staged_f32(float* P, int32_t d, int64_t n, const int32_t* u, co
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(P && u && pos_i && pos_j && R && D && loss, "qrec_bpr_sgd_staged_f32: null pointer");
   const int nvec = d / 4;
-  const long long cap = (long long)sm_count() * 8;
   cudaStream_t st = (cudaStream_t)stream;
 #define QREC_STAGED(LPR)                                                                        \
   {                                                                                             \
     const long long per_block = 8 * (32 / LPR);                                                 \
-    long long blocks = (n + per_block - 1) / per_block;                                         \
-    if (blocks > cap) blocks = cap;                                                             \
-    bpr_sgd_staged_kernel<LPR><<<(int)blocks, 256, 0, st>>>(P, nvec, n, u, pos_i, pos_j, R, D,  \
-                                                            lr, reg_u, reg_i, loss);            \
+    const int grid = capped_grid((n + per_block - 1) / per_block, 8);                           \
+    bpr_sgd_staged_kernel<LPR><<<grid, 256, 0, st>>>(P, nvec, n, u, pos_i, pos_j, R, D,         \
+                                                     lr, reg_u, reg_i, loss);                   \
   }
   if (nvec <= 4) QREC_STAGED(4)
   else if (nvec <= 8) QREC_STAGED(8)
@@ -956,9 +841,7 @@ int qrec_sumsq_f32(const float* x, int64_t n, double* out, void* stream) {
   QREC_REQUIRE(out && (x || n == 0) && n >= 0, "qrec_sumsq_f32: bad argument");
   if (n == 0) return QREC_OK;
   QREC_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "qrec_sumsq_f32: x not 16-byte aligned");
-  const long long blocks = (n / 4 + 255) / 256 + 1;
-  const long long cap = (long long)sm_count() * 8;
-  sumsq_kernel<float><<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(x, n, out);
+  sumsq_kernel<float><<<capped_grid((n / 4 + 255) / 256 + 1, 8), 256, 0, (cudaStream_t)stream>>>(x, n, out);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -966,9 +849,7 @@ int qrec_sumsq_f32(const float* x, int64_t n, double* out, void* stream) {
 int qrec_sumsq_f64(const double* x, int64_t n, double* out, void* stream) {
   QREC_REQUIRE(out && (x || n == 0) && n >= 0, "qrec_sumsq_f64: bad argument");
   if (n == 0) return QREC_OK;
-  const long long blocks = (n + 255) / 256;
-  const long long cap = (long long)sm_count() * 8;
-  sumsq_kernel<double><<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(x, n, out);
+  sumsq_kernel<double><<<capped_grid((n + 255) / 256, 8), 256, 0, (cudaStream_t)stream>>>(x, n, out);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }

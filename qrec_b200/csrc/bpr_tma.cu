@@ -10,52 +10,18 @@
 // Pipeline per lane group (16 lanes): the rows of the next 4 triples (8 rows, 2 KB) are requested while the current
 // 4 are being computed: two staging slots, two mbarriers, phase bits tracked in registers.
 #include "common.h"
+#include "device.cuh"
 #include "philox.cuh"
 #include "bpr_step.cuh"
 
 namespace {
 
+using namespace qrec;
 using namespace qrec::bpr;
 
 constexpr int LPR = 16, G = 4, CH = 32, ROWS = 2 * G, GROUPS = 16;   // 256 threads = 16 lane groups
 constexpr int STAGE_FLOATS = ROWS * 64;
 
-struct FusedSampler {
-  const long long* rated_rowptr;
-  const int* rated_cols;
-  int num_items;
-  uint32_t seed_lo, seed_hi, epoch;
-  int* j_out;
-};
-
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ float dot4(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
-__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-__device__ __forceinline__ float fast_neg_log(float s) { return -__logf(s); }
-__device__ __forceinline__ float group_sum16(float v, unsigned gmask) {
-#pragma unroll
-  for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(gmask, v, o);
-  return v;
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
 // one 256-byte row: global -> this CTA's shared memory, completion counted on `bar`
 __device__ __forceinline__ void bulk_row_load(float* smem_dst, const float* gsrc, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 256, [%2];"
@@ -174,7 +140,7 @@ bpr_sgd_usermajor_tma_kernel(float* __restrict__ P, float* __restrict__ Q, int n
               p0 = p;
             }
             float x = dot4(p, qi[f]) - dot4(p, qj[f]);
-            x = group_sum16(x, gmask);
+            x = group_sum<LPR>(x, gmask);
             const float s = fast_sigmoid(x);
             const float g = lr * (1.0f - s);
             if (l == 0) lsum += fast_neg_log(s);
@@ -188,17 +154,7 @@ bpr_sgd_usermajor_tma_kernel(float* __restrict__ P, float* __restrict__ Q, int n
     }
     red_add_v4(prow, make_float4(p.x - p0.x, p.y - p0.y, p.z - p0.z, p.w - p0.w));
   }
-  __shared__ float wsum[8];
-  float t = lsum;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-  if (lane == 0) wsum[threadIdx.x >> 5] = t;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double acc = 0.0;
-    for (int w = 0; w < 8; ++w) acc += (double)wsum[w];
-    if (acc != 0.0) atomicAdd(loss, acc);
-  }
+  block_add_loss(lsum, loss);
 }
 
 }  // namespace
@@ -215,22 +171,13 @@ extern "C" int qrec_bpr_epoch_usermajor_tma_f32(float* P, float* Q, int32_t d, i
   QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols, "qrec_bpr_epoch_usermajor_tma_f32: null index pointer");
   QREC_REQUIRE((reinterpret_cast<uintptr_t>(Q) & 15) == 0, "qrec_bpr_epoch_usermajor_tma_f32: Q must be 16-byte aligned");
   constexpr size_t smem = (size_t)GROUPS * 2 * STAGE_FLOATS * 4 + GROUPS * 2 * 8;
-  static bool attr_set = false;
-  if (!attr_set) {
-    QREC_CUDA(cudaFuncSetAttribute(bpr_sgd_usermajor_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long blocks = ((n + CH - 1) / CH + GROUPS - 1) / GROUPS;
+  QREC_CUDA(allow_dynamic_smem((const void*)bpr_sgd_usermajor_tma_kernel<true>, (int)smem));
   int occ = 3;                                       // one sweep over the stream: grid = resident CTAs (see launch_usermajor)
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, bpr_sgd_usermajor_tma_kernel<true>, 256, smem) != cudaSuccess || occ < 1) occ = 3;
-  const long long cap = (long long)sms * occ;
-  if (blocks > cap) blocks = cap;
+  const int grid = capped_grid(((n + CH - 1) / CH + GROUPS - 1) / GROUPS, occ);
   FusedSampler fs = {reinterpret_cast<const long long*>(rated_rowptr), rated_cols, num_items, (uint32_t)seed,
                      (uint32_t)(seed >> 32), epoch, j_out};
-  bpr_sgd_usermajor_tma_kernel<true><<<(int)blocks, 256, smem, (cudaStream_t)stream>>>(
+  bpr_sgd_usermajor_tma_kernel<true><<<grid, 256, smem, (cudaStream_t)stream>>>(
       P, Q, n_users, n, reinterpret_cast<const long long*>(rowptr), i, nullptr, lr, reg_u, reg_i, loss, fs);
   QREC_LAUNCH_CHECK();
   return QREC_OK;

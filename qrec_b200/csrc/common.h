@@ -12,6 +12,15 @@ namespace qrec {
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
 
+// Launch sizing (core.cpp).  sm_count(): SMs of the current device, queried once per device (132, an H100 SXM's,
+// if the query fails).  capped_grid(): `blocks` CTAs, but at most ctas_per_sm per SM and at least one (the
+// kernels are grid-stride loops).
+int sm_count();
+int capped_grid(long long blocks, int ctas_per_sm);
+// Raises `kernel`'s dynamic shared-memory limit to at least `bytes` on the current device.  The limit belongs to
+// the kernel as loaded on each device, so it is set once per (kernel, device); safe to call from several threads.
+cudaError_t allow_dynamic_smem(const void* kernel, int bytes);
+
 inline int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
   set_error("%s failed at %s:%d: %s", what, file, line, cudaGetErrorString(e));
   return QREC_ERR_CUDA;

@@ -1,7 +1,10 @@
-// Error reporting, version string and launch accounting for libqrec.so.
+// Error reporting, version string, launch accounting and launch sizing for libqrec.so.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "common.h"
 
@@ -18,6 +21,37 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+int sm_count() {
+  static std::atomic<int> cached[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  int v = cached[dev].load(std::memory_order_relaxed);
+  if (v == 0) {
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
+    cached[dev].store(v, std::memory_order_relaxed);
+  }
+  return v;
+}
+
+int capped_grid(long long blocks, int ctas_per_sm) {
+  const long long cap = (long long)sm_count() * ctas_per_sm;
+  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+}
+
+cudaError_t allow_dynamic_smem(const void* kernel, int bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, int> granted;   // (kernel, device) -> limit set
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lock(mu);
+  int& have = granted[{kernel, dev}];
+  if (bytes <= have) return cudaSuccess;
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) have = bytes;
+  return e;
+}
 }  // namespace qrec
 
 extern "C" {

@@ -12,21 +12,18 @@
 #include <cmath>
 
 #include "common.h"
+#include "device.cuh"
 #include "philox.cuh"
 
 namespace {
 
 using qrec::philox4x32_10;
+using qrec::red_add_v4;
+using qrec::capped_grid;
+using qrec::sm_count;
 
 __device__ __forceinline__ float u01(uint32_t w) { return (float)(w >> 8) * (1.0f / 16777216.0f); }
 __device__ __forceinline__ float sgn(float x) { return (x > 0.f) ? 1.f : ((x < 0.f) ? -1.f : 0.f); }
-
-int sm_count() {
-  int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
-  return v;
-}
 
 // one warp per row, lanes stride over float4 slices (d multiple of 4, any size)
 __global__ void __launch_bounds__(256)
@@ -395,8 +392,7 @@ scatter_add_rows_kernel(float* __restrict__ G, const int* __restrict__ idx, long
     if (row < 0) continue;                                // empty slot
     float4 x = *reinterpret_cast<const float4*>(src + (size_t)b * ld_src + v * 4);
     x.x *= scale; x.y *= scale; x.z *= scale; x.w *= scale;
-    float* dst = G + (size_t)row * nvec * 4 + v * 4;
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(x.x), "f"(x.y), "f"(x.z), "f"(x.w) : "memory");
+    red_add_v4(G + (size_t)row * nvec * 4 + v * 4, x);
   }
 }
 
@@ -544,13 +540,7 @@ mask_rated_kernel(float* __restrict__ scores, int n_rows, long long ld, const in
   }
 }
 
-inline int grid_for(long long work_items, int per_block) {
-  long long blocks = (work_items + per_block - 1) / per_block;
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
+inline int grid_for(long long work_items, int per_block) { return capped_grid((work_items + per_block - 1) / per_block, 8); }
 
 }  // namespace
 

@@ -18,36 +18,11 @@
 #include <cstdlib>
 
 #include "common.h"
+#include "device.cuh"
 
 namespace {
 
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y),
-               "f"(v.z), "f"(v.w)
-               : "memory");
-}
-
-template <int LPR>
-__device__ __forceinline__ float group_sum(float v) {
-#pragma unroll
-  for (int o = LPR / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ float dot4(float4 a, float4 b) {
-  return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
-}
-__device__ __forceinline__ void fma4(float4& acc, float s, float4 x) {
-  acc.x = fmaf(s, x.x, acc.x); acc.y = fmaf(s, x.y, acc.y);
-  acc.z = fmaf(s, x.z, acc.z); acc.w = fmaf(s, x.w, acc.w);
-}
-
-int sm_count() {
-  int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
-  return v;
-}
+using namespace qrec;
 
 // ------------------------------------------------------------------------------------------ K2
 template <int LPR, int VPL>
@@ -470,16 +445,7 @@ bpr_grad_scatter_kernel(const float* __restrict__ U, const float* __restrict__ V
       }
     }
   }
-  __shared__ float wsum[8];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
-  if (lane == 0) wsum[threadIdx.x >> 5] = lsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)wsum[w];
-    if (t != 0.0) atomicAdd(loss, t);
-  }
+  block_add_loss(lsum, loss);
 }
 
 // ------------------------------------------------------------------------------------------ K4
@@ -553,14 +519,12 @@ int qrec_spmm_csr_f32(int32_t n_rows, int64_t nnz, const int64_t* rowptr, const 
   if (nnz == 0) return QREC_OK;
   QREC_REQUIRE(cols && vals, "qrec_spmm_csr_f32: null cols/vals");
   const int nvec = d / 4;
-  const long long cap = (long long)sm_count() * 8;
   constexpr int QN = 1024;
 #define QREC_SPMMB(LPR, VPL)                                                                     \
   {                                                                                              \
     const long long groups_per_block = 8 * (32 / LPR);                                           \
-    long long blocks = ((nnz + QN - 1) / QN + groups_per_block - 1) / groups_per_block;          \
-    if (blocks > cap) blocks = cap;                                                              \
-    spmm_csr_balanced_kernel<LPR, VPL, QN><<<(int)blocks, 256, 0, st>>>(                         \
+    const int grid = capped_grid(((nnz + QN - 1) / QN + groups_per_block - 1) / groups_per_block, 8); \
+    spmm_csr_balanced_kernel<LPR, VPL, QN><<<grid, 256, 0, st>>>(                                \
         n_rows, nnz, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale); \
   }
   if (nvec <= 4) QREC_SPMMB(4, 1)
@@ -594,13 +558,11 @@ int qrec_spmm_csr_rowsplit_f32(int32_t n_rows, int64_t nnz, const int64_t* rowpt
   }
   const int nvec = d / 4;
   cudaStream_t st = (cudaStream_t)stream;
-  const long long cap = (long long)sm_count() * 8;
 #define QREC_SPMM(LPR, VPL)                                                                      \
   {                                                                                              \
     const long long groups_per_block = 8 * (32 / LPR);                                           \
-    long long blocks = (n_rows + groups_per_block - 1) / groups_per_block;                       \
-    if (blocks > cap) blocks = cap;                                                              \
-    spmm_csr_kernel<LPR, VPL><<<(int)blocks, 256, 0, st>>>(                                      \
+    const int grid = capped_grid((n_rows + groups_per_block - 1) / groups_per_block, 8);         \
+    spmm_csr_kernel<LPR, VPL><<<grid, 256, 0, st>>>(                                             \
         n_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale); \
   }
   if (nvec <= 4) QREC_SPMM(4, 1)
@@ -627,13 +589,11 @@ int qrec_spmm_csr_scatter_rows_f32(int32_t n_rows, int32_t n_src, const int32_t*
   if (n_src == 0) return QREC_OK;
   QREC_REQUIRE(src_rows && cols && vals, "qrec_spmm_csr_scatter_rows_f32: null index pointer");
   const int nvec = d / 4;
-  const long long cap = (long long)sm_count() * 8;
 #define QREC_SCAT(LPR)                                                                           \
   {                                                                                              \
     const long long per_block = 8 * (32 / LPR);                                                  \
-    long long blocks = ((long long)n_src * 64 + per_block - 1) / per_block;                      \
-    if (blocks > cap) blocks = cap;                                                              \
-    spmm_scatter_rows_kernel<LPR><<<(int)blocks, 256, 0, st>>>(                                  \
+    const int grid = capped_grid(((long long)n_src * 64 + per_block - 1) / per_block, 8);        \
+    spmm_scatter_rows_kernel<LPR><<<grid, 256, 0, st>>>(                                         \
         n_src, src_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale); \
   }
   if (nvec <= 4) QREC_SCAT(4)
@@ -655,13 +615,11 @@ int qrec_spmm_csr_rows_f32(int32_t n_list, const int32_t* rows, const int64_t* r
   QREC_REQUIRE(aligned16(X) && (!Y || aligned16(Y)) && (!acc || aligned16(acc)),
                "qrec_spmm_csr_rows_f32: matrices must be 16-byte aligned");
   const int nvec = d / 4;
-  const long long cap = (long long)sm_count() * 8;
-  long long blocks = ((long long)n_list + 7) / 8;          // one warp per listed row, 8 warps per block
-  if (blocks > cap) blocks = cap;
+  const int grid = capped_grid(((long long)n_list + 7) / 8, 8);   // one warp per listed row, 8 warps per block
   cudaStream_t st = (cudaStream_t)stream;
 #define QREC_LIST(LPR)                                                                                     \
-  spmm_list_rows_kernel<LPR><<<(int)blocks, 256, 0, st>>>(n_list, rows, reinterpret_cast<const long long*>(rowptr), \
-                                                          cols, vals, X, Y, compact, nvec, acc, acc_scale)
+  spmm_list_rows_kernel<LPR><<<grid, 256, 0, st>>>(n_list, rows, reinterpret_cast<const long long*>(rowptr), \
+                                                   cols, vals, X, Y, compact, nvec, acc, acc_scale)
   if (nvec <= 4) QREC_LIST(4);
   else if (nvec <= 8) QREC_LIST(8);
   else if (nvec <= 16) QREC_LIST(16);
@@ -681,9 +639,7 @@ int qrec_bpr_grad_scatter_f32(const float* U, const float* V, int32_t d, int64_t
   QREC_REQUIRE(aligned16(U) && aligned16(V) && aligned16(gU) && aligned16(gV),
                "qrec_bpr_grad_scatter_f32: tables must be 16-byte aligned");
   const int nvec = d / 4;
-  const long long blocks_needed = ((n + 31) / 32 + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;
-  const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
+  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
   cudaStream_t st = (cudaStream_t)stream;
 #define QREC_K3(LPR, VPL, UN)                                                                    \
   bpr_grad_scatter_kernel<LPR, VPL, UN><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, eps, reg,  \
@@ -708,9 +664,7 @@ int qrec_bpr_grad_scatter_scaled_f32(const float* U, const float* V, int32_t d, 
   QREC_REQUIRE(aligned16(U) && aligned16(V) && aligned16(gU) && aligned16(gV),
                "qrec_bpr_grad_scatter_scaled_f32: tables must be 16-byte aligned");
   const int nvec = d / 4;
-  const long long blocks_needed = ((n + 31) / 32 + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;
-  const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
+  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
   cudaStream_t st = (cudaStream_t)stream;
 #define QREC_K3S(LPR, VPL, UN)                                                                      \
   bpr_grad_scatter_kernel<LPR, VPL, UN><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, eps, reg, gU, \
@@ -733,9 +687,7 @@ int qrec_bpr_partial_scores_f32(const float* U, const float* V, int32_t d, int64
   QREC_REQUIRE(U && V && u && i && j && y_part && loss, "qrec_bpr_partial_scores_f32: null pointer");
   QREC_REQUIRE(aligned16(U) && aligned16(V), "qrec_bpr_partial_scores_f32: tables must be 16-byte aligned");
   const int nvec = d / 4;
-  const long long blocks_needed = ((n + 31) / 32 + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;
-  const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
+  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
   cudaStream_t st = (cudaStream_t)stream;
 #define QREC_K3P(LPR, VPL, UN)                                                                   \
   bpr_grad_scatter_kernel<LPR, VPL, UN, 1><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, 0.f, reg, nullptr, nullptr, loss, y_part, 0.f)
@@ -759,9 +711,7 @@ int qrec_bpr_grad_from_scores_f32(const float* U, const float* V, int32_t d, int
   QREC_REQUIRE(aligned16(U) && aligned16(V) && aligned16(gU) && aligned16(gV),
                "qrec_bpr_grad_from_scores_f32: tables must be 16-byte aligned");
   const int nvec = d / 4;
-  const long long blocks_needed = ((n + 31) / 32 + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;
-  const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
+  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
   cudaStream_t st = (cudaStream_t)stream;
   float* yb = const_cast<float*>(y_full);
 #define QREC_K3A(LPR, VPL, UN)                                                                   \
@@ -787,9 +737,7 @@ int qrec_adam_dense_tf1_f32(float* var, float* m, float* v, const float* g, int6
   // a running fp32 product, which differs in the last bits only)
   const float b1p = (float)pow((double)beta1, (double)t), b2p = (float)pow((double)beta2, (double)t);
   const float lr_t = lr * sqrtf(1.0f - b2p) / (1.0f - b1p);
-  const long long blocks = (n / 4 + 255) / 256 + 1;
-  const long long cap = (long long)sm_count() * 8;
-  adam_dense_tf1_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(
+  adam_dense_tf1_kernel<<<capped_grid((n / 4 + 255) / 256 + 1, 8), 256, 0, (cudaStream_t)stream>>>(
       var, m, v, g, n, lr_t, beta1, beta2, eps, nullptr);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
@@ -802,9 +750,7 @@ int qrec_adam_dense_tf1_devstep_f32(float* var, float* m, float* v, const float*
   QREC_REQUIRE(var && m && v && g && dev_lr_t, "qrec_adam_dense_tf1_devstep_f32: null pointer");
   QREC_REQUIRE(aligned16(var) && aligned16(m) && aligned16(v) && aligned16(g),
                "qrec_adam_dense_tf1_devstep_f32: buffers must be 16-byte aligned");
-  const long long blocks = (n / 4 + 255) / 256 + 1;
-  const long long cap = (long long)sm_count() * 8;
-  adam_dense_tf1_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(
+  adam_dense_tf1_kernel<<<capped_grid((n / 4 + 255) / 256 + 1, 8), 256, 0, (cudaStream_t)stream>>>(
       var, m, v, g, n, 0.f, beta1, beta2, eps, dev_lr_t);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
@@ -816,9 +762,7 @@ int qrec_axpby_f32(float* dst, const float* a, const float* b, float alpha, floa
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(dst && a && b, "qrec_axpby_f32: null pointer");
   QREC_REQUIRE(aligned16(dst) && aligned16(a) && aligned16(b), "qrec_axpby_f32: buffers must be 16-byte aligned");
-  const long long blocks = (n / 4 + 255) / 256 + 1;
-  const long long cap = (long long)sm_count() * 8;
-  axpby_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(dst, a, b, alpha, beta, n);
+  axpby_kernel<<<capped_grid((n / 4 + 255) / 256 + 1, 8), 256, 0, (cudaStream_t)stream>>>(dst, a, b, alpha, beta, n);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }

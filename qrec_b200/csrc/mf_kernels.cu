@@ -23,30 +23,12 @@
 //   * mf_predict_pairs_kernel -- predictForRating for a list of (u,i) pairs (the per-epoch
 //     rating_performance of iterativeRecommender.py:104-113 without moving the tables).
 #include "common.h"
+#include "device.cuh"
 #include "mf_step.cuh"
 
 namespace {
 
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
-  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y),
-               "f"(v.z), "f"(v.w)
-               : "memory");
-}
-
-template <typename T>
-__device__ __forceinline__ T warp_sum(T v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
+using namespace qrec;
 
 // ------------------------------------------------------------------------------------------
 // parity mode
@@ -127,10 +109,6 @@ mf_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
 // ------------------------------------------------------------------------------------------
 // throughput mode
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float dot4(float4 a, float4 b) {
-  return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
-}
-
 template <int LPR, int KIND, int UNROLL>
 __global__ void __launch_bounds__(256)
 mf_sgd_batch_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec, long long n,
@@ -185,9 +163,7 @@ mf_sgd_batch_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec, long
       }
 #pragma unroll
       for (int f = 0; f < UNROLL; ++f) {
-        float dot = dot4(p[f], q[f]);
-#pragma unroll
-        for (int o = LPR / 2; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+        const float dot = group_sum<LPR>(dot4(p[f], q[f]));
         float pred = dot;
         if (KIND == 2) pred = ((dot + global_mean) + bi[f]) + bu[f];
         const float e = rt[f] - pred;
@@ -212,15 +188,7 @@ mf_sgd_batch_kernel(float* __restrict__ P, float* __restrict__ Q, int nvec, long
       }
     }
   }
-  __shared__ float wsum[8];
-  lsum = warp_sum(lsum);
-  if (lane == 0) wsum[threadIdx.x >> 5] = lsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)wsum[w];
-    if (t != 0.0) atomicAdd(loss, t);
-  }
+  block_add_loss(lsum, loss);
 }
 
 // one warp per pair; out[k] = P[u].Q[i] (+ globalMean + Bi[i] + Bu[u] when Bu != null)
@@ -243,13 +211,6 @@ mf_predict_pairs_kernel(const T* __restrict__ P, const T* __restrict__ Q, int d,
   }
 }
 
-int sm_count() {
-  int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
-  return v;
-}
-
 template <typename T>
 int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const int* i, const T* r,
                    const int* wu, const int* wi, int* ver_p, int* ver_q, unsigned long long* ticket, T lr,
@@ -263,12 +224,7 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && r && wu && wi, "mf_sgd_ordered: null entry pointer");
   const int e = (d + 31) / 32;
-  int grid = sm_count() * 2;
-  if (n_warps > 0) {
-    grid = (n_warps + 7) / 8;
-    if (grid < 1) grid = 1;
-    if (grid > sm_count() * 2) grid = sm_count() * 2;
-  }
+  const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
 #define QREC_MFO(E, K)                                                                                 \
   mf_sgd_ordered_kernel<T, E, K><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, r, wu, wi, ver_p, ver_q,      \
                                                        ticket, lr, reg_u, reg_i, Bu, Bi, reg_b,        \
@@ -296,10 +252,7 @@ int launch_predict(const T* P, const T* Q, int d, long long n, const int* u, con
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(P && Q && u && i && out, "mf_predict_pairs: null pointer");
   QREC_REQUIRE((Bu == nullptr) == (Bi == nullptr), "mf_predict_pairs: give both bias vectors or neither");
-  long long blocks = (n + 7) / 8;
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  mf_predict_pairs_kernel<T><<<(int)blocks, 256, 0, st>>>(P, Q, d, n, u, i, Bu, Bi, global_mean, out);
+  mf_predict_pairs_kernel<T><<<capped_grid((n + 7) / 8, 8), 256, 0, st>>>(P, Q, d, n, u, i, Bu, Bi, global_mean, out);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -340,9 +293,7 @@ int qrec_mf_sgd_batch_f32(int32_t kind, float* P, float* Q, int32_t d, int64_t n
   QREC_REQUIRE(u && i && r, "mf_sgd_batch: null entry pointer");
   cudaStream_t st = (cudaStream_t)stream;
   const int nvec = d / 4;
-  long long blocks = (n + 255) / 256;                    // 32 entries per warp and pass
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
+  long long blocks = capped_grid((n + 255) / 256, 8);    // 32 entries per warp and pass
   if (max_inflight > 0) {
     // a lane group has UNROLL = 4 entries between their row reads and their reductions: bound the
     // number of such entries across the grid (the staleness window of the Hogwild update)

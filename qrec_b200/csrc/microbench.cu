@@ -62,10 +62,7 @@ extern "C" int qrec_ubench_row_ops_f32(float* dev_table, int64_t rows, int64_t n
   QREC_REQUIRE(rows > 0 && rows < (1LL << 32) && n_ops >= 0, "ubench_row_ops: bad sizes");
   QREC_REQUIRE(mode >= 0 && mode <= 2, "ubench_row_ops: mode must be 0 (gather), 1 (reduce) or 2 (both)");
   if (n_ops == 0) return QREC_OK;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = sms * 8;                       // 8 CTAs of 256 threads per SM: full occupancy at <= 32 registers
+  const int grid = qrec::sm_count() * 8;         // 8 CTAs of 256 threads per SM: full occupancy at <= 32 registers
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (mode == 0) row_op_kernel<0, 8><<<grid, 256, 0, st>>>(dev_table, (uint32_t)rows, n_ops, seed, dev_sink);
   else if (mode == 1) row_op_kernel<1, 8><<<grid, 256, 0, st>>>(dev_table, (uint32_t)rows, n_ops, seed, dev_sink);

@@ -78,4 +78,14 @@ __device__ __forceinline__ int sample_negative_sig(long long k, uint32_t epoch, 
   }
 }
 
+// Arguments of the negatives drawn inside the fused user-major kernels (bpr_kernels.cu, bpr_tma.cu): the rejection
+// sets, the Philox key and epoch of sample_negative(), and where to write the drawn j (may be null).
+struct FusedSampler {
+  const long long* rated_rowptr;   // rejection sets: CSR over users, sorted columns
+  const int* rated_cols;
+  int num_items;
+  uint32_t seed_lo, seed_hi, epoch;
+  int* j_out;
+};
+
 }  // namespace qrec

@@ -12,15 +12,13 @@
 //   6  variant 0 + L2 residency hints: (col, val) streamed (L2::evict_first, no L1 allocation), X rows evict_last
 // Reached only through qrec_spmm_csr_rowsplit_var_f32 (tests/test_gpu_spmm_variants.py, tools/bench_graph.py).
 #include "common.h"
+#include "device.cuh"
 
 namespace {
 
-constexpr int LPR = 16;   // lanes per row: d = 64, one float4 per lane
+using qrec::fma4;
 
-__device__ __forceinline__ void fma4(float4& acc, float s, float4 x) {
-  acc.x = fmaf(s, x.x, acc.x); acc.y = fmaf(s, x.y, acc.y);
-  acc.z = fmaf(s, x.z, acc.z); acc.w = fmaf(s, x.w, acc.w);
-}
+constexpr int LPR = 16;   // lanes per row: d = 64, one float4 per lane
 
 __device__ __forceinline__ void store_row(float* __restrict__ Y, float* __restrict__ acc, float acc_scale, long long r,
                                           int l, float4 a) {
@@ -195,13 +193,6 @@ spmm_rowsplit_pipe_kernel(int n_rows, const long long* __restrict__ rowptr, cons
   }
 }
 
-int sm_count() {
-  int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
-  return v;
-}
-
 }  // namespace
 
 extern "C" int qrec_spmm_csr_rowsplit_var_f32(int32_t variant, int32_t n_rows, const int64_t* rowptr,
@@ -216,11 +207,9 @@ extern "C" int qrec_spmm_csr_rowsplit_var_f32(int32_t variant, int32_t n_rows, c
   QREC_REQUIRE(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(acc)) & 15) == 0,
                "qrec_spmm_csr_rowsplit_var_f32: tables must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  long long blocks = ((long long)n_rows + 15) / 16;      // 16 lane groups (rows) per 256-thread block
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
+  const int grid = qrec::capped_grid(((long long)n_rows + 15) / 16, 8);   // 16 lane groups (rows) per 256-thread block
   const long long* rp = reinterpret_cast<const long long*>(rowptr);
-#define QREC_VAR(KERNEL) KERNEL<<<(int)blocks, 256, 0, st>>>(n_rows, rp, cols, vals, X, Y, acc, acc_scale)
+#define QREC_VAR(KERNEL) KERNEL<<<grid, 256, 0, st>>>(n_rows, rp, cols, vals, X, Y, acc, acc_scale)
   switch (variant) {
     case 0: QREC_VAR((spmm_rowsplit_batch_kernel<8, 4>)); break;
     case 1: QREC_VAR((spmm_rowsplit_batch_kernel<8, 5>)); break;

@@ -17,15 +17,15 @@
 // rank reads the summed slices from their owners and applies them).  All kernels here are built to
 // co-reside with K1 (128 threads, <= 32 registers: K1 leaves 4096 registers per SM free at 3 CTAs/SM).
 #include "common.h"
+#include "device.cuh"
 
 namespace {
+
+using qrec::red_add_v4;
 
 constexpr int kMaxPeers = 16;
 struct PeerPtrs { const float* p[kMaxPeers]; };
 
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
 // peer data is written by another GPU between launches: bypass L1, read at system scope
 __device__ __forceinline__ float4 ld_peer_v4(const float* p) {
   float4 v;
@@ -101,14 +101,7 @@ table_all_gather_kernel(PeerPtrs peers_S, int world, long long slice4, float4* _
   }
 }
 
-int grid_for(long long n4) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long blocks = (n4 + 127) / 128;
-  const long long cap = (long long)sms * 4;
-  return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
-}
+int grid_for(long long n4) { return qrec::capped_grid((n4 + 127) / 128, 4); }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

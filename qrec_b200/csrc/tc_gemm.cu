@@ -14,31 +14,18 @@
 //     ReLU-mask applied.
 // Tile: 128 x 64 per CTA, 128 threads.
 #include "common.h"
+#include "device.cuh"
 #include "wgmma.cuh"
 
 namespace {
 
+using qrec::smem_u32;
+using wg::sw_off;
+using wg::to_tf32;
+
 constexpr int BM = 128, BN = 64, BK = 32;           // BK fp32 = 128 B = one swizzle span
 constexpr int STAGE_A = BM * 128, STAGE_B = BN * 128;
 constexpr int SMEM_BYTES = 2 * (STAGE_A + STAGE_B) + 1024;   // + alignment slack
-
-// byte offset of element (row, k) inside a K-major SWIZZLE_128B tile (k in [0,32) fp32)
-__device__ __forceinline__ uint32_t sw_off(int row, int k) {
-  const int chunk = (k >> 2) ^ (row & 7);
-  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + chunk * 16 + (k & 3) * 4);
-}
-
-// The tensor cores read the top 19 bits of each fp32 operand, i.e. truncate.  Rounding to
-// nearest-away while staging removes the systematic toward-zero bias (2^-11 unbiased instead of up
-// to 2^-10 one-sided per operand), which matters over the 6-GEMM forward/backward chain of the MLP.
-__device__ __forceinline__ float to_tf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-__device__ __forceinline__ float4 to_tf32(float4 v) {
-  return make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
-}
 
 enum Epilogue { EPI_NONE = 0, EPI_BIAS_RELU = 1, EPI_RELU_MASK = 2, EPI_BIAS = 3 };
 
@@ -120,7 +107,7 @@ tc_gemm_tf32_kernel(int M, int N, int K, const float* __restrict__ A, int lda,
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> async proxy (wgmma)
     __syncthreads();
     wg::fence();
-    const uint64_t da = wg::desc_sw128(wg::smem_u32(sA_s)), db = wg::desc_sw128(wg::smem_u32(sB_s));
+    const uint64_t da = wg::desc_sw128(smem_u32(sA_s)), db = wg::desc_sw128(smem_u32(sB_s));
 #pragma unroll
     for (int k4 = 0; k4 < BK / 8; ++k4) {                              // +2 = 32 bytes (8 tf32) along K
       wg::mma_m64n64k8_tf32(acc[0], da + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), 1u);
@@ -198,12 +185,8 @@ extern "C" int qrec_tc_gemm_tf32(int32_t b_is_nk, int32_t M, int32_t N, int32_t 
   QREC_REQUIRE(epilogue >= 0 && epilogue <= 3, "qrec_tc_gemm_tf32: unknown epilogue %d", epilogue);
   QREC_REQUIRE((epilogue != EPI_BIAS_RELU && epilogue != EPI_BIAS) || bias, "qrec_tc_gemm_tf32: bias epilogue without bias");
   QREC_REQUIRE(epilogue != EPI_RELU_MASK || mask, "qrec_tc_gemm_tf32: mask epilogue without mask");
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[b_is_nk ? 1 : 0]) {
-    if (b_is_nk) QREC_CUDA(cudaFuncSetAttribute(tc_gemm_tf32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    else QREC_CUDA(cudaFuncSetAttribute(tc_gemm_tf32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set[b_is_nk ? 1 : 0] = true;
-  }
+  QREC_CUDA(qrec::allow_dynamic_smem(b_is_nk ? (const void*)tc_gemm_tf32_kernel<true> : (const void*)tc_gemm_tf32_kernel<false>,
+                                      SMEM_BYTES));
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
   cudaStream_t st = (cudaStream_t)stream;
   if (b_is_nk) tc_gemm_tf32_kernel<true><<<grid, 128, SMEM_BYTES, st>>>(M, N, K, A, lda, B, ldb, C, ldc, epilogue, bias, mask, ldmask);

@@ -19,9 +19,14 @@
 #include <cuda.h>
 
 #include "common.h"
+#include "device.cuh"
 #include "wgmma.cuh"
 
 namespace {
+
+using namespace qrec;
+using wg::sw_off;
+using wg::to_tf32;
 
 constexpr int BM = 128, BN = 64, BK = 32;           // BK fp32 = 128 B = one swizzle span
 constexpr int NSTAGE = 4;
@@ -32,27 +37,6 @@ constexpr int EPI_PITCH = BN + 4;                   // floats; 272-byte rows
 constexpr int EPI_BYTES = BM * EPI_PITCH * 4;
 constexpr int NTHREADS = 160;                       // the consumer warpgroup + the producer warp
 
-using wg::smem_u32;
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
@@ -61,16 +45,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
 }
 __device__ __forceinline__ void group_sync() {     // the 128 threads of the consumer warpgroup
   asm volatile("bar.sync 1, 128;" ::: "memory");
-}
-
-__device__ __forceinline__ uint32_t sw_off(int row, int k) {   // (row, k) inside a K-major SWIZZLE_128B tile
-  const int chunk = (k >> 2) ^ (row & 7);
-  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + chunk * 16 + (k & 3) * 4);
-}
-__device__ __forceinline__ float to_tf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
 }
 
 enum Epilogue { EPI_NONE = 0, EPI_BIAS_RELU = 1, EPI_RELU_MASK = 2, EPI_BIAS = 3 };
@@ -113,7 +87,7 @@ tc_gemm_tf32_v2_kernel(const __grid_constant__ CUtensorMap mapA, int M, int N, i
         const int gn = n0 + row, gk = k0 + c * 4;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (gn < N && gk < K) v = __ldg(reinterpret_cast<const float4*>(B + (size_t)gn * ldb + gk));
-        *reinterpret_cast<float4*>(dst + sw_off(row, c * 4)) = make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
+        *reinterpret_cast<float4*>(dst + sw_off(row, c * 4)) = to_tf32(v);
       }
     } else {                                         // B [K,N] row-major: transposed on the way in
       for (int e = tid; e < BN * BK; e += NTHREADS) {
@@ -230,13 +204,6 @@ EncodeTiledFn encode_tiled() {
   return fn;
 }
 
-int sm_count() {
-  int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
-  return v;
-}
-
 }  // namespace
 
 extern "C" int qrec_tc_gemm_tf32_v2(int32_t b_is_nk, int32_t M, int32_t N, int32_t K, const float* A,
@@ -274,8 +241,7 @@ extern "C" int qrec_tc_gemm_tf32_v2(int32_t b_is_nk, int32_t M, int32_t N, int32
   if (ctas_per_n < 1) ctas_per_n = 1;
   const int nkb = (K + BK - 1) / BK;
   const int smem = NSTAGE * STAGE_A + nkb * KB_B + EPI_BYTES + 1024;
-  if (b_is_nk) QREC_CUDA(cudaFuncSetAttribute(tc_gemm_tf32_v2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  else QREC_CUDA(cudaFuncSetAttribute(tc_gemm_tf32_v2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  QREC_CUDA(allow_dynamic_smem(b_is_nk ? (const void*)tc_gemm_tf32_v2_kernel<true> : (const void*)tc_gemm_tf32_v2_kernel<false>, smem));
   const int grid = n_blocks * ctas_per_n;
   cudaStream_t st = (cudaStream_t)stream;
   if (b_is_nk)

@@ -15,51 +15,14 @@
 // earlier item: strict `>`), and makes the order among equal scores deterministic (the heap's is an
 // implementation detail of heapq).
 #include "common.h"
+#include "topn.cuh"
 
 namespace {
 
+using namespace qrec;
+
 constexpr int CAP = 256;   // candidate slots per user (>= N_max + items per tile)
 constexpr int NMAX = 100;  // base/recommender.py:131-134 clamps N to <= 100
-
-__device__ __forceinline__ uint32_t ord_of(float s) {          // monotone float -> uint
-  const uint32_t u = __float_as_uint(s);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float score_of(uint32_t o) {
-  return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
-}
-__device__ __forceinline__ unsigned long long key_of(float s, int item) {
-  return ((unsigned long long)ord_of(s) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)item);
-}
-
-__device__ __forceinline__ bool is_rated(const int* __restrict__ cols, long long lo, long long hi, int item) {
-  while (lo < hi) {
-    const long long mid = (lo + hi) >> 1;
-    const int c = __ldg(cols + mid);
-    if (c == item) return true;
-    if (c < item) lo = mid + 1; else hi = mid;
-  }
-  return false;
-}
-
-// one warp sorts the CAP keys of one row, descending (bitonic network in shared memory)
-__device__ __forceinline__ void warp_sort_desc(unsigned long long* k, int lane) {
-#pragma unroll 1
-  for (int size = 2; size <= CAP; size <<= 1) {
-#pragma unroll 1
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncwarp();
-      for (int t = lane; t < CAP / 2; t += 32) {
-        const int lo = 2 * t - (t & (stride - 1));           // index of the lower partner
-        const int hi = lo + stride;
-        const bool desc = (lo & size) == 0;
-        const unsigned long long a = k[lo], b = k[hi];
-        if ((a < b) == desc) { k[lo] = b; k[hi] = a; }
-      }
-    }
-  }
-  __syncwarp();
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // The kernel: 128 users x 128 items per tile, 8 x 8 register tile per thread, double-buffered k-chunks of 16
@@ -106,7 +69,7 @@ score_topn_kernel(const float* __restrict__ U, const float* __restrict__ V, int 
       if (c > CAP - VN) {
         unsigned long long* k = scratch[warp];
         for (int t = lane; t < CAP; t += 32) k[t] = t < c ? __ldcg(cand + (size_t)r * CAP + t) : 0ULL;
-        warp_sort_desc(k, lane);
+        warp_sort_desc<CAP>(k, lane);
         for (int t = lane; t < N; t += 32) cand[(size_t)r * CAP + t] = k[t];
         if (lane == 0) { cnt[r] = N; thr[r] = k[N - 1]; }
         __syncwarp();
@@ -191,7 +154,7 @@ score_topn_kernel(const float* __restrict__ U, const float* __restrict__ V, int 
     const int c = cnt[r];
     unsigned long long* k = scratch[warp];
     for (int t = lane; t < CAP; t += 32) k[t] = t < c ? __ldcg(cand + (size_t)r * CAP + t) : 0ULL;
-    warp_sort_desc(k, lane);
+    warp_sort_desc<CAP>(k, lane);
     for (int t = lane; t < N; t += 32) {
       const unsigned long long key = k[t];
       out_ids[(size_t)(row0 + r) * N + t] = (int)(0xffffffffu - (uint32_t)(key & 0xffffffffULL));

@@ -2,8 +2,8 @@
 // top-N").  Same contract and same selection rule as csrc/topn_kernels.cu (the reference flow of
 // base/recommender.py:143-152 + util/qmath.py:134-146); what changes is where the scores come from:
 //
-//   * a CTA owns 128 users.  Their rows of U are split once into two TF32 operands, hi = rna_tf32(x) and
-//     lo = rna_tf32(x - hi), stored K-major / SWIZZLE_128B in shared memory (the layout of csrc/tc_gemm.cu);
+//   * a CTA owns 128 users.  Their rows of U are split once into two TF32 operands, hi = to_tf32(x) and
+//     lo = to_tf32(x - hi) (csrc/wgmma.cuh), stored K-major / SWIZZLE_128B in shared memory (the layout of csrc/tc_gemm.cu);
 //   * the item table is split the same way ONCE per call by a small pre-pass (split_items_kernel) that writes each
 //     128-item tile as one contiguous block already in the shared-memory layout; the main kernel streams those blocks
 //     through a 2-stage ring with cp.async.bulk (one 64 KB bulk copy per tile, completion on an mbarrier) -- no
@@ -26,9 +26,15 @@
 //     tile streams in during the selection.
 // Nothing of the [users x items] matrix is written.  d <= 64, a multiple of 4 (one or two 128-byte k-blocks, zero-padded).
 #include "common.h"
+#include "device.cuh"
+#include "topn.cuh"
 #include "wgmma.cuh"
 
 namespace {
+
+using namespace qrec;
+using wg::sw_off;
+using wg::to_tf32;
 
 constexpr int CAP = 320;   // candidate slots per half-row list (>= N_max + TRIG_EXTRA + the 64 items a tile can add)
 constexpr int TRIG_EXTRA = 96;   // a list is cut back to its N best once it holds more than N + TRIG_EXTRA keys
@@ -40,65 +46,6 @@ constexpr int TM = 128, TN = 128;
 constexpr int KBLK = TM * 128;                       // bytes of one k-block (32 fp32 = 128 B per row) of a 128-row operand
 constexpr int SP = TN + 4;                           // row pitch (floats) of a warpgroup's score tile: conflict-free row reads
 
-__device__ __forceinline__ uint32_t ord_of(float s) {          // monotone float -> uint
-  const uint32_t u = __float_as_uint(s);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float score_of(uint32_t o) {
-  return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
-}
-__device__ __forceinline__ bool is_rated(const int* __restrict__ cols, long long lo, long long hi, int item) {
-  while (lo < hi) {
-    const long long mid = (lo + hi) >> 1;
-    const int c = __ldg(cols + mid);
-    if (c == item) return true;
-    if (c < item) lo = mid + 1; else hi = mid;
-  }
-  return false;
-}
-// one warp sorts SZ keys, descending (bitonic network in shared memory)
-template <int SZ>
-__device__ __forceinline__ void warp_sort_desc(unsigned long long* k, int lane) {
-#pragma unroll 1
-  for (int size = 2; size <= SZ; size <<= 1) {
-#pragma unroll 1
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncwarp();
-      for (int t = lane; t < SZ / 2; t += 32) {
-        const int lo = 2 * t - (t & (stride - 1));
-        const int hi = lo + stride;
-        const bool desc = (lo & size) == 0;
-        const unsigned long long a = k[lo], b = k[hi];
-        if ((a < b) == desc) { k[lo] = b; k[hi] = a; }
-      }
-    }
-  }
-  __syncwarp();
-}
-
-using wg::smem_u32;
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-// Bounded wait: a protocol error traps (the launch fails with an error) instead of hanging the device.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  for (uint32_t spins = 0;; ++spins) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (spins > (1u << 22)) __trap();
-  }
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
 // bulk copy global -> shared (TMA engine), completion counted in bytes on `bar`
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -107,20 +54,10 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 __device__ __forceinline__ void group_sync(int group) {     // the 128 threads of one warpgroup
   asm volatile("bar.sync %0, 128;" ::"r"(1 + group) : "memory");
 }
-// byte offset of element (row, k) inside one K-major SWIZZLE_128B k-block (k in [0,32) fp32)
-__device__ __forceinline__ uint32_t sw_off(int row, int k) {
-  const int chunk = (k >> 2) ^ (row & 7);
-  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + chunk * 16 + (k & 3) * 4);
-}
-__device__ __forceinline__ float rna_tf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
 // x = hi + lo with hi, lo representable in TF32 (up to 2^-22 |x|)
 __device__ __forceinline__ void split_tf32(const float4 v, float4& hi, float4& lo) {
-  hi = make_float4(rna_tf32(v.x), rna_tf32(v.y), rna_tf32(v.z), rna_tf32(v.w));
-  lo = make_float4(rna_tf32(v.x - hi.x), rna_tf32(v.y - hi.y), rna_tf32(v.z - hi.z), rna_tf32(v.w - hi.w));
+  hi = to_tf32(v);
+  lo = to_tf32(make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w));
 }
 
 // Pre-pass: tile t of the item table (items [128 t, 128 t + 128), zero rows past the end, zero columns past d) as one
@@ -327,7 +264,7 @@ score_topn_tc_kernel(const float* __restrict__ U, const uint8_t* __restrict__ it
       wg::commit();
       wg::wait<0>();
       __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
+      if (lane == 0) mbar_arrive(&empty[s]);
       group_sync(grp);                                // every warp of the group is done reading the previous tile's scores
       const int w4 = warp & 3;
 #pragma unroll
@@ -432,11 +369,7 @@ int launch_tc(const float* U, const float* V, int d, int n_items, const int* use
               const int* cols, float rated_value, int N, int* out_ids, float* out_scores, cudaStream_t st) {
   constexpr int SMEM = (2 + 2 * (3 - KB)) * KB * KBLK + 8 * SORTN * (int)sizeof(unsigned long long) + SIGW * TM * (int)sizeof(uint32_t) +
                        2 * 64 * SP * (int)sizeof(float) + 1024;   // operands + sort buffers + signatures + score tiles + alignment
-  static bool attr_set = false;
-  if (!attr_set) {
-    QREC_CUDA(cudaFuncSetAttribute(score_topn_tc_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attr_set = true;
-  }
+  QREC_CUDA(allow_dynamic_smem((const void*)score_topn_tc_kernel<KB>, SMEM));
   const int grid = (n_rows + TM - 1) / TM;
   const int n_tiles = (n_items + TN - 1) / TN;
   const size_t list_bytes = (size_t)grid * TM * 2 * CAP * sizeof(unsigned long long);   // candidate lists: 2 x 2.5 KB per user

@@ -10,7 +10,21 @@
 
 namespace wg {
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// byte offset of element (row, k) inside a K-major SWIZZLE_128B tile (k in [0,32) fp32)
+__device__ __forceinline__ uint32_t sw_off(int row, int k) {
+  const int chunk = (k >> 2) ^ (row & 7);
+  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + chunk * 16 + (k & 3) * 4);
+}
+
+// fp32 -> TF32, rounded to nearest (ties away).  The tensor cores read the top 19 bits of an fp32 operand, i.e.
+// truncate; rounding while staging removes that systematic toward-zero bias (2^-11 unbiased instead of up to
+// 2^-10 one-sided per operand).
+__device__ __forceinline__ float to_tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+__device__ __forceinline__ float4 to_tf32(float4 v) { return make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w)); }
 
 // shared-memory matrix descriptor, K-major SWIZZLE_128B: start >> 4 | LBO 16 B (unused by this layout) | SBO 1024 B
 // (one 8-row atom) | layout type 1 (128B swizzle).  The atom must be 1024-byte aligned; a step of 8 tf32 along K is
