@@ -652,6 +652,36 @@ int qrec_mf_predict_pairs_f64(const double* dev_P, const double* dev_Q, int32_t 
                               const int32_t* dev_u, const int32_t* dev_i, const double* dev_Bu,
                               const double* dev_Bi, double global_mean, double* dev_out, void* stream);
 
+/* =====================================================================================
+ * K10 -- WRMF (implicit-feedback ALS, model/ranking/WRMF.py:19-61).  A half-epoch solves every row of one
+ * table X against the other table Z, which it only reads:
+ *   A = Z^T Z + lambda*I + alpha * sum_k v_k z_k z_k^T,   b = sum_k (1 + alpha*v_k) z_k,   X[r] = A^-1 b
+ * over the entries (c_k, v_k) of row r.  A and b are float64 for both table types.  d: 1..128.
+ * ===================================================================================== */
+/* Bytes of device workspace qrec_als_gram_* needs for n rows of width d (0 for n = 0); < 0 on bad arguments. */
+int64_t qrec_als_gram_workspace_bytes(int64_t n, int32_t d);
+/* G[d][d] (float64, row-major, exactly symmetric) = Z^T Z of the table Z[n][d].  Partial Grams of fixed 2048-row
+ * chunks go to the caller's workspace (workspace_bytes >= qrec_als_gram_workspace_bytes(n, d)) and are summed in
+ * chunk order, so G is bitwise the same from run to run and on any H100.  n = 0 gives G = 0. */
+int qrec_als_gram_f32(const float* dev_Z, int64_t n, int32_t d, double* dev_G, void* dev_workspace,
+                      int64_t workspace_bytes, void* stream);
+int qrec_als_gram_f64(const double* dev_Z, int64_t n, int32_t d, double* dev_G, void* dev_workspace,
+                      int64_t workspace_bytes, void* stream);
+/* Solves the rows row_order[0..n_rows) of X (a different table from Z) with G = Z^T Z from qrec_als_gram_*:
+ * row r's entries are cols[rowptr[r]..rowptr[r+1]) (rows of Z) with values vals[...].  One CTA solves one row
+ * (Cholesky in float64), so X is bitwise reproducible; row_order only balances the work (longest rows first).
+ * A row without entries gets x = 0.  dev_loss (optional, double[1]) accumulates sum_k (1 - x_old.z_k)^2 with the
+ * row's value before the solve.  A row whose A has a pivot that is not positive is left unchanged and counted in
+ * dev_n_failed (optional, int32[1]).  d > 128 is QREC_ERR_ARG. */
+int qrec_als_solve_rows_f32(float* dev_X, const float* dev_Z, const double* dev_G, int32_t d, int64_t n_rows,
+                            const int32_t* dev_row_order, const int64_t* dev_rowptr, const int32_t* dev_cols,
+                            const float* dev_vals, double lambda, double alpha, double* dev_loss,
+                            int32_t* dev_n_failed, void* stream);
+int qrec_als_solve_rows_f64(double* dev_X, const double* dev_Z, const double* dev_G, int32_t d, int64_t n_rows,
+                            const int32_t* dev_row_order, const int64_t* dev_rowptr, const int32_t* dev_cols,
+                            const double* dev_vals, double lambda, double alpha, double* dev_loss,
+                            int32_t* dev_n_failed, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -81,6 +81,13 @@ SIGNATURES = {
                                         C.c_float, vp, vp, C.c_float, C.c_float, vp, C.c_int64, vp]),
     'qrec_mf_predict_pairs_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_float, vp, vp]),
     'qrec_mf_predict_pairs_f64': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_double, vp, vp]),
+    'qrec_als_gram_workspace_bytes': (C.c_int64, [C.c_int64, C.c_int32]),
+    'qrec_als_gram_f32': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),
+    'qrec_als_gram_f64': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),
+    'qrec_als_solve_rows_f32': (C.c_int, [vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double,
+                                          vp, vp, vp]),
+    'qrec_als_solve_rows_f64': (C.c_int, [vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double,
+                                          vp, vp, vp]),
     'qrec_bpr_sgd_batch_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float,
                                          C.c_float, C.c_float, vp, vp]),
     'qrec_bpr_sgd_batch_tma_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float,

@@ -1,0 +1,399 @@
+// WRMF (implicit-feedback ALS): the Gram matrix of a table and the per-row normal-equation solve.
+//
+//   reference: model/ranking/WRMF.py:19-61.  Within one half-epoch every row's solve reads only the other table Z:
+//     G = Z^T Z;   for each row r with entries (c_k, v_k):
+//       A = G + lambda*I + sum_k alpha*v_k z_k z_k^T,   b = sum_k (1 + alpha*v_k) z_k,   x_r = A^-1 b
+//
+//   * als_gram_partial_kernel / als_gram_sum_kernel -- G in two stages: every chunk of kGramChunk rows gets its own
+//     partial Gram in the caller's workspace, then the partials are summed in chunk order.  Neither the chunking nor
+//     any summation order depends on the grid, so G is bitwise the same on every run and every H100.
+//   * als_solve_rows_kernel -- one CTA solves one row completely: it stages the row's z vectors into shared memory
+//     kStage at a time, accumulates the upper triangle of A in float64 registers (4x4 tiles: each staged element
+//     feeds four FMAs), factors A in shared memory (als_step.cuh) and substitutes with one warp.  The grid is
+//     persistent and walks the caller's row order (longest rows first keeps one long row from becoming the tail).
+//     Nothing depends on scheduling, so the solved tables are bitwise reproducible.
+#include "common.h"
+#include "device.cuh"
+#include "als_step.cuh"
+
+namespace {
+
+using namespace qrec;
+
+constexpr int kThreads = 256;
+constexpr int kStage = 32;         // z rows staged in shared memory at a time
+constexpr int kGramChunk = 2048;   // rows per partial Gram
+constexpr int kMaxD = 128;
+
+__host__ __device__ inline int pad4(int d) { return (d + 3) & ~3; }
+__host__ __device__ inline int tiles_of(int d) { const int nb = pad4(d) / 4; return nb * (nb + 1) / 2; }
+
+// Shared-memory carve-up (doubles): A [d][ld] (ld = pad4(d)+1: odd, so column walks are conflict-free),
+// Zs [kStage][dp], W [kStage], x_old [dp], b [dp], s [dp].
+__host__ __device__ inline int a_words(int d) { return (d * (pad4(d) + 1) + 1) & ~1; }
+inline size_t smem_bytes(int d) { return sizeof(double) * ((size_t)a_words(d) + (size_t)(kStage + 3) * pad4(d) + kStage); }
+
+// The upper-triangle 4x4 tiles of A, split into work items (tile, group): group g accumulates the staged entries
+// k = g, g + ngroups, ...  Small d has few tiles, so the entries are spread over several groups, reduced in group
+// order.  Every tile has a group-0 item (NT * kThreads >= tiles).
+template <int NT>
+struct Tiles {
+  double acc[NT][16];
+  int a0[NT], b0[NT], grp[NT];
+  int ngroups;
+
+  __device__ void setup(int d) {
+    const int nb = pad4(d) / 4, nt = tiles_of(d);
+    ngroups = NT * kThreads / nt;
+    if (ngroups > kStage) ngroups = kStage;
+#pragma unroll
+    for (int s = 0; s < NT; ++s) {
+      const int id = threadIdx.x + s * kThreads;
+      grp[s] = id < nt * ngroups ? id / nt : -1;
+      int q = id % nt, I = 0;
+      while (q >= nb - I) { q -= nb - I; ++I; }
+      a0[s] = 4 * I;
+      b0[s] = 4 * (I + q);
+    }
+  }
+
+  __device__ void zero() {
+#pragma unroll
+    for (int s = 0; s < NT; ++s)
+#pragma unroll
+      for (int e = 0; e < 16; ++e) acc[s][e] = 0.0;
+  }
+
+  // acc += sum over the staged entries of (W[k] z_k[a]) z_k[b]
+  __device__ void accumulate(const double* Zs, const double* W, int dp, int cnt) {
+#pragma unroll
+    for (int s = 0; s < NT; ++s) {
+      if (grp[s] < 0) continue;
+      for (int k = grp[s]; k < cnt; k += ngroups) {
+        const double w = W[k];
+        const double* z = Zs + k * dp;
+        const double2 x0 = *reinterpret_cast<const double2*>(z + a0[s]);
+        const double2 x1 = *reinterpret_cast<const double2*>(z + a0[s] + 2);
+        const double2 y0 = *reinterpret_cast<const double2*>(z + b0[s]);
+        const double2 y1 = *reinterpret_cast<const double2*>(z + b0[s] + 2);
+        const double za[4] = {w * x0.x, w * x0.y, w * x1.x, w * x1.y};
+        const double zb[4] = {y0.x, y0.y, y1.x, y1.y};
+#pragma unroll
+        for (int p = 0; p < 4; ++p)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) acc[s][p * 4 + q] = fma(za[p], zb[q], acc[s][p * 4 + q]);
+      }
+    }
+  }
+
+  // S = sum of the groups' tiles, upper triangle of A (ld); ends with a barrier
+  __device__ void reduce_into(double* A, int d, int ld) {
+    for (int g = 0; g < ngroups; ++g) {
+#pragma unroll
+      for (int s = 0; s < NT; ++s) {
+        if (grp[s] != g) continue;
+#pragma unroll
+        for (int p = 0; p < 4; ++p)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int a = a0[s] + p, b = b0[s] + q;
+            if (a <= b && b < d) A[a * ld + b] = g == 0 ? acc[s][p * 4 + q] : A[a * ld + b] + acc[s][p * 4 + q];
+          }
+      }
+      __syncthreads();
+    }
+  }
+};
+
+// Stages rows row_of(k) of Z (k < cnt) as float64 with zero columns up to dp.  Each warp gathers its kStage/8 rows
+// into registers first, so all of a thread's loads are in flight together, then stores them.
+template <typename T, class RowOf>
+__device__ __forceinline__ void stage_rows(double* Zs, const T* __restrict__ Z, int d, int dp, int cnt, RowOf row_of) {
+  constexpr int kWarps = kThreads / 32, R = kStage / kWarps, C = kMaxD / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double v[R][C];
+#pragma unroll
+  for (int m = 0; m < R; ++m) {
+    const int k = warp + m * kWarps;
+    const T* z = Z + (size_t)(k < cnt ? row_of(k) : 0) * d;
+#pragma unroll
+    for (int e = 0; e < C; ++e) {
+      const int c = e * 32 + lane;
+      v[m][e] = k < cnt && c < d ? (double)__ldg(z + c) : 0.0;
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < R; ++m) {
+    const int k = warp + m * kWarps;
+#pragma unroll
+    for (int e = 0; e < C; ++e)
+      if (k < cnt && e * 32 + lane < dp) Zs[k * dp + e * 32 + lane] = v[m][e];
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Gram
+// ------------------------------------------------------------------------------------------
+template <typename T, int NT>
+__global__ void __launch_bounds__(kThreads)
+als_gram_partial_kernel(const T* __restrict__ Z, long long n, int d, double* __restrict__ parts) {
+  extern __shared__ __align__(16) double smem[];
+  const int dp = pad4(d), ld = dp + 1;
+  double* A = smem;
+  double* Zs = A + a_words(d);
+  double* W = Zs + kStage * dp;
+  for (int k = threadIdx.x; k < kStage; k += kThreads) W[k] = 1.0;
+  Tiles<NT> tl;
+  tl.setup(d);
+  const long long nchunks = (n + kGramChunk - 1) / kGramChunk;
+  for (long long c = blockIdx.x; c < nchunks; c += gridDim.x) {
+    tl.zero();
+    const long long r0 = c * kGramChunk;
+    const long long r1 = r0 + kGramChunk < n ? r0 + kGramChunk : n;
+    for (long long k0 = r0; k0 < r1; k0 += kStage) {
+      const int cnt = (int)(r1 - k0 < kStage ? r1 - k0 : kStage);
+      __syncthreads();
+      stage_rows<T>(Zs, Z, d, dp, cnt, [=](int k) { return k0 + k; });
+      __syncthreads();
+      tl.accumulate(Zs, W, dp, cnt);
+    }
+    __syncthreads();
+    tl.reduce_into(A, d, ld);
+    double* out = parts + (size_t)c * d * d;
+    for (int e = threadIdx.x; e < d * d; e += kThreads) {
+      const int a = e / d, b = e % d;
+      out[e] = a <= b ? A[a * ld + b] : A[b * ld + a];     // mirrored: G is exactly symmetric
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+als_gram_sum_kernel(const double* __restrict__ parts, long long nchunks, int dd, double* __restrict__ G) {
+  const int e = blockIdx.x * kThreads + threadIdx.x;
+  if (e >= dd) return;
+  double g = 0.0;
+  for (long long c = 0; c < nchunks; ++c) g += parts[(size_t)c * dd + e];
+  G[e] = g;
+}
+
+// ------------------------------------------------------------------------------------------
+// row solve
+// ------------------------------------------------------------------------------------------
+template <typename T, int NT>
+__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
+als_solve_rows_kernel(T* __restrict__ X, const T* __restrict__ Z, const double* __restrict__ G, int d,
+                      long long n_order, const int* __restrict__ order, const long long* __restrict__ rowptr,
+                      const int* __restrict__ cols, const T* __restrict__ vals, double lambda, double alpha,
+                      double* loss, int* n_failed) {
+  extern __shared__ __align__(16) double smem[];
+  const int dp = pad4(d), ld = dp + 1;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  double* A = smem;
+  double* Zs = A + a_words(d);
+  double* W = Zs + kStage * dp;
+  double* xo = W + kStage;
+  double* bv = xo + dp;
+  double* sd = bv + dp;
+  Tiles<NT> tl;
+  tl.setup(d);
+  double lsum = 0.0;
+  for (long long q = blockIdx.x; q < n_order; q += gridDim.x) {
+    const int r = __ldg(order + q);
+    const long long beg = __ldg(rowptr + r), end = __ldg(rowptr + r + 1);
+    T* x = X + (size_t)r * d;
+    tl.zero();
+    double bacc = 0.0;
+    __syncthreads();                                   // the previous row's solve is done with the buffers
+    if (loss != nullptr)
+      for (int c = t; c < dp; c += kThreads) xo[c] = c < d ? (double)x[c] : 0.0;
+    for (long long k0 = beg; k0 < end; k0 += kStage) {
+      const int cnt = (int)(end - k0 < kStage ? end - k0 : kStage);
+      __syncthreads();
+      stage_rows<T>(Zs, Z, d, dp, cnt, [=](int k) { return __ldg(cols + k0 + k); });
+      for (int k = t; k < cnt; k += kThreads) W[k] = als_conf<T>(__ldg(vals + k0 + k), alpha);
+      __syncthreads();
+      tl.accumulate(Zs, W, dp, cnt);
+      if (t < d)
+        for (int k = 0; k < cnt; ++k) bacc = fma(als_rhs_weight(W[k]), Zs[k * dp + t], bacc);
+      if (loss != nullptr) {
+        for (int k = warp; k < cnt; k += kThreads / 32) {
+          double xz = 0.0;
+          for (int c = lane; c < d; c += 32) xz = fma(xo[c], Zs[k * dp + c], xz);
+          xz = warp_sum(xz);
+          if (lane == 0) lsum += als_loss_term(xz);
+        }
+      }
+    }
+    __syncthreads();
+    tl.reduce_into(A, d, ld);
+    // A = (G + S) + lambda*I  (WRMF.py:41: YtY + Y^T C_u Y + regU * eye)
+    for (int e = t; e < d * d; e += kThreads) {
+      const int a = e / d, b = e % d;
+      if (a <= b) A[a * ld + b] = (__ldg(G + e) + A[a * ld + b]) + (a == b ? lambda : 0.0);
+    }
+    if (t < d) bv[t] = bacc;
+    __syncthreads();
+    bool ok = true;
+    for (int j = 0; j < d; ++j) {
+      const double p = A[j * ld + j];
+      if (!als_pivot_ok(p)) { ok = false; break; }      // uniform: every thread reads the same pivot
+      const double s = als_pivot_scale(p);
+      if (t == 0) sd[j] = s;
+      als_chol_step(A, d, ld, j, s, t, kThreads);
+      __syncthreads();
+    }
+    if (!ok) {                                          // the row keeps its old value
+      if (t == 0 && n_failed != nullptr) atomicAdd(n_failed, 1);
+      continue;
+    }
+    als_chol_scale_rows(A, d, ld, sd, t, kThreads);
+    __syncthreads();
+    if (warp == 0) {                                    // U^T y = b, U x = y (als_solve, one warp)
+      double y[kMaxD / 32];
+#pragma unroll
+      for (int e = 0; e < kMaxD / 32; ++e) y[e] = e * 32 + lane < d ? bv[e * 32 + lane] : 0.0;
+      for (int j = 0; j < d; ++j) {
+        double v = 0.0;
+#pragma unroll
+        for (int e = 0; e < kMaxD / 32; ++e) if (e == (j >> 5)) v = y[e];
+        const double yj = __shfl_sync(0xffffffffu, v, j & 31) * sd[j];
+#pragma unroll
+        for (int e = 0; e < kMaxD / 32; ++e) {
+          const int i = e * 32 + lane;
+          if (i == j) y[e] = yj;
+          else if (i > j && i < d) y[e] = als_sub(y[e], A[j * ld + i], yj);
+        }
+      }
+      for (int i = d - 1; i >= 0; --i) {
+        double v = 0.0;
+#pragma unroll
+        for (int e = 0; e < kMaxD / 32; ++e) if (e == (i >> 5)) v = y[e];
+        const double xi = __shfl_sync(0xffffffffu, v, i & 31) * sd[i];
+#pragma unroll
+        for (int e = 0; e < kMaxD / 32; ++e) {
+          const int m = e * 32 + lane;
+          if (m == i) y[e] = xi;
+          else if (m < i) y[e] = als_sub(y[e], A[m * ld + i], xi);
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < kMaxD / 32; ++e)
+        if (e * 32 + lane < d) x[e * 32 + lane] = (T)y[e];
+    }
+  }
+  if (loss != nullptr) {
+    __shared__ double wsum[kThreads / 32];
+    lsum = warp_sum(lsum);
+    __syncthreads();
+    if (lane == 0) wsum[warp] = lsum;
+    __syncthreads();
+    if (t == 0) {
+      double s = 0.0;
+      for (int w = 0; w < kThreads / 32; ++w) s += wsum[w];
+      if (s != 0.0) atomicAdd(loss, s);
+    }
+  }
+}
+
+// persistent grid: as many CTAs as fit on the GPU at `bytes` of dynamic shared memory, at most `work`
+template <class K>
+int persistent_grid(K kernel, size_t bytes, long long work, int* grid) {
+  QREC_CUDA(allow_dynamic_smem((const void*)kernel, (int)bytes));
+  int per_sm = 0;
+  QREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, bytes));
+  *grid = capped_grid(work, per_sm > 0 ? per_sm : 1);
+  return QREC_OK;
+}
+
+long long gram_chunks(long long n) { return (n + kGramChunk - 1) / kGramChunk; }
+
+template <typename T>
+int launch_gram(const T* Z, long long n, int d, double* G, void* ws, long long ws_bytes, cudaStream_t st) {
+  QREC_REQUIRE(d >= 1 && d <= kMaxD, "als_gram: d=%d unsupported (1..%d)", d, kMaxD);
+  QREC_REQUIRE(n >= 0, "als_gram: n < 0");
+  QREC_REQUIRE(G != nullptr, "als_gram: null G");
+  const long long nchunks = gram_chunks(n);
+  QREC_REQUIRE(nchunks == 0 || (Z != nullptr && ws != nullptr), "als_gram: null pointer");
+  QREC_REQUIRE(ws_bytes >= nchunks * d * d * (long long)sizeof(double),
+               "als_gram: workspace of %lld bytes, %lld needed (qrec_als_gram_workspace_bytes)", ws_bytes,
+               nchunks * d * d * (long long)sizeof(double));
+  double* parts = (double*)ws;
+  if (nchunks > 0) {
+    const size_t bytes = smem_bytes(d);
+    int grid = 0;
+    if (tiles_of(d) <= kThreads) {
+      const int rc = persistent_grid(als_gram_partial_kernel<T, 1>, bytes, nchunks, &grid);
+      if (rc) return rc;
+      als_gram_partial_kernel<T, 1><<<grid, kThreads, bytes, st>>>(Z, n, d, parts);
+    } else {
+      const int rc = persistent_grid(als_gram_partial_kernel<T, 3>, bytes, nchunks, &grid);
+      if (rc) return rc;
+      als_gram_partial_kernel<T, 3><<<grid, kThreads, bytes, st>>>(Z, n, d, parts);
+    }
+    QREC_LAUNCH_CHECK();
+  }
+  als_gram_sum_kernel<<<(d * d + kThreads - 1) / kThreads, kThreads, 0, st>>>(parts, nchunks, d * d, G);
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
+template <typename T>
+int launch_solve(T* X, const T* Z, const double* G, int d, long long n_order, const int* order,
+                 const long long* rowptr, const int* cols, const T* vals, double lambda, double alpha, double* loss,
+                 int* n_failed, cudaStream_t st) {
+  QREC_REQUIRE(d >= 1 && d <= kMaxD, "als_solve_rows: d=%d unsupported (1..%d)", d, kMaxD);
+  QREC_REQUIRE(n_order >= 0, "als_solve_rows: n_rows < 0");
+  if (n_order == 0) return QREC_OK;
+  QREC_REQUIRE(X && Z && G && order && rowptr, "als_solve_rows: null pointer");
+  QREC_REQUIRE((const void*)X != (const void*)Z, "als_solve_rows: X and Z must be different tables");
+  const size_t bytes = smem_bytes(d);
+  int grid = 0;
+  if (tiles_of(d) <= kThreads) {
+    const int rc = persistent_grid(als_solve_rows_kernel<T, 1>, bytes, n_order, &grid);
+    if (rc) return rc;
+    als_solve_rows_kernel<T, 1><<<grid, kThreads, bytes, st>>>(X, Z, G, d, n_order, order, rowptr, cols, vals,
+                                                                lambda, alpha, loss, n_failed);
+  } else {
+    const int rc = persistent_grid(als_solve_rows_kernel<T, 3>, bytes, n_order, &grid);
+    if (rc) return rc;
+    als_solve_rows_kernel<T, 3><<<grid, kThreads, bytes, st>>>(X, Z, G, d, n_order, order, rowptr, cols, vals,
+                                                                lambda, alpha, loss, n_failed);
+  }
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t qrec_als_gram_workspace_bytes(int64_t n, int32_t d) {
+  QREC_REQUIRE(n >= 0 && d >= 1 && d <= kMaxD, "als_gram_workspace_bytes: n=%lld d=%d", (long long)n, d);
+  return gram_chunks(n) * d * d * (int64_t)sizeof(double);
+}
+
+int qrec_als_gram_f32(const float* Z, int64_t n, int32_t d, double* G, void* workspace, int64_t workspace_bytes,
+                      void* stream) {
+  return launch_gram<float>(Z, n, d, G, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int qrec_als_gram_f64(const double* Z, int64_t n, int32_t d, double* G, void* workspace, int64_t workspace_bytes,
+                      void* stream) {
+  return launch_gram<double>(Z, n, d, G, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int qrec_als_solve_rows_f32(float* X, const float* Z, const double* G, int32_t d, int64_t n_rows,
+                            const int32_t* row_order, const int64_t* rowptr, const int32_t* cols, const float* vals,
+                            double lambda, double alpha, double* loss, int32_t* n_failed, void* stream) {
+  return launch_solve<float>(X, Z, G, d, n_rows, row_order, (const long long*)rowptr, cols, vals, lambda, alpha, loss,
+                             n_failed, (cudaStream_t)stream);
+}
+
+int qrec_als_solve_rows_f64(double* X, const double* Z, const double* G, int32_t d, int64_t n_rows,
+                            const int32_t* row_order, const int64_t* rowptr, const int32_t* cols, const double* vals,
+                            double lambda, double alpha, double* loss, int32_t* n_failed, void* stream) {
+  return launch_solve<double>(X, Z, G, d, n_rows, row_order, (const long long*)rowptr, cols, vals, lambda, alpha,
+                              loss, n_failed, (cudaStream_t)stream);
+}
+
+}  // extern "C"

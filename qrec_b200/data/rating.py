@@ -105,6 +105,27 @@ class Rating(object):
             self._csr = RatedCSR(len(self.user), len(self.item), u, i, r)
         return self._csr
 
+    def rating_csr(self, by='user'):
+        """(rowptr int64, cols int32, vals float64) of trainSet_u (by='user': rows are user ids, columns item ids)
+        or trainSet_i (by='item': rows are item ids, columns user ids), each row in the dict's insertion order.
+        Built from the dicts, so a repeated (user, item) line counts once with its last value and `-b` is already
+        applied -- the entries WRMF.py:30-36 / 51-57 visit."""
+        if by not in ('user', 'item'):
+            raise ValueError("by must be 'user' or 'item'")
+        cache = self.__dict__.setdefault('_rating_csr', {})
+        if by not in cache:
+            rows, names, ids, other = ((self.trainSet_u, self.id2user, self.user, self.item) if by == 'user'
+                                       else (self.trainSet_i, self.id2item, self.item, self.user))
+            lengths = np.fromiter((len(rows[names[k]]) for k in range(len(ids))), dtype=np.int64, count=len(ids))
+            rowptr = np.zeros(len(ids) + 1, dtype=np.int64)
+            np.cumsum(lengths, out=rowptr[1:])
+            n = int(rowptr[-1])
+            cols = np.fromiter((other[c] for k in range(len(ids)) for c in rows[names[k]]), dtype=np.int32, count=n)
+            vals = np.fromiter((float(v) for k in range(len(ids)) for v in rows[names[k]].values()), dtype=np.float64,
+                               count=n)
+            cache[by] = (rowptr, cols, vals)
+        return cache[by]
+
     # ------------------------------------------------------------------ reference API
     def getUserId(self, u):
         return self.user.get(u)

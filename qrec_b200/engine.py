@@ -997,3 +997,63 @@ def mf_predict_pairs(P, Q, u, i, Bu=None, Bi=None, global_mean=0.0, out=None):
              _dev(i, torch.int32, 'i'), _opt(Bu, dt, 'Bu'), _opt(Bi, dt, 'Bi'), float(global_mean),
              _dev(out, dt, 'out'), _stream()), 'qrec_mf_predict_pairs')
     return out
+
+
+# =============================================================================================
+# K10: WRMF (implicit-feedback ALS) -- Gram matrix and per-row normal-equation solve
+# =============================================================================================
+def als_row_order(rowptr):
+    """Rows by decreasing entry count (ties by id): the order als_solve_rows hands rows to its persistent grid,
+    so that one long row does not become the tail.  rowptr: host int64 array."""
+    lengths = np.diff(np.asarray(rowptr, dtype=np.int64))
+    return np.argsort(-lengths, kind='stable').astype(np.int32)
+
+
+def als_gram(Z, G=None, workspace=None):
+    """G = Z^T Z as a float64 [d, d] CUDA tensor for a float32 / float64 table Z (bitwise reproducible).
+    workspace: optional uint8 CUDA tensor of at least qrec_als_gram_workspace_bytes(n, d) bytes, reused across calls."""
+    torch = _torch()
+    n, d = Z.shape
+    if Z.dtype not in (torch.float32, torch.float64):
+        raise QRecError('Z must be float32 or float64, got %s' % Z.dtype)
+    need = int(lib.qrec_als_gram_workspace_bytes(n, d))
+    if need < 0:
+        check(need, 'qrec_als_gram_workspace_bytes')
+    if G is None:
+        G = torch.empty(d, d, dtype=torch.float64, device=Z.device)
+    if workspace is None:
+        workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=Z.device)
+    fn = lib.qrec_als_gram_f64 if Z.dtype == torch.float64 else lib.qrec_als_gram_f32
+    check(fn(_dev(Z, Z.dtype, 'Z'), n, d, _dev(G, torch.float64, 'G'), _dev(workspace, torch.uint8, 'workspace'),
+             workspace.numel(), _stream()), 'qrec_als_gram')
+    return G
+
+
+def als_solve_rows(X, Z, G, rowptr, cols, vals, lam, alpha, row_order, loss=None, n_failed=None):
+    """Solves the rows `row_order` of X against Z (WRMF.py:22-42 / 44-61): X[r] = (G + lam*I + alpha*sum v z z^T)^-1
+    sum (1 + alpha*v) z over row r's entries (cols, vals) of the CSR (rowptr int64, cols int32, vals like X).
+    loss: optional float64 CUDA tensor that accumulates sum (1 - x_old.z)^2.  n_failed: optional int32 CUDA tensor
+    counting rows whose normal equations were not positive definite (left unchanged); when it is not given, the count
+    is read back here and a failed row raises QRecError."""
+    torch = _torch()
+    d = X.shape[1]
+    if X.dtype not in (torch.float32, torch.float64):
+        raise QRecError('X must be float32 or float64, got %s' % X.dtype)
+    dt = X.dtype
+    if Z.shape[1] != d:
+        raise QRecError('X and Z differ in width (%d, %d)' % (d, Z.shape[1]))
+    own = n_failed is None
+    if own:
+        n_failed = torch.zeros(1, dtype=torch.int32, device=X.device)
+    fn = lib.qrec_als_solve_rows_f64 if dt == torch.float64 else lib.qrec_als_solve_rows_f32
+    check(fn(_dev(X, dt, 'X'), _dev(Z, dt, 'Z'), _dev(G, torch.float64, 'G'), d, row_order.shape[0],
+             _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
+             _dev(cols, torch.int32, 'cols'), _dev(vals, dt, 'vals'), float(lam), float(alpha),
+             _opt(loss, torch.float64, 'loss'), _dev(n_failed, torch.int32, 'n_failed'), _stream()),
+          'qrec_als_solve_rows')
+    if own:
+        bad = int(n_failed.item())
+        if bad:
+            raise QRecError('als_solve_rows: %d row(s) with normal equations that are not positive definite were '
+                            'left unchanged' % bad)
+    return X

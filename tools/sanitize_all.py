@@ -130,6 +130,19 @@ def main():
         E.simgcl_perturb(X, 0.1, 7, 1, 1, acc=acc, acc_scale=0.5, d_valid=62, row_offset=12345)
         torch.cuda.synchronize()
         print('sanitize_all: + round 2, launched', E.launch_count(), 'kernels')
+        # K10 (WRMF): Gram + row solve, both table types, the one-tile-per-thread and three-tiles-per-thread builds
+        rp_u = torch.from_numpy(np.bincount(u, minlength=nu).cumsum()).cuda()
+        rowptr = torch.cat([torch.zeros(1, dtype=torch.int64, device='cuda'), rp_u])
+        cols = dev(i[np.argsort(u, kind='stable')])
+        order = dev(E.als_row_order(rowptr.cpu().numpy()))
+        for dd in (20, 128):
+            for dt in (torch.float64, torch.float32):
+                Xs, Ys = torch.rand(nu, dd, device='cuda', dtype=dt), torch.rand(ni, dd, device='cuda', dtype=dt)
+                G = E.als_gram(Ys)
+                E.als_solve_rows(Xs, Ys, G, rowptr, cols, torch.ones(n, device='cuda', dtype=dt), 1.0, 10.0, order,
+                                 loss=loss)
+        torch.cuda.synchronize()
+        print('sanitize_all: + K10, launched', E.launch_count(), 'kernels')
 
 
 if __name__ == '__main__':
