@@ -236,8 +236,10 @@ int qrec_bpr_epoch_usermajor_f32(float* dev_P, float* dev_Q, int32_t d, int32_t 
 
 /* The fused epoch with the item rows staged through shared memory by the bulk-copy (TMA) engine: one
  * cp.async.bulk (256 bytes) per row into a per-lane-group staging slot, completion on an mbarrier, lanes read their
- * slices with LDS.128; two slots per group, so the next 4 triples' rows are in flight while 4 are computed.  Same
- * step, order, sampler (identical negatives) and scatter-add as qrec_bpr_epoch_usermajor_f32.  d = 64 only. */
+ * slices with LDS.128; two slots per group, so the next 4 triples' rows are in flight while 4 are computed.  The
+ * same kernel body, chunking, waves and wave snapshot of the item table as qrec_bpr_epoch_usermajor_f32, so it
+ * draws the same negatives and gives the same result up to the summation order of the scatter-adds.  d = 64 only;
+ * dev_Q 16-byte aligned. */
 int qrec_bpr_epoch_usermajor_tma_f32(float* dev_P, float* dev_Q, int32_t d, int32_t n_users, int64_t n,
                                      const int64_t* dev_rowptr, const int32_t* dev_i,
                                      const int64_t* dev_rated_rowptr, const int32_t* dev_rated_cols,

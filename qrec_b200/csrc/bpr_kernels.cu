@@ -18,7 +18,6 @@
 //     REDG.E.ADD.F32x4 (red.global.add.v4.f32).  UNROLL triples per lane group are in flight
 //     before the first use so each warp keeps 2*UNROLL*3 row loads outstanding.
 #include <cmath>
-#include <cstdlib>
 
 #include "common.h"
 #include "device.cuh"
@@ -367,17 +366,33 @@ bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long
 // SAMPLE: the negatives are drawn inside the kernel (lane l draws the negative of triple base+l with
 // the same Philox counter as the stand-alone sampler, so both give identical j) instead of being
 // read from j[] (FusedSampler, philox.cuh); they are optionally written to j_out.
-
 // SIG: the sampler pre-tests every draw against the user's 512-bit rated signature (philox.cuh).
-template <int LPR, int G, int CH, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>   // FULL: d == 4*LPR (every lane owns a slice)
-__global__ void __launch_bounds__(256, MINB)
-bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, int n_users,
-                         long long n, long long ch_begin, long long ch_end, const long long* __restrict__ rowptr,
-                         const int* __restrict__ i, const int* __restrict__ j, float lr,
-                         float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
-                         const uint32_t* __restrict__ rated_sig) {
+// TMA (d = 64 only): the item rows reach the lane group through shared memory instead of one LDG.128 per lane
+// and row.  One lane per row issues a 256-byte cp.async.bulk from Qr into the group's staging slot, completion is
+// signalled on the slot's mbarrier and the lanes read their slices with LDS.128, so the gathers leave the
+// LSU/L1TEX path, which then carries only the scatter-adds.  Two slots per lane group: the rows of the next G
+// triples are requested while the current G are computed.
+constexpr int UM_CH = 32;                                    // triples per chunk
+constexpr int UM_STAGE_FLOATS = 2 * 4 * 64;                  // one slot: the 2 x G rows of G = 4 triples, d = 64
+constexpr int UM_STAGE_GROUPS = 16;                          // lane groups of 16 lanes in a 256-thread CTA
+constexpr int UM_STAGE_SMEM = UM_STAGE_GROUPS * 2 * (UM_STAGE_FLOATS * 4 + 8);   // two slots + two mbarriers per group
+
+// one 256-byte row: global -> this CTA's shared memory, completion counted on `bar`
+__device__ __forceinline__ void bulk_row_load(float* smem_dst, const float* gsrc, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 256, [%2];"
+               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(smem_u32(bar)) : "memory");
+}
+
+template <int LPR, int G, int CH, bool FULL, bool SAMPLE, bool SIG, bool TMA>   // FULL: d == 4*LPR (every lane owns a slice)
+__device__ __forceinline__ void
+usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, int n_users,
+                long long n, long long ch_begin, long long ch_end, const long long* __restrict__ rowptr,
+                const int* __restrict__ i, const int* __restrict__ j, float lr,
+                float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
+                const uint32_t* __restrict__ rated_sig) {
   // rowptr holds GLOBAL triple offsets; i/j are indexed relative to trip_off (a chunk of users of a
   // larger epoch: the host pipeline stages one chunk at a time).  Philox counters use global indices.
+  static_assert(!TMA || (LPR == 16 && G == 4 && FULL), "the TMA fetch is laid out for d = 64, G = 4");
   constexpr int GPW = 32 / LPR;
   const int lane = threadIdx.x & 31;
   const int sub = lane / LPR, l = lane % LPR;
@@ -389,6 +404,21 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const flo
   const float a_u = lr * reg_u, a_i = lr * reg_i;
   const float one_m_au = 1.0f - a_u, one_m_ai = 1.0f - a_i;
   float lsum = 0.f;
+  float* stage = nullptr;                                    // TMA: this group's two slots and their mbarriers
+  uint64_t* bar = nullptr;
+  uint32_t phase0 = 0, phase1 = 0;
+  if constexpr (TMA) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    float* stage_all = reinterpret_cast<float*>(smem_raw);                                         // [GROUPS][2][8][64]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(stage_all + UM_STAGE_GROUPS * 2 * UM_STAGE_FLOATS);  // [GROUPS][2]
+    const int g_in_cta = (threadIdx.x >> 5) * GPW + sub;
+    stage = stage_all + (size_t)g_in_cta * 2 * UM_STAGE_FLOATS;
+    bar = bars + g_in_cta * 2;
+    if (l == 0) { mbar_init(bar, 1); mbar_init(bar + 1, 1); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+  }
   // user of triple t: smallest r with rowptr[r+1] > t (LPR-ary search by the lane group)
   auto user_of = [&](long long t) {
     int a = 0, b = n_users - 1;
@@ -454,7 +484,26 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const flo
           mj = __ldg(j + base + l);
         }
       }
+      // TMA: request the rows of triples t0 .. t0+G-1 into slot (t0 / G) & 1: lane 2f -> Qr[i_f], lane 2f+1 -> Qr[j_f]
+      auto issue = [&](int t0) {
+        const int src = sub * LPR + ((t0 + (l >> 1)) & (LPR - 1));
+        const int idi = __shfl_sync(gmask, mi, src), idj = __shfl_sync(gmask, mj, src);
+        const int rows_now = 2 * ((m - t0) < G ? (m - t0) : G);
+        uint64_t* bb = bar + ((t0 / G) & 1);
+        if (l == 0) mbar_expect_tx(bb, 256u * rows_now);
+        __syncwarp(gmask);
+        if (l < rows_now) bulk_row_load(stage + ((t0 / G) & 1) * UM_STAGE_FLOATS + l * 64, Qr + (size_t)((l & 1) ? idj : idi) * d, bb);
+      };
+      if constexpr (TMA) issue(0);
       for (int t0 = 0; t0 < m; t0 += G) {
+        const float* slot = nullptr;
+        if constexpr (TMA) {
+          if (t0 + G < m) issue(t0 + G);
+          const int s = (t0 / G) & 1;
+          mbar_wait(bar + s, s ? phase1 : phase0);
+          if (s) phase1 ^= 1u; else phase0 ^= 1u;
+          slot = stage + s * UM_STAGE_FLOATS;
+        }
         float4 qi[G], qj[G];
         int ri[G], rj[G];
 #pragma unroll
@@ -462,12 +511,18 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const flo
           ri[f] = __shfl_sync(gmask, mi, sub * LPR + ((t0 + f) & (LPR - 1)));
           rj[f] = __shfl_sync(gmask, mj, sub * LPR + ((t0 + f) & (LPR - 1)));
           if (t0 + f < m && act) {
-            qi[f] = __ldg(reinterpret_cast<const float4*>(Qr + (size_t)ri[f] * d + l * 4));
-            qj[f] = __ldg(reinterpret_cast<const float4*>(Qr + (size_t)rj[f] * d + l * 4));
+            if constexpr (TMA) {
+              qi[f] = *reinterpret_cast<const float4*>(slot + (2 * f) * 64 + l * 4);
+              qj[f] = *reinterpret_cast<const float4*>(slot + (2 * f + 1) * 64 + l * 4);
+            } else {
+              qi[f] = __ldg(reinterpret_cast<const float4*>(Qr + (size_t)ri[f] * d + l * 4));
+              qj[f] = __ldg(reinterpret_cast<const float4*>(Qr + (size_t)rj[f] * d + l * 4));
+            }
           } else {
             qi[f] = qj[f] = make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
+        if constexpr (TMA) __syncwarp(gmask);         // the slot may be requested again G triples on
 #pragma unroll
         for (int f = 0; f < G; ++f) {
           const long long t = base + t0 + f;
@@ -500,6 +555,39 @@ bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const flo
     if (act) red_add_v4(prow, make_float4(p.x - p0.x, p.y - p0.y, p.z - p0.z, p.w - p0.w));
   }
   block_add_loss(lsum, loss);
+}
+
+template <int LPR, int G, int CH, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>
+__global__ void __launch_bounds__(256, MINB)
+bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, int n_users,
+                         long long n, long long ch_begin, long long ch_end, const long long* __restrict__ rowptr,
+                         const int* __restrict__ i, const int* __restrict__ j, float lr,
+                         float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
+                         const uint32_t* __restrict__ rated_sig) {
+  usermajor_epoch<LPR, G, CH, FULL, SAMPLE, SIG, false>(P, Q, Qr, nvec, n_users, n, ch_begin, ch_end, rowptr, i, j, lr,
+                                                         reg_u, reg_i, loss, fs, trip_off, rated_sig);
+}
+
+// d = 64 with fused sampling, item rows staged in shared memory (UM_STAGE_SMEM bytes of dynamic shared memory)
+__global__ void __launch_bounds__(256, 3)
+bpr_sgd_usermajor_tma_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec,
+                             int n_users, long long n, long long ch_begin, long long ch_end,
+                             const long long* __restrict__ rowptr, const int* __restrict__ i, const int* __restrict__ j,
+                             float lr, float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
+                             const uint32_t* __restrict__ rated_sig) {
+  usermajor_epoch<16, 4, UM_CH, true, true, false, true>(P, Q, Qr, nvec, n_users, n, ch_begin, ch_end, rowptr, i, j,
+                                                         lr, reg_u, reg_i, loss, fs, trip_off, rated_sig);
+}
+
+using UserMajorKernel = decltype(&bpr_sgd_usermajor_tma_kernel);
+
+// The instantiation for lane groups of LPR lanes: FULL when d = 4 LPR; the signature pre-test only then.
+template <int LPR>
+UserMajorKernel usermajor_kernel(int nvec, bool sample, bool sig) {
+  if (nvec != LPR)
+    return sample ? bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, false, true> : bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, false, false>;
+  if (sig) return bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, true, true, 3, true>;
+  return sample ? bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, true, true> : bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, true, false>;
 }
 
 // one warp per user: bit (c & 511) of the user's 16-word signature for every rated column c
@@ -639,28 +727,13 @@ int qrec_bpr_sgd_batch_tma_f32(float* P, float* Q, int32_t d, int64_t n, const i
   QREC_REQUIRE(n >= 0, "qrec_bpr_sgd_batch_tma_f32: n < 0");
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && j, "qrec_bpr_sgd_batch_tma_f32: null index pointer");
-  constexpr int UN = 4;
-  // which rows use the bulk engine: P only by default (fewest bytes through the copy engine);
-  // QREC_K1_TMA_MASK=7 sends all three rows through it, 6 the two item rows
-  static int mask = -1;
-  if (mask < 0) {
-    const char* e = getenv("QREC_K1_TMA_MASK");
-    mask = e ? atoi(e) : 1;
-    if (mask != 1 && mask != 6 && mask != 7) mask = 1;
-  }
-  const long long blocks_needed = ((n + 31) / 32 + 7) / 8;
-  cudaStream_t st = (cudaStream_t)stream;
-#define QREC_TMA(MASK, ROWS, CTAS)                                                                \
-  {                                                                                               \
-    constexpr int smem = 8 * 2 * UN * 2 * ROWS * 64 * 4;                                          \
-    QREC_CUDA(allow_dynamic_smem((const void*)bpr_sgd_batch_tma_kernel<UN, MASK>, smem));         \
-    const int grid = capped_grid(blocks_needed, CTAS);                                            \
-    bpr_sgd_batch_tma_kernel<UN, MASK><<<grid, 256, smem, st>>>(P, Q, n, u, i, j, lr, reg_u, reg_i, loss); \
-  }
-  if (mask == 7) QREC_TMA(7, 3, 2)
-  else if (mask == 6) QREC_TMA(6, 2, 2)
-  else QREC_TMA(1, 1, 2)
-#undef QREC_TMA
+  // only P's row goes through the bulk engine (TMA_MASK 1: the fewest bytes through the copy engine); the item rows
+  // keep REDG
+  constexpr int UN = 4, MASK = 1;
+  constexpr int smem = 8 * 2 * UN * 2 * 64 * 4;   // 8 warps x 2 buffers x UN*2 triples x one 256-byte row
+  QREC_CUDA(allow_dynamic_smem((const void*)bpr_sgd_batch_tma_kernel<UN, MASK>, smem));
+  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 2);
+  bpr_sgd_batch_tma_kernel<UN, MASK><<<grid, 256, smem, (cudaStream_t)stream>>>(P, Q, n, u, i, j, lr, reg_u, reg_i, loss);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -672,63 +745,29 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
                      const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i, double* loss,
                      bool sample, const int64_t* rated_rowptr, const int32_t* rated_cols, int32_t num_items,
                      uint64_t seed, uint32_t epoch, int32_t* j_out, long long trip_off, cudaStream_t st,
-                     const uint32_t* rated_sig) {
+                     const uint32_t* rated_sig, bool tma) {
+  if (n <= 0) return QREC_OK;
+  QREC_REQUIRE(num_items >= 1, "qrec user-major epoch: num_items=%d (the item table's rows) must be given", num_items);
+  QREC_REQUIRE(!tma || (d == 64 && sample), "qrec user-major epoch: the TMA fetch needs d = 64 and fused sampling");
   FusedSampler fs = {reinterpret_cast<const long long*>(rated_rowptr), rated_cols, num_items, (uint32_t)seed,
                      (uint32_t)(seed >> 32), epoch, j_out};
   const int nvec = d / 4;
+  const int lpr = nvec <= 4 ? 4 : nvec <= 8 ? 8 : nvec <= 16 ? 16 : 32;
+  const bool sig = sample && rated_sig != nullptr;
+  const UserMajorKernel kernel = tma        ? bpr_sgd_usermajor_tma_kernel
+                                 : lpr == 4  ? usermajor_kernel<4>(nvec, sample, sig)
+                                 : lpr == 8  ? usermajor_kernel<8>(nvec, sample, sig)
+                                 : lpr == 16 ? usermajor_kernel<16>(nvec, sample, sig)
+                                             : usermajor_kernel<32>(nvec, sample, sig);
+  const int smem = tma ? UM_STAGE_SMEM : 0;
+  if (tma) QREC_CUDA(allow_dynamic_smem((const void*)kernel, smem));
   // Grid = exactly the CTAs that are resident at once (occupancy API per instantiation); the stream is swept in
   // waves, each reading the item table as the previous waves left it (a snapshot copied on the stream).
-  // QREC_K1_UM_CAP=<CTAs per SM> overrides
-  // (experiment switch).
-  static int cap_mult = -1;
-  if (cap_mult < 0) {
-    const char* e = getenv("QREC_K1_UM_CAP");
-    cap_mult = e ? atoi(e) : 0;
-    if (cap_mult < 0) cap_mult = 0;
-  }
-  constexpr int CH = 32;
-  // experiment switch (d = 64 only): 0 = 3 CTAs/SM, 4 triples in flight (default); 1 = 4 CTAs/SM at 64
-  // registers (spills); 2 = 2 CTAs/SM, 8 triples in flight
-  static int variant = -1;
-  if (variant < 0) {
-    const char* e = getenv("QREC_K1_UM_VARIANT");
-    variant = e ? atoi(e) : 0;
-  }
-#define QREC_UM_LAUNCH(KERNEL, SIGPTR)                                                           \
-  {                                                                                              \
-    int occ = 3;                                                                                 \
-    if (cap_mult > 0) occ = cap_mult;                                                            \
-    else if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, KERNEL, 256, 0) != cudaSuccess || occ < 1) occ = 3; \
-    const int grid = capped_grid(blocks, occ);                                                   \
-    for (long long c0 = 0; c0 < nchunks; c0 += wave) {                                           \
-      QREC_CUDA(cudaMemcpyAsync(Qr, Q, q_bytes, cudaMemcpyDeviceToDevice, st));                  \
-      const long long c1 = (c0 + wave) < nchunks ? (c0 + wave) : nchunks;                        \
-      KERNEL<<<grid, 256, 0, st>>>(P, Q, Qr, nvec, n_users, n, c0, c1, reinterpret_cast<const long long*>(rowptr), \
-                                          i, j, lr, reg_u, reg_i, loss, fs, trip_off, SIGPTR);   \
-      QREC_CUDA(cudaGetLastError());                                                             \
-      if (c1 < nchunks) qrec::count_launch();                                                    \
-    }                                                                                            \
-  }
-#define QREC_UM2(LPR, FULLV, SAMPLEV) QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<LPR, 4, CH, FULLV, SAMPLEV>), nullptr)
-#define QREC_UM(LPR)                                                                             \
-  {                                                                                              \
-    const long long per_block = 8 * (32 / LPR);                                                  \
-    const long long blocks = (nchunks + per_block - 1) / per_block;                              \
-    if (nvec == LPR && sample && rated_sig != nullptr) {                                         \
-      QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<LPR, 4, CH, true, true, 3, true>), rated_sig)     \
-    } else if (nvec == LPR && LPR == 16 && variant == 1) {                                       \
-      if (sample) QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<16, 4, CH, true, true, 4>), nullptr)  \
-      else QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<16, 4, CH, true, false, 4>), nullptr)        \
-    } else if (nvec == LPR && LPR == 16 && variant == 2) {                                       \
-      if (sample) QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<16, 8, CH, true, true, 2>), nullptr)  \
-      else QREC_UM_LAUNCH((bpr_sgd_usermajor_kernel<16, 8, CH, true, false, 2>), nullptr)        \
-    } else                                                                                       \
-    if (nvec == LPR) { if (sample) QREC_UM2(LPR, true, true) else QREC_UM2(LPR, true, false) }   \
-    else { if (sample) QREC_UM2(LPR, false, true) else QREC_UM2(LPR, false, false) }             \
-  }
-  if (n <= 0) return QREC_OK;
-  QREC_REQUIRE(num_items >= 1, "qrec user-major epoch: num_items=%d (the item table's rows) must be given", num_items);
-  const long long nchunks = (n + CH - 1) / CH;
+  int occ = 3;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, 256, smem) != cudaSuccess || occ < 1) occ = 3;
+  const long long nchunks = (n + UM_CH - 1) / UM_CH;
+  const long long per_block = 8 * (32 / lpr);                                 // lane groups per CTA
+  const int grid = capped_grid((nchunks + per_block - 1) / per_block, occ);
   const size_t q_bytes = (size_t)num_items * d * sizeof(float);
   // Wave size in triples: no more than 4 x the item rows, so an item row is read only a few of its own updates late.
   // On a small table (snapshot copy under 8 MB, about the cost of a launch) at least 64 waves per launch: on a small
@@ -738,19 +777,20 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
   const long long copy_floor = copy_bytes > (8LL << 20) ? 8 * copy_bytes / (24LL * d + 12) : 0;
   long long wave_triples = n / 64 > copy_floor ? n / 64 : copy_floor;
   if (wave_triples > 4LL * num_items) wave_triples = 4LL * num_items;
-  const long long wave = wave_triples / CH > 1 ? wave_triples / CH : 1;      // in chunks
+  const long long wave = wave_triples / UM_CH > 1 ? wave_triples / UM_CH : 1;      // in chunks
   float* Qr = nullptr;                                // the item table as the current wave started (stream-ordered scratch)
   QREC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&Qr), q_bytes, st));
   const int rc = [&]() -> int {
-    if (nvec <= 4) QREC_UM(4)
-    else if (nvec <= 8) QREC_UM(8)
-    else if (nvec <= 16) QREC_UM(16)
-    else QREC_UM(32)
+    for (long long c0 = 0; c0 < nchunks; c0 += wave) {
+      QREC_CUDA(cudaMemcpyAsync(Qr, Q, q_bytes, cudaMemcpyDeviceToDevice, st));
+      const long long c1 = (c0 + wave) < nchunks ? (c0 + wave) : nchunks;
+      kernel<<<grid, 256, smem, st>>>(P, Q, Qr, nvec, n_users, n, c0, c1, reinterpret_cast<const long long*>(rowptr), i, j,
+                                      lr, reg_u, reg_i, loss, fs, trip_off, rated_sig);
+      QREC_CUDA(cudaGetLastError());
+      if (c1 < nchunks) count_launch();
+    }
     return QREC_OK;
   }();
-#undef QREC_UM
-#undef QREC_UM2
-#undef QREC_UM_LAUNCH
   QREC_CUDA(cudaFreeAsync(Qr, st));
   if (rc != QREC_OK) return rc;
   QREC_LAUNCH_CHECK();
@@ -769,7 +809,7 @@ int qrec_bpr_sgd_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users, i
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && j, "qrec_bpr_sgd_usermajor_f32: null index pointer");
   return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, j, lr, reg_u, reg_i, loss, false, nullptr, nullptr, num_items,
-                                0, 0, nullptr, 0, (cudaStream_t)stream, nullptr);
+                                0, 0, nullptr, 0, (cudaStream_t)stream, nullptr, false);
 }
 
 int qrec_bpr_epoch_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
@@ -782,7 +822,7 @@ int qrec_bpr_epoch_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users,
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols, "qrec_bpr_epoch_usermajor_f32: null index pointer");
   return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, nullptr, lr, reg_u, reg_i, loss, true, rated_rowptr,
-                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, nullptr);
+                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, nullptr, false);
 }
 
 int qrec_rated_signature_build(int32_t n_users, const int64_t* rated_rowptr, const int32_t* rated_cols,
@@ -809,7 +849,22 @@ int qrec_bpr_epoch_usermajor_sig_f32(float* P, float* Q, int32_t d, int32_t n_us
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols && rated_sig, "qrec_bpr_epoch_usermajor_sig_f32: null index pointer");
   return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, nullptr, lr, reg_u, reg_i, loss, true, rated_rowptr,
-                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, rated_sig);
+                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, rated_sig, false);
+}
+
+int qrec_bpr_epoch_usermajor_tma_f32(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
+                                     const int32_t* i, const int64_t* rated_rowptr, const int32_t* rated_cols,
+                                     int32_t num_items, uint64_t seed, uint32_t epoch, int32_t* j_out, float lr,
+                                     float reg_u, float reg_i, double* loss, void* stream) {
+  QREC_REQUIRE(P && Q && loss, "qrec_bpr_epoch_usermajor_tma_f32: null pointer");
+  QREC_REQUIRE(d == 64, "qrec_bpr_epoch_usermajor_tma_f32: d=%d unsupported (64 only: one 256-byte bulk copy per row); use "
+                        "qrec_bpr_epoch_usermajor_f32", d);
+  QREC_REQUIRE(n_users >= 0 && n >= 0 && num_items >= 1, "qrec_bpr_epoch_usermajor_tma_f32: bad size");
+  if (n_users == 0 || n == 0) return QREC_OK;
+  QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols, "qrec_bpr_epoch_usermajor_tma_f32: null index pointer");
+  QREC_REQUIRE((reinterpret_cast<uintptr_t>(Q) & 15) == 0, "qrec_bpr_epoch_usermajor_tma_f32: Q must be 16-byte aligned");
+  return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, nullptr, lr, reg_u, reg_i, loss, true, rated_rowptr,
+                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, nullptr, true);
 }
 
 int qrec_bpr_sgd_staged_f32(float* P, int32_t d, int64_t n, const int32_t* u, const int32_t* pos_i,

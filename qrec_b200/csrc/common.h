@@ -21,6 +21,19 @@ int capped_grid(long long blocks, int ctas_per_sm);
 // the kernel as loaded on each device, so it is set once per (kernel, device); safe to call from several threads.
 cudaError_t allow_dynamic_smem(const void* kernel, int bytes);
 
+// K1 launchers (bpr_kernels.cu), also driven chunk by chunk by the host-buffer pipeline (runtime.cu).
+// launch_bpr_batch: the order-agnostic fused SGD step over n triples (u, i, j).
+int launch_bpr_batch(float* P, float* Q, int d, long long n, const int* u, const int* i, const int* j, float lr,
+                     float reg_u, float reg_i, double* loss, cudaStream_t st);
+// launch_usermajor: the user-major epoch over a CSR of whole users.  rowptr holds global triple offsets, i / j are
+// indexed from trip_off.  sample: draw the negatives in the kernel (FusedSampler) instead of reading j; rated_sig
+// (may be null) adds the signature pre-test; tma (d = 64, sample) stages the item rows with bulk copies.
+int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
+                     const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i, double* loss,
+                     bool sample, const int64_t* rated_rowptr, const int32_t* rated_cols, int32_t num_items,
+                     uint64_t seed, uint32_t epoch, int32_t* j_out, long long trip_off, cudaStream_t st,
+                     const uint32_t* rated_sig, bool tma);
+
 inline int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
   set_error("%s failed at %s:%d: %s", what, file, line, cudaGetErrorString(e));
   return QREC_ERR_CUDA;

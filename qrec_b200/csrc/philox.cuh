@@ -78,7 +78,7 @@ __device__ __forceinline__ int sample_negative_sig(long long k, uint32_t epoch, 
   }
 }
 
-// Arguments of the negatives drawn inside the fused user-major kernels (bpr_kernels.cu, bpr_tma.cu): the rejection
+// Arguments of the negatives drawn inside the fused user-major kernels (bpr_kernels.cu): the rejection
 // sets, the Philox key and epoch of sample_negative(), and where to write the drawn j (may be null).
 struct FusedSampler {
   const long long* rated_rowptr;   // rejection sets: CSR over users, sorted columns

@@ -11,17 +11,6 @@
 
 #include "common.h"
 
-namespace qrec {
-int launch_bpr_batch(float* P, float* Q, int d, long long n, const int* u, const int* i,
-                     const int* j, float lr, float reg_u, float reg_i, double* loss,
-                     cudaStream_t st);
-int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
-                     const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i, double* loss,
-                     bool sample, const int64_t* rated_rowptr, const int32_t* rated_cols, int32_t num_items,
-                     uint64_t seed, uint32_t epoch, int32_t* j_out, long long trip_off, cudaStream_t st,
-                     const uint32_t* rated_sig = nullptr);
-}
-
 struct qrec_ctx {
   int device = 0;
   long long chunk = 0;
@@ -156,7 +145,7 @@ int qrec_bpr_epoch_usermajor_host(qrec_ctx* c, float* P, float* Q, int32_t d, in
       const int rc = qrec::launch_usermajor(P + (size_t)ua * d, Q, d, ub - ua, m, c->rp_slot[r], c->slot[r], nullptr, lr,
                                             reg_u, reg_i, c->dev_loss, true, dev_rated_rowptr + ua, dev_rated_cols,
                                             num_items, seed, epoch, nullptr, t0, c->compute,
-                                            c->rated_sig ? c->rated_sig + (size_t)ua * 16 : nullptr);
+                                            c->rated_sig ? c->rated_sig + (size_t)ua * 16 : nullptr, false);
       if (rc != QREC_OK) return rc;
     }
     QREC_CUDA(cudaEventRecord(c->freed[r], c->compute));

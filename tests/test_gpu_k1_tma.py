@@ -1,11 +1,13 @@
-"""qrec_bpr_epoch_usermajor_tma_f32 (csrc/bpr_tma.cu): the fused user-major epoch with the item rows staged through
-shared memory by cp.async.bulk + mbarrier.  It must draw exactly the negatives of the stand-alone Philox sampler
-(bit-exact index parity) and apply the same updates as qrec_bpr_epoch_usermajor_f32 (compared at a small learning
-rate, where the order in which concurrent item deltas land is second order), on ragged inputs too."""
+"""qrec_bpr_epoch_usermajor_tma_f32: the fused user-major epoch with the item rows staged through shared memory by
+cp.async.bulk + mbarrier (the TMA fetch of the user-major kernel body in csrc/bpr_kernels.cu).  It must draw exactly
+the negatives of the stand-alone Philox sampler (bit-exact index parity) and apply the same updates as
+qrec_bpr_epoch_usermajor_f32, on ragged inputs and at the benchmark learning rate."""
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
+
+LR, REG = 0.01, 0.001          # bench.py's learning rate and regularisation
 
 
 @pytest.fixture(scope='module')
@@ -52,6 +54,30 @@ def test_tma_epoch_equals_ldg_epoch(torch, E, nu, ni, maxdeg):
     assert float((dPa - dPb).abs().max()) <= 0.02 * float(dPa.abs().max())
     assert float((dQa - dQb).abs().max()) <= 0.02 * float(dQa.abs().max())
     assert abs(la.item() - lb.item()) <= 1e-4 * abs(la.item())
+
+
+def test_tma_epoch_equals_ldg_epoch_at_benchmark_rate(torch, E):
+    """On the schedule of test_usermajor_epoch_is_the_same_every_run (tests/test_gpu_bpr.py) the staged epoch reads
+    the same wave snapshots as the LDG epoch, so the two agree up to the summation order of the scatter-adds.  A
+    staged kernel that read the live item table while other lane groups added into it would miss by far more."""
+    from qrec_b200 import synthetic
+    dev = torch.device('cuda', 0)
+    users, items, deg, d = 200_000, 20_000, 20, 64
+    data = synthetic.make_interactions(users, items, deg, device=dev, seed=5)
+    runs = []
+    for epoch in (E.bpr_epoch_usermajor, E.bpr_epoch_usermajor_tma):
+        P, Q = synthetic.init_tables(users, items, d, seed=6, device=dev)
+        loss = torch.zeros(1, dtype=torch.float64, device=dev)
+        epoch(P, Q, data['sorted_rowptr'], data['i'], data['sorted_rowptr'], data['sorted_cols'], items, 77, 0, LR, REG, REG,
+              loss)
+        torch.cuda.synchronize()
+        runs.append((P.cpu(), Q.cpu(), loss.item()))
+    P0, Q0 = synthetic.init_tables(users, items, d, seed=6, device=dev)
+    for k, X0 in ((0, P0.cpu()), (1, Q0.cpu())):
+        update = float((runs[0][k] - X0).abs().max())
+        assert update > 0
+        assert float((runs[0][k] - runs[1][k]).abs().max()) <= 1e-4 * update
+    assert abs(runs[0][2] - runs[1][2]) <= 1e-9 * abs(runs[0][2])
 
 
 def test_tma_epoch_rejects_other_widths(torch, E):
