@@ -23,6 +23,7 @@
 #include "device.cuh"
 #include "philox.cuh"
 #include "bpr_step.cuh"
+#include "um_waves.cuh"
 
 namespace {
 
@@ -356,13 +357,11 @@ bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long
 // REDG.E.ADD.F32x4 as in the batch kernel.  Per triple: 2 row loads + 2 row REDs instead of 3 + 3.
 // Input: CSR over users (rowptr), i[] / j[] in that order.
 // ------------------------------------------------------------------------------------------
-// Work is cut into chunks of CH consecutive triples of the CSR order; a chunk takes the users whose first
-// triple lies inside it, so every user is processed whole by one lane group (P[u] register-resident,
-// updated sequentially, one row RED at the end) -- except at the ends of the launch, which are cut
-// where the caller cut them.  The chunks run in waves (ch_begin..ch_end);
-// inside a wave the item rows are READ from Qr, the table as it was when the wave started, and
-// scatter-added into Q.  Nothing a triple reads depends on timing: the result is the same every run up
-// to the summation order of the float REDs, and an item row is read at most about one wave late.
+// The launch runs in waves (um_waves.cuh); inside a wave the item rows are READ from Qr, the table as it was when
+// the wave started, and scatter-added into Q.  Lane group g of a wave's launch takes the wave's users ua + g,
+// ua + g + ngroups, ... and runs each one whole (P[u] register-resident, updated sequentially, one row RED at the
+// end).  Nothing a triple reads depends on timing: the result is the same every run up to the summation order of
+// the float REDs, and an item row is read at most about one wave late.
 // SAMPLE: the negatives are drawn inside the kernel (lane l draws the negative of triple base+l with
 // the same Philox counter as the stand-alone sampler, so both give identical j) instead of being
 // read from j[] (FusedSampler, philox.cuh); they are optionally written to j_out.
@@ -372,7 +371,6 @@ bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long
 // signalled on the slot's mbarrier and the lanes read their slices with LDS.128, so the gathers leave the
 // LSU/L1TEX path, which then carries only the scatter-adds.  Two slots per lane group: the rows of the next G
 // triples are requested while the current G are computed.
-constexpr int UM_CH = 32;                                    // triples per chunk
 constexpr int UM_STAGE_FLOATS = 2 * 4 * 64;                  // one slot: the 2 x G rows of G = 4 triples, d = 64
 constexpr int UM_STAGE_GROUPS = 16;                          // lane groups of 16 lanes in a 256-thread CTA
 constexpr int UM_STAGE_SMEM = UM_STAGE_GROUPS * 2 * (UM_STAGE_FLOATS * 4 + 8);   // two slots + two mbarriers per group
@@ -383,22 +381,22 @@ __device__ __forceinline__ void bulk_row_load(float* smem_dst, const float* gsrc
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(smem_u32(bar)) : "memory");
 }
 
-template <int LPR, int G, int CH, bool FULL, bool SAMPLE, bool SIG, bool TMA>   // FULL: d == 4*LPR (every lane owns a slice)
+template <int LPR, int G, bool FULL, bool SAMPLE, bool SIG, bool TMA>   // FULL: d == 4*LPR (every lane owns a slice)
 __device__ __forceinline__ void
-usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, int n_users,
-                long long n, long long ch_begin, long long ch_end, const long long* __restrict__ rowptr,
-                const int* __restrict__ i, const int* __restrict__ j, float lr,
-                float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
-                const uint32_t* __restrict__ rated_sig) {
+usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, long long n,
+                const int* __restrict__ wave_user, const long long* __restrict__ rowptr, const int* __restrict__ i,
+                const int* __restrict__ j, float lr, float reg_u, float reg_i, double* loss, FusedSampler fs,
+                long long trip_off, const uint32_t* __restrict__ rated_sig) {
   // rowptr holds GLOBAL triple offsets; i/j are indexed relative to trip_off (a chunk of users of a
   // larger epoch: the host pipeline stages one chunk at a time).  Philox counters use global indices.
+  // wave_user[0 .. 1]: the wave's users [ua, ub).
   static_assert(!TMA || (LPR == 16 && G == 4 && FULL), "the TMA fetch is laid out for d = 64, G = 4");
   constexpr int GPW = 32 / LPR;
   const int lane = threadIdx.x & 31;
   const int sub = lane / LPR, l = lane % LPR;
   const unsigned gmask = (LPR == 32) ? 0xffffffffu : (((1u << LPR) - 1u) << (sub * LPR));
-  const long long group = (((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * GPW + sub;
-  const long long ngroups = (((long long)gridDim.x * blockDim.x) >> 5) * GPW;
+  const int group = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * GPW + sub;
+  const int ngroups = (int)((gridDim.x * blockDim.x) >> 5) * GPW;
   const int d = FULL ? LPR * 4 : nvec * 4;
   const bool act = FULL ? true : (l < nvec);
   const float a_u = lr * reg_u, a_i = lr * reg_i;
@@ -419,66 +417,33 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
   }
-  // user of triple t: smallest r with rowptr[r+1] > t (LPR-ary search by the lane group)
-  auto user_of = [&](long long t) {
-    int a = 0, b = n_users - 1;
-    while (a < b) {
-      const int len = b - a + 1;
-      const int step = (len + LPR - 1) / LPR;
-      int pp = a + (l + 1) * step - 1;
-      if (pp > b) pp = b;
-      const bool pred = (__ldg(rowptr + pp + 1) - trip_off) > t;
-      const unsigned bal = (__ballot_sync(gmask, pred) & gmask) >> (sub * LPR);
-      const int f = __ffs(bal) - 1;
-      int pf = a + (f + 1) * step - 1;
-      if (pf > b) pf = b;
-      a = a + f * step;
-      b = pf;
-    }
-    return a;
-  };
-  for (long long ch = ch_begin + group; ch < ch_end; ch += ngroups) {
-    // the users whose first triple lies in [ch * CH, ch * CH + CH): a user cut by the chunk edge belongs to the
-    // chunk it starts in (the launch's own ends stay where they are)
-    long long lo = ch * CH;
-    long long hi = (lo + CH) < n ? (lo + CH) : n;
-    int uu = user_of(lo);
-    if (lo > 0 && __ldg(rowptr + uu) - trip_off < lo) {
-      lo = __ldg(rowptr + uu + 1) - trip_off;
-      ++uu;
-    }
-    if (hi < n) {
-      const int ub = user_of(hi);
-      if (__ldg(rowptr + ub) - trip_off < hi) {
-        const long long e = __ldg(rowptr + ub + 1) - trip_off;
-        hi = e < n ? e : n;
-      }
-    }
+  const int ub = __ldg(wave_user + 1);
+  for (int uu = __ldg(wave_user) + group; uu < ub; uu += ngroups) {
+    // the launch's first and last users are cut where the caller cut the launch
+    long long lo = __ldg(rowptr + uu) - trip_off, hi = __ldg(rowptr + uu + 1) - trip_off;
+    lo = lo > 0 ? lo : 0;
+    hi = hi < n ? hi : n;
     if (lo >= hi) continue;
-    long long uend = __ldg(rowptr + uu + 1) - trip_off;
     float* prow = P + (size_t)uu * d + l * 4;
     float4 p = act ? *reinterpret_cast<const float4*>(prow) : make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 p0 = p;
+    long long rated_lo = 0, rated_hi = 0;
+    if (SAMPLE) {
+      rated_lo = __ldg(fs.rated_rowptr + uu);
+      rated_hi = __ldg(fs.rated_rowptr + uu + 1);
+    }
     for (long long base = lo; base < hi; base += LPR) {
       const int m = (hi - base) < LPR ? (int)(hi - base) : LPR;
       int mi = 0, mj = 0;
       if (l < m) {
         mi = __ldg(i + base + l);
         if (SAMPLE) {
-          // user of triple base+l: walk forward from the group's current user
-          int us = uu;
-          long long ue = uend;
-          while (ue <= base + l) {
-            ++us;
-            ue = __ldg(rowptr + us + 1) - trip_off;
-          }
           if (SIG)
             mj = qrec::sample_negative_sig(base + l + trip_off, fs.epoch, fs.seed_lo, fs.seed_hi, fs.num_items,
-                                           fs.rated_cols, __ldg(fs.rated_rowptr + us), __ldg(fs.rated_rowptr + us + 1),
-                                           rated_sig + (size_t)us * qrec::RATED_SIG_WORDS);
+                                           fs.rated_cols, rated_lo, rated_hi,
+                                           rated_sig + (size_t)uu * qrec::RATED_SIG_WORDS);
           else
             mj = qrec::sample_negative(base + l + trip_off, fs.epoch, fs.seed_lo, fs.seed_hi, fs.num_items, fs.rated_cols,
-                                       __ldg(fs.rated_rowptr + us), __ldg(fs.rated_rowptr + us + 1));
+                                       rated_lo, rated_hi);
           if (fs.j_out != nullptr) fs.j_out[base + l] = mj;
         } else {
           mj = __ldg(j + base + l);
@@ -525,18 +490,7 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
         if constexpr (TMA) __syncwarp(gmask);         // the slot may be requested again G triples on
 #pragma unroll
         for (int f = 0; f < G; ++f) {
-          const long long t = base + t0 + f;
           if (t0 + f < m) {                              // uniform inside the lane group
-            if (t >= uend) {                             // next user: flush P delta, load the new row
-              if (act) red_add_v4(prow, make_float4(p.x - p0.x, p.y - p0.y, p.z - p0.z, p.w - p0.w));
-              do {
-                ++uu;
-                uend = __ldg(rowptr + uu + 1) - trip_off;
-              } while (uend <= t);
-              prow = P + (size_t)uu * d + l * 4;
-              p = act ? *reinterpret_cast<const float4*>(prow) : make_float4(0.f, 0.f, 0.f, 0.f);
-              p0 = p;
-            }
             float x = dot4(p, qi[f]) - dot4(p, qj[f]);
             x = group_sum<LPR>(x, gmask);
             const float s = fast_sigmoid(x);
@@ -552,42 +506,54 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
         }
       }
     }
-    if (act) red_add_v4(prow, make_float4(p.x - p0.x, p.y - p0.y, p.z - p0.z, p.w - p0.w));
+    if (act) {
+      // only this lane group touches P[u] in the launch: the row still holds what p was loaded from
+      const float4 p0 = __ldcg(reinterpret_cast<const float4*>(prow));
+      red_add_v4(prow, make_float4(p.x - p0.x, p.y - p0.y, p.z - p0.z, p.w - p0.w));
+    }
   }
   block_add_loss(lsum, loss);
 }
 
-template <int LPR, int G, int CH, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>
+template <int LPR, int G, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>
 __global__ void __launch_bounds__(256, MINB)
-bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, int n_users,
-                         long long n, long long ch_begin, long long ch_end, const long long* __restrict__ rowptr,
-                         const int* __restrict__ i, const int* __restrict__ j, float lr,
-                         float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
-                         const uint32_t* __restrict__ rated_sig) {
-  usermajor_epoch<LPR, G, CH, FULL, SAMPLE, SIG, false>(P, Q, Qr, nvec, n_users, n, ch_begin, ch_end, rowptr, i, j, lr,
-                                                         reg_u, reg_i, loss, fs, trip_off, rated_sig);
+bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, long long n,
+                         const int* __restrict__ wave_user, const long long* __restrict__ rowptr,
+                         const int* __restrict__ i, const int* __restrict__ j, float lr, float reg_u, float reg_i,
+                         double* loss, FusedSampler fs, long long trip_off, const uint32_t* __restrict__ rated_sig) {
+  usermajor_epoch<LPR, G, FULL, SAMPLE, SIG, false>(P, Q, Qr, nvec, n, wave_user, rowptr, i, j, lr, reg_u, reg_i, loss, fs,
+                                                    trip_off, rated_sig);
 }
 
 // d = 64 with fused sampling, item rows staged in shared memory (UM_STAGE_SMEM bytes of dynamic shared memory)
 __global__ void __launch_bounds__(256, 3)
 bpr_sgd_usermajor_tma_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec,
-                             int n_users, long long n, long long ch_begin, long long ch_end,
-                             const long long* __restrict__ rowptr, const int* __restrict__ i, const int* __restrict__ j,
-                             float lr, float reg_u, float reg_i, double* loss, FusedSampler fs, long long trip_off,
-                             const uint32_t* __restrict__ rated_sig) {
-  usermajor_epoch<16, 4, UM_CH, true, true, false, true>(P, Q, Qr, nvec, n_users, n, ch_begin, ch_end, rowptr, i, j,
-                                                         lr, reg_u, reg_i, loss, fs, trip_off, rated_sig);
+                             long long n, const int* __restrict__ wave_user, const long long* __restrict__ rowptr,
+                             const int* __restrict__ i, const int* __restrict__ j, float lr, float reg_u, float reg_i,
+                             double* loss, FusedSampler fs, long long trip_off, const uint32_t* __restrict__ rated_sig) {
+  usermajor_epoch<16, 4, true, true, false, true>(P, Q, Qr, nvec, n, wave_user, rowptr, i, j, lr, reg_u, reg_i, loss, fs,
+                                                  trip_off, rated_sig);
 }
 
 using UserMajorKernel = decltype(&bpr_sgd_usermajor_tma_kernel);
 
-// The instantiation for lane groups of LPR lanes: FULL when d = 4 LPR; the signature pre-test only then.
+// The instantiation for lane groups of LPR lanes: FULL when d = 4 LPR; the signature pre-test only then.  With FULL
+// fused sampling, G = 2 triples in flight fit 64 registers, so four 256-thread CTAs are resident per SM instead of
+// three: 8,448 lane groups on an H100, one round for the 8,000 users of a benchmark wave (400K triples / 50).
 template <int LPR>
 UserMajorKernel usermajor_kernel(int nvec, bool sample, bool sig) {
   if (nvec != LPR)
-    return sample ? bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, false, true> : bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, false, false>;
-  if (sig) return bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, true, true, 3, true>;
-  return sample ? bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, true, true> : bpr_sgd_usermajor_kernel<LPR, 4, UM_CH, true, false>;
+    return sample ? bpr_sgd_usermajor_kernel<LPR, 4, false, true> : bpr_sgd_usermajor_kernel<LPR, 4, false, false>;
+  if (sig) return bpr_sgd_usermajor_kernel<LPR, 2, true, true, 4, true>;
+  return sample ? bpr_sgd_usermajor_kernel<LPR, 2, true, true, 4> : bpr_sgd_usermajor_kernel<LPR, 4, true, false>;
+}
+
+// wave_user[w] = first user of wave w, w = 0 .. nwaves (um_waves.cuh)
+__global__ void __launch_bounds__(256)
+um_wave_table_kernel(const long long* __restrict__ rowptr, int n_users, long long n, long long trip_off,
+                     long long wave_chunks, long long nwaves, int* __restrict__ wave_user) {
+  const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (w <= nwaves) wave_user[w] = um_wave_first_user(rowptr, n_users, n, trip_off, wave_chunks, w);
 }
 
 // one warp per user: bit (c & 511) of the user's 16-word signature for every rated column c
@@ -762,35 +728,34 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
   const int smem = tma ? UM_STAGE_SMEM : 0;
   if (tma) QREC_CUDA(allow_dynamic_smem((const void*)kernel, smem));
   // Grid = exactly the CTAs that are resident at once (occupancy API per instantiation); the stream is swept in
-  // waves, each reading the item table as the previous waves left it (a snapshot copied on the stream).
+  // waves (um_waves.cuh), each reading the item table as the previous waves left it (a snapshot copied on the stream).
   int occ = 3;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, 256, smem) != cudaSuccess || occ < 1) occ = 3;
-  const long long nchunks = (n + UM_CH - 1) / UM_CH;
   const long long per_block = 8 * (32 / lpr);                                 // lane groups per CTA
-  const int grid = capped_grid((nchunks + per_block - 1) / per_block, occ);
+  const long long max_users = n < n_users ? n : n_users;                      // users with triples in the launch
+  const int grid = capped_grid((max_users + per_block - 1) / per_block, occ);
   const size_t q_bytes = (size_t)num_items * d * sizeof(float);
-  // Wave size in triples: no more than 4 x the item rows, so an item row is read only a few of its own updates late.
-  // On a small table (snapshot copy under 8 MB, about the cost of a launch) at least 64 waves per launch: on a small
-  // data set the hot items recur within a few hundred triples.  On a large one the wave is long enough that the
-  // copy stays under 1/8 of the wave's algorithmic bytes (24 d + 12 per triple).
-  const long long copy_bytes = 2 * (long long)q_bytes;
-  const long long copy_floor = copy_bytes > (8LL << 20) ? 8 * copy_bytes / (24LL * d + 12) : 0;
-  long long wave_triples = n / 64 > copy_floor ? n / 64 : copy_floor;
-  if (wave_triples > 4LL * num_items) wave_triples = 4LL * num_items;
-  const long long wave = wave_triples / UM_CH > 1 ? wave_triples / UM_CH : 1;      // in chunks
+  const long long wave = um_wave_chunks(n, num_items, d);
+  const long long nwaves = um_num_waves(n, wave);
   float* Qr = nullptr;                                // the item table as the current wave started (stream-ordered scratch)
+  int* wave_user = nullptr;                           // first user of every wave, and one past the last (nwaves + 1)
   QREC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&Qr), q_bytes, st));
   const int rc = [&]() -> int {
-    for (long long c0 = 0; c0 < nchunks; c0 += wave) {
+    QREC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&wave_user), sizeof(int) * (size_t)(nwaves + 1), st));
+    um_wave_table_kernel<<<(unsigned)((nwaves + 256) / 256), 256, 0, st>>>(reinterpret_cast<const long long*>(rowptr), n_users,
+                                                                          n, trip_off, wave, nwaves, wave_user);
+    QREC_CUDA(cudaGetLastError());
+    count_launch();
+    for (long long w = 0; w < nwaves; ++w) {
       QREC_CUDA(cudaMemcpyAsync(Qr, Q, q_bytes, cudaMemcpyDeviceToDevice, st));
-      const long long c1 = (c0 + wave) < nchunks ? (c0 + wave) : nchunks;
-      kernel<<<grid, 256, smem, st>>>(P, Q, Qr, nvec, n_users, n, c0, c1, reinterpret_cast<const long long*>(rowptr), i, j,
-                                      lr, reg_u, reg_i, loss, fs, trip_off, rated_sig);
+      kernel<<<grid, 256, smem, st>>>(P, Q, Qr, nvec, n, wave_user + w, reinterpret_cast<const long long*>(rowptr), i, j, lr,
+                                      reg_u, reg_i, loss, fs, trip_off, rated_sig);
       QREC_CUDA(cudaGetLastError());
-      if (c1 < nchunks) count_launch();
+      if (w + 1 < nwaves) count_launch();
     }
     return QREC_OK;
   }();
+  if (wave_user != nullptr) QREC_CUDA(cudaFreeAsync(wave_user, st));
   QREC_CUDA(cudaFreeAsync(Qr, st));
   if (rc != QREC_OK) return rc;
   QREC_LAUNCH_CHECK();
