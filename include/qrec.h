@@ -684,6 +684,41 @@ int qrec_als_solve_rows_f64(double* dev_X, const double* dev_Z, const double* de
                             const double* dev_vals, double lambda, double alpha, double* dev_loss,
                             int32_t* dev_n_failed, void* stream);
 
+/* =====================================================================================
+ * K11 -- SVD++ (model/rating/SVDPlusPlus.py:26-88).  Tables P[num_users][d], Q, Y[num_items][d], Bu, Bi.  Per entry
+ * (u, i, r), with N(u) the user's distinct items (one CSR row) and w = |N(u)|:
+ *   pred = (sum_{N(u)} Y / w).Q[i] + P[u].Q[i] + mean + Bi[i] + Bu[u];   e = r - pred;   dev_loss += e^2
+ *   Bu[u], Bi[i] += lr*(e - regB*b);
+ *   w > 1:  Y[j] += lr*(e*Q[i]/(w-1) - regY*Y[j]) for j in N(u), j != i;   Q[i] += lr*e*sum_{j != i} Y[j] / (w-1)
+ *   P[u] += lr*(e*Q[i] - regU*P[u]);  Q[i] += lr*(e*P[u] - regI*Q[i])   (Q[i] after the implicit step, the new P[u])
+ * rowptr (int64 [num_users + 1]) / cols (int32): N(u) in the order of the user's row.
+ * ===================================================================================== */
+/* Parity mode: the entries (u[k], i[k], r[k]) one after another in array order, by ONE CTA (parallel inside an
+ * entry only), with the reference's evaluation order; float64 tables follow the reference to the grouping of the
+ * two dot products.  d: 1..256. */
+int qrec_svdpp_sgd_ordered_f64(double* dev_P, double* dev_Q, double* dev_Y, double* dev_Bu, double* dev_Bi, int32_t d,
+                               int64_t n, const int32_t* dev_u, const int32_t* dev_i, const double* dev_r,
+                               const int64_t* dev_rowptr, const int32_t* dev_cols, double lr, double reg_u,
+                               double reg_i, double reg_b, double reg_y, double global_mean, double* dev_loss,
+                               void* stream);
+int qrec_svdpp_sgd_ordered_f32(float* dev_P, float* dev_Q, float* dev_Y, float* dev_Bu, float* dev_Bi, int32_t d,
+                               int64_t n, const int32_t* dev_u, const int32_t* dev_i, const float* dev_r,
+                               const int64_t* dev_rowptr, const int32_t* dev_cols, float lr, float reg_u, float reg_i,
+                               float reg_b, float reg_y, float global_mean, double* dev_loss, void* stream);
+/* Throughput mode: one user-major epoch over the CSR's entries (cols, vals: each user's distinct items and their
+ * ratings), users taken from row_order[0..n_rows).  One lane group runs a user's entries in row order through the
+ * per-user closed form (csrc/svdpp_step.cuh), so a step moves Q[i] and Y[i] instead of all the user's Y rows; the
+ * Q / Y / Bi deltas are added back atomically, P[u] and Bu[u] are written once.
+ * d: multiple of 4, 4..128 (pad with zero columns; they stay zero).
+ * max_users_in_flight: 0 = fill the GPU; k > 0 = at most k users at a time.  Users in flight read each other's
+ * rows stale, like qrec_mf_sgd_batch_f32's entries: small or skewed data needs about (0.25/lr) / (share of the users
+ * who rated the most-rated item).  k = 1 applies the users one after another.  n_rows = 0 launches nothing. */
+int qrec_svdpp_epoch_usermajor_f32(float* dev_P, float* dev_Q, float* dev_Y, float* dev_Bu, float* dev_Bi, int32_t d,
+                                   int32_t n_rows, const int32_t* dev_row_order, const int64_t* dev_rowptr,
+                                   const int32_t* dev_cols, const float* dev_vals, float lr, float reg_u, float reg_i,
+                                   float reg_b, float reg_y, float global_mean, double* dev_loss,
+                                   int64_t max_users_in_flight, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

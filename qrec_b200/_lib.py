@@ -88,6 +88,13 @@ SIGNATURES = {
                                           vp, vp, vp]),
     'qrec_als_solve_rows_f64': (C.c_int, [vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double,
                                           vp, vp, vp]),
+    'qrec_svdpp_sgd_ordered_f64': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_double,
+                                             C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
+    'qrec_svdpp_sgd_ordered_f32': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_float,
+                                             C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp]),
+    'qrec_svdpp_epoch_usermajor_f32': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_float,
+                                                 C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, vp, C.c_int64,
+                                                 vp]),
     'qrec_bpr_sgd_batch_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float,
                                          C.c_float, C.c_float, vp, vp]),
     'qrec_bpr_sgd_batch_tma_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float,

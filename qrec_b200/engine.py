@@ -1057,3 +1057,57 @@ def als_solve_rows(X, Z, G, rowptr, cols, vals, lam, alpha, row_order, loss=None
             raise QRecError('als_solve_rows: %d row(s) with normal equations that are not positive definite were '
                             'left unchanged' % bad)
     return X
+
+
+# =============================================================================================
+# K11: SVD++ -- in-order parity epoch and user-major closed-form fast epoch
+# =============================================================================================
+def _svdpp_tables(P, Q, Y, Bu, Bi, dt):
+    d = P.shape[1]
+    if P.dim() != 2 or Q.dim() != 2 or Y.dim() != 2 or Q.shape[1] != d or Y.shape[1] != d:
+        raise QRecError('svdpp: P, Q, Y must be 2-D tables of one width')
+    if Y.shape[0] != Q.shape[0] or Bu.shape[0] != P.shape[0] or Bi.shape[0] != Q.shape[0]:
+        raise QRecError('svdpp: Y / Bi need one row per item of Q, Bu one per user of P')
+    return [_dev(t, dt, name) for t, name in ((P, 'P'), (Q, 'Q'), (Y, 'Y'), (Bu, 'Bu'), (Bi, 'Bi'))], d
+
+
+def svdpp_sgd_ordered(P, Q, Y, Bu, Bi, u, i, r, rowptr, cols, lr, reg_u, reg_i, reg_b, reg_y, global_mean, loss):
+    """Parity mode (SVDPlusPlus.py:30-61): the entries (u, i, r) one after another in array order on one CTA.
+    rowptr (int64 [num_users + 1]) / cols (int32): every user's distinct items in insertion order
+    (Rating.rating_csr('user')).  Tables float64 or float32 (all five alike, r likewise); loss: float64 [1], += sum e^2."""
+    torch = _torch()
+    dt = P.dtype
+    if dt not in (torch.float32, torch.float64):
+        raise QRecError('P must be float32 or float64, got %s' % dt)
+    if not (u.shape[0] == i.shape[0] == r.shape[0]):
+        raise QRecError('svdpp_sgd_ordered: u, i, r differ in length')
+    if rowptr.shape[0] != P.shape[0] + 1:
+        raise QRecError('svdpp_sgd_ordered: rowptr has %d entries for %d users' % (rowptr.shape[0], P.shape[0]))
+    (pP, pQ, pY, pBu, pBi), d = _svdpp_tables(P, Q, Y, Bu, Bi, dt)
+    fn = lib.qrec_svdpp_sgd_ordered_f64 if dt == torch.float64 else lib.qrec_svdpp_sgd_ordered_f32
+    check(fn(pP, pQ, pY, pBu, pBi, d, u.shape[0], _dev(u, torch.int32, 'u'), _dev(i, torch.int32, 'i'), _dev(r, dt, 'r'),
+             _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'), float(lr), float(reg_u), float(reg_i),
+             float(reg_b), float(reg_y), float(global_mean), _dev(loss, torch.float64, 'loss'), _stream()),
+          'qrec_svdpp_sgd_ordered')
+    return loss
+
+
+def svdpp_epoch_usermajor(P, Q, Y, Bu, Bi, rowptr, cols, vals, row_order, lr, reg_u, reg_i, reg_b, reg_y, global_mean,
+                          loss, max_users_in_flight=0):
+    """Throughput mode: one user-major epoch over the CSR (rowptr int64, cols int32, vals fp32: every user's distinct
+    items and ratings), users in `row_order` (int32; als_row_order gives longest first), fp32 tables whose width is
+    a multiple of 4 up to 128.  max_users_in_flight: 0 fills the GPU, k > 0 runs at most k users at a time."""
+    torch = _torch()
+    f32 = torch.float32
+    if rowptr.shape[0] != P.shape[0] + 1:
+        raise QRecError('svdpp_epoch_usermajor: rowptr has %d entries for %d users' % (rowptr.shape[0], P.shape[0]))
+    if cols.shape[0] != vals.shape[0]:
+        raise QRecError('svdpp_epoch_usermajor: cols and vals differ in length')
+    (pP, pQ, pY, pBu, pBi), d = _svdpp_tables(P, Q, Y, Bu, Bi, f32)
+    check(lib.qrec_svdpp_epoch_usermajor_f32(pP, pQ, pY, pBu, pBi, d, row_order.shape[0],
+                                             _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
+                                             _dev(cols, torch.int32, 'cols'), _dev(vals, f32, 'vals'), float(lr),
+                                             float(reg_u), float(reg_i), float(reg_b), float(reg_y), float(global_mean),
+                                             _dev(loss, torch.float64, 'loss'), int(max_users_in_flight), _stream()),
+          'qrec_svdpp_epoch_usermajor_f32')
+    return loss

@@ -143,6 +143,23 @@ def main():
                                  loss=loss)
         torch.cuda.synchronize()
         print('sanitize_all: + K10, launched', E.launch_count(), 'kernels')
+        # K11 (SVD++): the ordered kernel (both table types, one staged chunk and several) and the user-major epoch
+        # at every lane-group width, one user in flight and a full grid
+        rv = torch.rand(n, device='cuda') * 4
+        for dd, dt in ((10, torch.float64), (256, torch.float64), (37, torch.float32)):
+            T = [torch.rand(nu, dd, device='cuda', dtype=dt), torch.rand(ni, dd, device='cuda', dtype=dt),
+                 torch.rand(ni, dd, device='cuda', dtype=dt), torch.rand(nu, device='cuda', dtype=dt),
+                 torch.rand(ni, device='cuda', dtype=dt)]
+            E.svdpp_sgd_ordered(*T, dev(np.sort(u)), cols, rv.to(dt), rowptr, cols, 0.01, 0.01, 0.01, 0.1, 0.01, 3.0,
+                                loss)
+        for dd in (4, 32, 64, 128):
+            T = [torch.rand(nu, dd, device='cuda'), torch.rand(ni, dd, device='cuda'), torch.rand(ni, dd, device='cuda'),
+                 torch.rand(nu, device='cuda'), torch.rand(ni, device='cuda')]
+            for k in (1, 0):
+                E.svdpp_epoch_usermajor(*T, rowptr, cols, rv, order, 0.01, 0.01, 0.01, 0.1, 0.01, 3.0, loss,
+                                        max_users_in_flight=k)
+        torch.cuda.synchronize()
+        print('sanitize_all: + K11, launched', E.launch_count(), 'kernels')
 
 
 if __name__ == '__main__':
