@@ -273,6 +273,10 @@ int qrec_bpr_sgd_staged_f32(float* dev_P, int32_t d, int64_t n, const int32_t* d
 int qrec_sumsq_f32(const float* dev_x, int64_t n, double* dev_out, void* stream);
 int qrec_sumsq_f64(const double* dev_x, int64_t n, double* dev_out, void* stream);
 
+/* dev_dst[0 .. n) = dev_src[0 .. n): the item-table snapshot the user-major epoch takes before each wave (both
+ * tables kept in L2 at evict_last).  n a multiple of 4, both pointers 16-byte aligned, no overlap. */
+int qrec_table_snapshot_f32(const float* dev_src, float* dev_dst, int64_t n, void* stream);
+
 /* =====================================================================================
  * Replicated item table across GPUs (SURVEY 8e, BPR throughput mode: users range-partitioned, Q
  * replicated; the data-parallel form of the in-place item updates of BPR.py:50-52).  B is the table all

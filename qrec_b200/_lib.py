@@ -122,6 +122,7 @@ SIGNATURES = {
     'qrec_adj_subgraph_fill_f32': (C.c_int, [C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     'qrec_sumsq_f32': (C.c_int, [vp, C.c_int64, vp, vp]),
     'qrec_sumsq_f64': (C.c_int, [vp, C.c_int64, vp, vp]),
+    'qrec_table_snapshot_f32': (C.c_int, [vp, vp, C.c_int64, vp]),
     'qrec_ctx_create': (C.c_int, [C.c_int, C.c_int64, C.POINTER(vp)]),
     'qrec_ctx_destroy': (C.c_int, [vp]),
     'qrec_ctx_set_rated_signature': (C.c_int, [vp, vp]),

@@ -11,6 +11,60 @@ __device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
+// ---- L2 residency hints: data read once is streamed (evict_first, and no L1 allocation on loads) so that it does not
+// push out what should stay (evict_last).  A policy is a 64-bit register made once per thread by createpolicy.
+__device__ __forceinline__ unsigned long long l2_policy_evict_first() {
+  unsigned long long pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ unsigned long long l2_policy_evict_last() {
+  unsigned long long pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+// read-only loads under policy `pol`; the streamed ones do not allocate in L1
+__device__ __forceinline__ int ld_stream_s32(const int* p, unsigned long long pol) {
+  int v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ float ld_stream_f32(const float* p, unsigned long long pol) {
+  float v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ float4 ld_hint_v4(const float4* p, unsigned long long pol) {
+  float4 v;
+  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ float4 ld_stream_v4(const float4* p, unsigned long long pol) {
+  float4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ void st_hint_v4(float4* p, float4 v, unsigned long long pol) {
+  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w),
+               "l"(pol) : "memory");
+}
+// a read-only float4 that is not allocated in L1 (no L2 policy)
+__device__ __forceinline__ float4 ldg_no_l1_v4(const float4* p) {
+  float4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+  return v;
+}
+
+// ---- Programmatic dependent launch (sm_90).  In a kernel launched with programmatic stream serialization,
+// pdl_wait() returns once the previous kernel on the stream has completed and its memory operations are visible;
+// everything before it may overlap that kernel.  pdl_launch_dependents() lets the next such kernel on the stream be
+// launched before this one ends.  In a kernel launched normally both are no-ops.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 __device__ __forceinline__ float dot4(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
 
 // acc += s * x

@@ -34,37 +34,17 @@ __device__ __forceinline__ void store_row(float* __restrict__ Y, float* __restri
 
 // L2 residency hints (variant 6): the (col, val) arrays are read once and only pollute the L2, the gathered X rows are
 // what should stay -- stream the former (evict_first, no L1 allocation), pin the latter (evict_last).
-__device__ __forceinline__ unsigned long long l2_policy_evict_first() {
-  unsigned long long pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ unsigned long long l2_policy_evict_last() {
-  unsigned long long pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
 template <bool HINT>
 __device__ __forceinline__ int ld_index(const int* p, unsigned long long pol) {
-  if (!HINT) return __ldg(p);
-  int v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
-  return v;
+  return HINT ? qrec::ld_stream_s32(p, pol) : __ldg(p);
 }
 template <bool HINT>
 __device__ __forceinline__ float ld_value(const float* p, unsigned long long pol) {
-  if (!HINT) return __ldg(p);
-  float v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
-  return v;
+  return HINT ? qrec::ld_stream_f32(p, pol) : __ldg(p);
 }
 template <bool HINT>
 __device__ __forceinline__ float4 ld_row(const float4* p, unsigned long long pol) {
-  if (!HINT) return __ldg(p);
-  float4 v;
-  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
-  return v;
+  return HINT ? qrec::ld_hint_v4(p, pol) : __ldg(p);
 }
 
 // lock-step batches of G gathers (the production structure with G and the occupancy as parameters)
@@ -73,7 +53,8 @@ __global__ void __launch_bounds__(256, MINB)
 spmm_rowsplit_batch_kernel(int n_rows, const long long* __restrict__ rowptr, const int* __restrict__ cols,
                            const float* __restrict__ vals, const float* __restrict__ X, float* __restrict__ Y,
                            float* __restrict__ acc, float acc_scale) {
-  const unsigned long long pol_stream = HINT ? l2_policy_evict_first() : 0ULL, pol_keep = HINT ? l2_policy_evict_last() : 0ULL;
+  const unsigned long long pol_stream = HINT ? qrec::l2_policy_evict_first() : 0ULL,
+                           pol_keep = HINT ? qrec::l2_policy_evict_last() : 0ULL;
   const int lane = threadIdx.x & 31;
   const int sub = lane / LPR, l = lane % LPR;
   const unsigned gmask = ((1u << LPR) - 1u) << (sub * LPR);

@@ -552,6 +552,17 @@ def sumsq(x, out):
     return out
 
 
+def table_snapshot(src, dst):
+    """dst = src for contiguous fp32 tables of the same size (csrc/bpr_kernels.cu: the user-major epoch's per-wave copy
+    of the item table)."""
+    torch = _torch()
+    if src.numel() != dst.numel():
+        raise QRecError('table_snapshot: src has %d elements, dst %d' % (src.numel(), dst.numel()))
+    check(lib.qrec_table_snapshot_f32(_dev(src, torch.float32, 'src'), _dev(dst, torch.float32, 'dst'), src.numel(),
+                                      _stream()), 'qrec_table_snapshot_f32')
+    return dst
+
+
 class HostPipeline(object):
     """qrec_ctx: copy/compute pipeline for epochs whose triples live in host memory."""
 

@@ -2,7 +2,9 @@
 
 The epoch is bench.py's: 1M users x 100K items x 50 positives per user, d = 64, fp32, fused Philox sampling with the
 rated-set signature pre-test (bpr_epoch_usermajor_sig), then |P|^2 and |Q|^2.  launch_usermajor runs it as waves,
-each a snapshot copy of the item table (Q -> Qr, device to device) followed by one user-major kernel launch.
+each a snapshot copy of the item table (Q -> Qr: um_snapshot_kernel, or a device-to-device copy in older builds)
+followed by one user-major kernel launch.  The waves of a call are chained with programmatic dependent launch, so
+neighbouring activities may overlap; `seams` is the epoch time not covered by a user-major launch or another kernel.
 
 After 3 warm-up epochs, one epoch is traced under torch.profiler (CUDA activities; the trace is written to
 OUT/trace.json) and reported as: total epoch time, the Qr copies (sum, median), the user-major launches (sum, median,
@@ -82,7 +84,8 @@ def main():
     acts = sorted((e for e in evs if e.get('ph') == 'X' and e.get('cat') in ('kernel', 'gpu_memcpy', 'gpu_memset')),
                   key=lambda e: e['ts'])
     assert acts, 'no device activity in the trace'
-    is_copy = lambda e: e['cat'] == 'gpu_memcpy' and 'DtoD' in e['name']             # noqa: E731
+    is_copy = lambda e: ((e['cat'] == 'gpu_memcpy' and 'DtoD' in e['name'])           # noqa: E731
+                         or (e['cat'] == 'kernel' and 'um_snapshot_kernel' in e['name']))
     is_k1 = lambda e: e['cat'] == 'kernel' and 'bpr_sgd_usermajor' in e['name']       # noqa: E731
     copies = np.array([e['dur'] for e in acts if is_copy(e)])
     k1 = np.array([e['dur'] for e in acts if is_k1(e)])
@@ -97,6 +100,7 @@ def main():
         'k1_us': {'sum': float(k1.sum()), 'median': float(np.median(k1)), 'min': float(k1.min()), 'max': float(k1.max())},
         'other_device_us': float(other),
         'gaps_us': float(gaps.sum()),
+        'seams_us': float(ends.max() - acts[0]['ts'] - k1.sum() - other),
         'k1_kernel': k1_names,
     }
 
@@ -122,6 +126,7 @@ def main():
         'user-major launches', p['k1_us']['sum'], p['k1_us']['median'], p['k1_us']['min'], p['k1_us']['max']))
     print('  %-28s %10.1f us' % ('other kernels and copies', p['other_device_us']))
     print('  %-28s %10.1f us' % ('gaps between activities', p['gaps_us']))
+    print('  %-28s %10.1f us' % ('seams (epoch - launches)', p['seams_us']))
     print('%d epochs, CUDA events, no profiler: %.3f ms per epoch = %.4g triples/s   (%s)' % (
         args.epochs, ms, rep['events']['triples_per_s'], on))
 
