@@ -294,10 +294,6 @@ int qrec_table_reduce_scatter_p2p_f32(const float* const* peer_D, int32_t world,
                                       void* stream);
 int qrec_table_gather_merge_p2p_f32(const float* const* peer_S, int32_t world, float* dev_Q, float* dev_B,
                                     const float* dev_D, int64_t n, void* stream);
-/* Plain all-gather of the reduce-scattered sums (peer_S as above): out[k] = S_owner(k)[k].  With
- * qrec_table_reduce_scatter_p2p_f32 and a barrier in between this is an all-reduce over peer memory (used for the
- * [I, d] item block of the user-sharded LightGCN / SimGCL layers, SURVEY 8e). */
-int qrec_table_all_gather_p2p_f32(const float* const* peer_S, int32_t world, float* dev_out, int64_t n, void* stream);
 
 /* K8 (SURVEY 8f-1): batched ranking evaluation, replaces the per-user loop of Recommender.evalRanking
  * (base/recommender.py:143-152) + find_k_largest (util/qmath.py:134-146).  For every row r of the block:
@@ -391,19 +387,11 @@ int qrec_spmm_csr_f32(int32_t n_rows, int64_t nnz, const int64_t* dev_rowptr, co
                       const float* dev_vals, const float* dev_X, float* dev_Y, int32_t d,
                       float* dev_acc, float acc_scale, void* stream);
 /* Same product with plain row partitioning (one lane group per row, no atomics, bit-reproducible
- * summation order).  qrec_spmm_csr_f32 balances by non-zeros instead and is the default. */
+ * summation order).  qrec_spmm_csr_f32 balances by non-zeros instead and is the default.  d = 64 runs
+ * its own specialisation (a half warp per row, 8 gathered rows in flight per lane, 4 CTAs per SM). */
 int qrec_spmm_csr_rowsplit_f32(int32_t n_rows, int64_t nnz, const int64_t* dev_rowptr, const int32_t* dev_cols,
                                const float* dev_vals, const float* dev_X, float* dev_Y, int32_t d,
                                float* dev_acc, float acc_scale, void* stream);
-
-/* Experiment entry point (d = 64): the row-split product with the number of outstanding gathers and
- * the occupancy as a parameter -- variant 0 = the production configuration, 1/2 = 5/6 CTAs per SM,
- * 3 = 16 gathers per batch, 4/5 = software-pipelined double buffers (csrc/spmm_variants.cu).  The
- * floating-point order is the production kernel's, so every variant returns its bits.
- * STATUS: compiled, not yet run on hardware. */
-int qrec_spmm_csr_rowsplit_var_f32(int32_t variant, int32_t n_rows, const int64_t* dev_rowptr,
-                                   const int32_t* dev_cols, const float* dev_vals, const float* dev_X,
-                                   float* dev_Y, int32_t d, float* dev_acc, float acc_scale, void* stream);
 
 /* Sparse-source product (the first backward layer of a minibatch step: the loss gradient touches at
  * most 3B rows).  (rowptr, cols, vals) is a CSR whose ROWS are source nodes and whose column ids index

@@ -68,7 +68,6 @@ SIGNATURES = {
     'qrec_rated_signature_build': (C.c_int, [C.c_int32, vp, vp, vp, vp]),
     'qrec_bpr_epoch_usermajor_sig_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_int32,
                                                    C.c_uint64, C.c_uint32, vp, C.c_float, C.c_float, C.c_float, vp, vp]),
-    'qrec_spmm_csr_rowsplit_var_f32': (C.c_int, [C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, C.c_float, vp]),
     'qrec_mf_order_prepare': (C.c_int, [C.c_int64, c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, c_i32p]),
     'qrec_mf_order_depth': (C.c_int64, [C.c_int64, c_i32p, c_i32p, C.c_int32, C.c_int32]),
     'qrec_mf_sgd_ordered_f32': (C.c_int, [C.c_int32, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp,
@@ -111,7 +110,6 @@ SIGNATURES = {
     'qrec_table_delta_f32': (C.c_int, [vp, vp, vp, vp, C.c_int64, vp]),
     'qrec_table_merge_f32': (C.c_int, [vp, vp, vp, vp, C.c_int64, vp]),
     'qrec_table_reduce_scatter_p2p_f32': (C.c_int, [C.POINTER(vp), C.c_int32, C.c_int32, vp, C.c_int64, vp]),
-    'qrec_table_all_gather_p2p_f32': (C.c_int, [C.POINTER(vp), C.c_int32, vp, C.c_int64, vp]),
     'qrec_table_gather_merge_p2p_f32': (C.c_int, [C.POINTER(vp), C.c_int32, vp, vp, vp, C.c_int64, vp]),
     'qrec_score_topn_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, C.c_int32, vp, vp, C.c_float, C.c_int32, vp, vp, vp]),
     'qrec_score_topn_tc_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, C.c_int32, vp, vp, C.c_float, C.c_int32, vp, vp, vp]),

@@ -40,9 +40,8 @@ class DeviceCSR(object):
         50-entry and on 500-entry rows at the same time keep neither table's rows in the L2, so the halves are launched one
         after the other.  With a split row `matmul` issues the row-split
         kernel once per half; rows, arithmetic and results are those of the single launch."""
-        import os
         n = self.shape[0]
-        self.split_row = int(row) if (row is not None and 0 < int(row) < n and os.environ.get('QREC_SPMM_SPLIT', '1') != '0') else None
+        self.split_row = int(row) if (row is not None and 0 < int(row) < n) else None
 
     def _finish(self, shape, rowptr, cols, vals):
         self.shape = shape

@@ -11,35 +11,14 @@ __device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
-// ---- L2 residency hints: data read once is streamed (evict_first, and no L1 allocation on loads) so that it does not
-// push out what should stay (evict_last).  A policy is a 64-bit register made once per thread by createpolicy.
-__device__ __forceinline__ unsigned long long l2_policy_evict_first() {
-  unsigned long long pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
+// ---- L2 residency hints: tables that should stay in L2 are read and written under an evict_last policy, and loads
+// that are not reused do not allocate in L1.  A policy is a 64-bit register made once per thread by createpolicy.
 __device__ __forceinline__ unsigned long long l2_policy_evict_last() {
   unsigned long long pol;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
-// read-only loads under policy `pol`; the streamed ones do not allocate in L1
-__device__ __forceinline__ int ld_stream_s32(const int* p, unsigned long long pol) {
-  int v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ float ld_stream_f32(const float* p, unsigned long long pol) {
-  float v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ float4 ld_hint_v4(const float4* p, unsigned long long pol) {
-  float4 v;
-  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
-  return v;
-}
+// a read-only load under policy `pol` that does not allocate in L1
 __device__ __forceinline__ float4 ld_stream_v4(const float4* p, unsigned long long pol) {
   float4 v;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"

@@ -2,11 +2,12 @@
 // (reference: model/ranking/LightGCN.py:11-41, util/loss.py:3-6, base/graphRecommender.py:10-39).
 //
 //   K2  spmm_csr_balanced_kernel Y = A X (+ fused layer accumulation), CSR, nnz-balanced chunks
-//       spmm_csr_kernel          the plain row-partitioned variant (kept for comparison):
+//       spmm_csr_kernel          the row-partitioned product, for graphs without very long rows:
 //                                LPR lanes own one row of Y (d=64: a half warp, float4 per lane);
 //                                the lane group streams the row's (col,val) pairs coalesced,
-//                                broadcasts them with group-masked shuffles and keeps 4 gathered
+//                                broadcasts them with group-masked shuffles and keeps 4 or 8 gathered
 //                                X rows in flight per lane.
+//       spmm_csr_d64_kernel      its d = 64 specialisation, 4 CTAs per SM.
 //   K3  bpr_grad_scatter_kernel  gather 3 rows of the propagated tables, -ln(sigmoid(y)+eps)
 //                                + batch L2, gradient scatter-added (REDG.ADD.F32x4) into the
 //                                dense gradient buffers.
@@ -14,8 +15,6 @@
 //                                the ApplyAdam form  m += (g-m)(1-b1); v += (g*g-v)(1-b2);
 //                                var -= m*alpha/(sqrt(v)+eps).
 #include <cmath>
-
-#include <cstdlib>
 
 #include "common.h"
 #include "device.cuh"
@@ -101,6 +100,73 @@ spmm_csr_kernel(int n_rows, const long long* __restrict__ rowptr, const int* __r
         }
       }
     }
+  }
+}
+
+// Y[r] = a (lane l's float4 of a d = 64 row); acc[r] += acc_scale * a.  A function of its own: written inline, nvcc
+// allocates the kernel's registers in a different order.
+__device__ __forceinline__ void store_row_d64(float* __restrict__ Y, float* __restrict__ acc, float acc_scale, long long r,
+                                              int l, float4 a) {
+  float4* yp = reinterpret_cast<float4*>(Y + (size_t)r * 64) + l;
+  *yp = a;
+  if (acc != nullptr) {
+    float4* ap = reinterpret_cast<float4*>(acc + (size_t)r * 64) + l;
+    float4 o = *ap;
+    fma4(o, acc_scale, a);
+    *ap = o;
+  }
+}
+
+// d = 64: spmm_csr_kernel<16, 1> with the width fixed at compile time and 4 CTAs per SM -- the same lane groups and
+// floating-point order, 8 gathered rows in flight per lane, issued and consumed in lock step.
+__global__ void __launch_bounds__(256, 4)
+spmm_csr_d64_kernel(int n_rows, const long long* __restrict__ rowptr, const int* __restrict__ cols,
+                    const float* __restrict__ vals, const float* __restrict__ X, float* __restrict__ Y,
+                    float* __restrict__ acc, float acc_scale) {
+  constexpr int LPR = 16, G = 8;   // a half warp per row, one float4 per lane
+  const int lane = threadIdx.x & 31;
+  const int sub = lane / LPR, l = lane % LPR;
+  const unsigned gmask = ((1u << LPR) - 1u) << (sub * LPR);
+  const long long group = (((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 2 + sub;
+  const long long ngroups = (((long long)gridDim.x * blockDim.x) >> 5) * 2;
+  for (long long r = group; r < n_rows; r += ngroups) {
+    const long long start = __ldg(rowptr + r), end = __ldg(rowptr + r + 1);
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    int c = 0;
+    float w = 0.f;
+    if (start + l < end) {
+      c = __ldg(cols + start + l);
+      w = __ldg(vals + start + l);
+    }
+    for (long long base = start; base < end; base += LPR) {
+      const int m = (end - base) < LPR ? (int)(end - base) : LPR;
+      int cn = 0;
+      float wn = 0.f;
+      if (base + LPR + l < end) {
+        cn = __ldg(cols + base + LPR + l);
+        wn = __ldg(vals + base + LPR + l);
+      }
+      for (int t = 0; t < m; t += G) {
+        int cc[G];
+        float ww[G];
+        float4 x[G];
+#pragma unroll
+        for (int q = 0; q < G; ++q) {
+          cc[q] = __shfl_sync(gmask, c, sub * LPR + ((t + q) & (LPR - 1)));
+          ww[q] = __shfl_sync(gmask, w, sub * LPR + ((t + q) & (LPR - 1)));
+          if (t + q >= m) ww[q] = 0.f;
+        }
+#pragma unroll
+        for (int q = 0; q < G; ++q)
+          x[q] = (t + q) < m ? __ldg(reinterpret_cast<const float4*>(X + (size_t)cc[q] * 64) + l)
+                             : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int q = 0; q < G; ++q) fma4(a, ww[q], x[q]);
+      }
+      c = cn;
+      w = wn;
+    }
+    store_row_d64(Y, acc, acc_scale, r, l, a);
   }
 }
 
@@ -546,18 +612,15 @@ int qrec_spmm_csr_rowsplit_f32(int32_t n_rows, int64_t nnz, const int64_t* rowpt
   QREC_REQUIRE(rowptr && X && Y, "qrec_spmm_csr_rowsplit_f32: null pointer");
   QREC_REQUIRE(aligned16(X) && aligned16(Y) && aligned16(acc), "qrec_spmm_csr_rowsplit_f32: tables must be 16-byte aligned");
   QREC_REQUIRE(X != Y, "qrec_spmm_csr_rowsplit_f32: X and Y must not alias");
-  // d = 64: the width-specialised instantiation at 4 CTAs/SM (spmm_variants.cu, variant 0) -- bit-identical results
-  if (d == 64 && X != nullptr && Y != nullptr) {
-    static int var = -1;                                  // QREC_SPMM_VARIANT: experiment switch (spmm_variants.cu)
-    if (var < 0) {
-      const char* e = getenv("QREC_SPMM_VARIANT");
-      var = e ? atoi(e) : 0;
-      if (var < 0 || var > 6) var = 0;
-    }
-    return qrec_spmm_csr_rowsplit_var_f32(var, n_rows, rowptr, cols, vals, X, Y, d, acc, acc_scale, stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d == 64) {
+    const int grid = capped_grid(((long long)n_rows + 15) / 16, 8);   // 16 lane groups (rows) per 256-thread block
+    spmm_csr_d64_kernel<<<grid, 256, 0, st>>>(n_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, acc,
+                                              acc_scale);
+    QREC_LAUNCH_CHECK();
+    return QREC_OK;
   }
   const int nvec = d / 4;
-  cudaStream_t st = (cudaStream_t)stream;
 #define QREC_SPMM(LPR, VPL)                                                                      \
   {                                                                                              \
     const long long groups_per_block = 8 * (32 / LPR);                                           \

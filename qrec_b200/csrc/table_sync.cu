@@ -90,17 +90,6 @@ table_gather_merge_kernel(PeerPtrs peers_S, int world, long long slice4, float* 
   }
 }
 
-// out[k] = the summed slice of its owner (plain all-gather of the reduce-scatter result)
-__global__ void __launch_bounds__(128, 16)
-table_all_gather_kernel(PeerPtrs peers_S, int world, long long slice4, float4* __restrict__ out, long long n4) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n4; k += stride) {
-    int owner = (int)(k / slice4);
-    if (owner >= world) owner = world - 1;
-    out[k] = ld_peer_v4(peers_S.p[owner] + 4 * k);
-  }
-}
-
 int grid_for(long long n4) { return qrec::capped_grid((n4 + 127) / 128, 4); }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -167,22 +156,6 @@ int qrec_table_gather_merge_p2p_f32(const float* const* peer_S, int32_t world, f
   const long long n4 = n / 4, slice4 = (n4 + world - 1) / world;
   table_gather_merge_kernel<<<grid_for(n4), 128, 0, (cudaStream_t)stream>>>(pp, world, slice4, Q, reinterpret_cast<float4*>(B),
                                                                             reinterpret_cast<const float4*>(D), n4);
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
-}
-
-int qrec_table_all_gather_p2p_f32(const float* const* peer_S, int32_t world, float* out, int64_t n, void* stream) {
-  QREC_REQUIRE(peer_S && out, "qrec_table_all_gather_p2p_f32: null pointer");
-  QREC_REQUIRE(world >= 1 && world <= kMaxPeers, "qrec_table_all_gather_p2p_f32: bad world");
-  QREC_REQUIRE(n >= 0 && (n % 4) == 0 && aligned16(out), "qrec_table_all_gather_p2p_f32: n must be a multiple of 4, out 16-byte aligned");
-  if (n == 0) return QREC_OK;
-  PeerPtrs pp;
-  for (int r = 0; r < world; ++r) {
-    QREC_REQUIRE(peer_S[r] && aligned16(peer_S[r]), "qrec_table_all_gather_p2p_f32: peer pointer %d null or unaligned", r);
-    pp.p[r] = peer_S[r];
-  }
-  const long long n4 = n / 4, slice4 = (n4 + world - 1) / world;
-  table_all_gather_kernel<<<grid_for(n4), 128, 0, (cudaStream_t)stream>>>(pp, world, slice4, reinterpret_cast<float4*>(out), n4);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }

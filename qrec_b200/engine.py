@@ -6,7 +6,6 @@ sm_90a kernels.  There is no CPU path here: device entry points raise if a tenso
 CUDA device.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
@@ -437,13 +436,6 @@ def table_reduce_scatter_p2p(peer_D_ptrs, rank, S, n):
           'qrec_table_reduce_scatter_p2p_f32')
 
 
-def table_all_gather_p2p(peer_S_ptrs, out):
-    """out[k] = the summed slice held by its owner (second half of the peer-memory all-reduce)."""
-    torch = _torch()
-    check(lib.qrec_table_all_gather_p2p_f32(_ptr_array(peer_S_ptrs), len(peer_S_ptrs), _dev(out, torch.float32, 'out'),
-                                            out.numel(), _stream()), 'qrec_table_all_gather_p2p_f32')
-
-
 def table_gather_merge_p2p(peer_S_ptrs, Q, B, D):
     """All-gather of the summed slices from their owners fused with the merge (Q += S - D; B += S)."""
     torch = _torch()
@@ -452,18 +444,14 @@ def table_gather_merge_p2p(peer_S_ptrs, Q, B, D):
           'qrec_table_gather_merge_p2p_f32')
 
 
-SCORE_TOPN_TENSOR_CORES = True       # default of score_topn(tensor_cores=None) for d <= 64; QREC_TOPN_TC=0/1 overrides
-
-
 def score_topn(U, V, user_ids, rated_rowptr, rated_cols, N, rated_value=0.0, out_ids=None, out_scores=None, tensor_cores=None):
     """K8: the N best items of every listed user in one kernel (scores, rated -> rated_value, top-N; nothing
     materialised).  Returns (ids int32 [n, N], scores fp32 [n, N]), best first, ties by ascending item id.
     tensor_cores: True = the wgmma 3xTF32 kernel (csrc/topn_tc.cu; d <= 64, multiple of 4), False = the fp32 SIMT kernel
-    (csrc/topn_kernels.cu), None = the module default where the width allows it."""
+    (csrc/topn_kernels.cu), None = the tensor-core kernel where the width allows it, else the SIMT kernel."""
     torch = _torch()
     if tensor_cores is None:
-        env = os.environ.get('QREC_TOPN_TC')
-        tensor_cores = (SCORE_TOPN_TENSOR_CORES if env is None else env == '1') and U.shape[1] <= 64 and U.shape[1] % 4 == 0
+        tensor_cores = U.shape[1] <= 64 and U.shape[1] % 4 == 0
     fn, name = (lib.qrec_score_topn_tc_f32, 'qrec_score_topn_tc_f32') if tensor_cores else (lib.qrec_score_topn_f32, 'qrec_score_topn_f32')
     n = int(user_ids.shape[0])
     if U.shape[1] != V.shape[1]:
@@ -651,18 +639,6 @@ def spmm_csr(rowptr, cols, vals, X, Y, acc=None, acc_scale=0.0, rowsplit=False):
                                 _dev(Y, torch.float32, 'Y'), d,
                                 _dev(acc, torch.float32, 'acc') if acc is not None else None,
                                 float(acc_scale), _stream()), 'qrec_spmm_csr_f32')
-    return Y
-
-
-def spmm_csr_rowsplit_variant(variant, rowptr, cols, vals, X, Y, acc=None, acc_scale=0.0):
-    """Experimental row-split SpMM configurations (d = 64; csrc/spmm_variants.cu); same bits as
-    spmm_csr(..., rowsplit=True)."""
-    torch = _torch()
-    check(lib.qrec_spmm_csr_rowsplit_var_f32(int(variant), rowptr.shape[0] - 1, _dev(rowptr, torch.int64, 'rowptr'),
-                                             _dev(cols, torch.int32, 'cols'), _dev(vals, torch.float32, 'vals'),
-                                             _dev(X, torch.float32, 'X'), _dev(Y, torch.float32, 'Y'), X.shape[1],
-                                             _dev(acc, torch.float32, 'acc') if acc is not None else None,
-                                             float(acc_scale), _stream()), 'qrec_spmm_csr_rowsplit_var_f32')
     return Y
 
 

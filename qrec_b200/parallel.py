@@ -448,62 +448,6 @@ class ShardedItemTableBPR(object):
 
 
 # =============================================================================================
-# all-reduce of a replicated block over peer memory (the [I, d] item block of the graph models' layers)
-# =============================================================================================
-class PeerAllReduce(object):
-    """In-place sum over ranks of equally shaped fp32 buffers that live in symmetric (peer-mapped) memory:
-    reduce-scatter by P2P loads over NVLink (each rank sums its slice of every rank's buffer), a barrier, then an
-    all-gather of the summed slices back into the buffer (csrc/table_sync.cu) -- 2 x (W-1)/W of the buffer per
-    rank on the wire, the same volume as a ring all-reduce, in two small-footprint kernels that co-reside with a
-    running SpMM.  The exchange runs on its own high-priority stream; `start(k)` returns a handle whose wait()
-    makes the current stream wait for it.  Buffers are allocated here (`self.bufs`), the producer kernels write
-    straight into them (no staging copy)."""
-
-    def __init__(self, shape, n_bufs, device, group=None):
-        import torch.distributed._symmetric_memory as symm
-        from . import engine as E
-        self.E = E
-        g = group if group is not None else dist.group.WORLD
-        self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
-        n = 1
-        for x in shape:
-            n *= int(x)
-        if n % 4:
-            raise ValueError('PeerAllReduce: buffer size must be a multiple of 4 floats')
-        self.n = n
-        self.flat = [symm.empty(n, dtype=torch.float32, device=device) for _ in range(n_bufs)]
-        self.sums = symm.empty(n, dtype=torch.float32, device=device)
-        self.h = [symm.rendezvous(t, g) for t in self.flat]
-        self.hs = symm.rendezvous(self.sums, g)
-        self.ptrs = [[int(p) for p in h.buffer_ptrs] for h in self.h]
-        self.ptr_s = [int(p) for p in self.hs.buffer_ptrs]
-        self.bufs = [t.view(*shape) for t in self.flat]
-        self.side = torch.cuda.Stream(device=device, priority=-1)
-        self.ev_in, self.ev_out = torch.cuda.Event(), torch.cuda.Event()
-
-    class _Handle(object):
-        def __init__(self, ev):
-            self.ev = ev
-
-        def wait(self):
-            torch.cuda.current_stream().wait_event(self.ev)
-
-    def start(self, k):
-        """bufs[k] <- sum over ranks of bufs[k]; asynchronous with respect to the current stream."""
-        cur = torch.cuda.current_stream()
-        self.ev_in.record(cur)
-        with torch.cuda.stream(self.side):
-            self.side.wait_event(self.ev_in)
-            self.h[k].barrier(channel=0)                        # every rank's partial sums are complete
-            self.E.table_reduce_scatter_p2p(self.ptrs[k], self.rank, self.sums, self.n)
-            self.hs.barrier(channel=0)                          # every slice is summed (and nobody reads bufs[k] any more)
-            self.E.table_all_gather_p2p(self.ptr_s, self.flat[k])
-            ev = torch.cuda.Event()
-            ev.record(self.side)
-        return PeerAllReduce._Handle(ev)
-
-
-# =============================================================================================
 # LightGCN, user-partitioned / item-replicated (the decomposition that scales: SURVEY.md 8e, config 3)
 # =============================================================================================
 def shard_bipartite_by_user(rowptr, cols, vals, num_users, num_items, rank, world):
@@ -601,20 +545,6 @@ class UserShardedLightGCN(object):
         nu, ni = E_u_local.shape[0], E_i.shape[0]
         z = lambda n: torch.zeros(n, d, device=dev)           # noqa: E731
         self.bu, self.bi = [z(nu), z(nu)], [z(ni), z(ni)]
-        # the item-side partial sums of a layer are written straight into peer-mapped buffers and summed over
-        # NVLink by our own kernels (PeerAllReduce) when QREC_PEER_ALLREDUCE=1; NCCL's all-reduce of the 25.6 MB
-        # block is the default;
-        # gloo / world 1: plain tensors
-        self.peer = None
-        import os as _os
-        if (dev.type == 'cuda' and dist.is_initialized() and dist.get_world_size(group) > 1 and spmm is None
-                and _os.environ.get('QREC_PEER_ALLREDUCE', '0') == '1'):
-            try:
-                self.peer = PeerAllReduce((ni, d), 2, dev, group)
-                self.bi = self.peer.bufs
-            except Exception as exc:                                   # noqa: BLE001
-                self.peer_error = '%s: %s' % (type(exc).__name__, exc)
-                self.peer = None
         self.mean_u, self.mean_i = z(nu), z(ni)
         self.tot_u, self.tot_i = z(nu), z(ni)
         self.gu, self.gi = z(nu), z(ni)
@@ -653,10 +583,6 @@ class UserShardedLightGCN(object):
         """Starts the all-reduce and returns its handle (None at world size 1): the caller launches the
         user-side SpMM of the same layer before waiting, so the NVLink transfer hides behind it."""
         if dist.is_initialized() and dist.get_world_size(self.group) > 1:
-            if self.peer is not None:
-                for k, b in enumerate(self.peer.bufs):
-                    if t is b:
-                        return self.peer.start(k)
             return dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group, async_op=True)
         return None
 
@@ -767,7 +693,7 @@ class UserShardedLightGCN(object):
         call for a batch size runs eagerly (NCCL communicators, lazily sized buffers), the second captures and replays,
         later ones replay.  Falls back to the eager step -- for good, the reason kept in `graph_error` -- if the capture
         fails, and when the tensors are not on a GPU or stand-in kernels are injected (the gloo / CPU tests)."""
-        if self.graph_error is not None or u.device.type != 'cuda' or self._scatter is None or self.peer is not None:
+        if self.graph_error is not None or u.device.type != 'cuda' or self._scatter is None:
             return self.train_step(u, i, j)
         from . import engine as E
         key = int(u.shape[0])

@@ -46,23 +46,28 @@ def test_spmm_reference_adjacency(torch, E, golden_graph, d, rowsplit):
 
 @pytest.mark.parametrize('rowsplit', [False, True])
 def test_spmm_ragged_rows(torch, E, rowsplit):
-    """Empty rows, a single huge row, and rows longer than one lane-group chunk."""
+    """Empty rows, a single huge row, rows longer than one lane-group chunk, and a row ending at every gather-batch and
+    index-chunk boundary of the d = 64 row-split kernel (8 gathers per batch, 16 entries per chunk)."""
     import scipy.sparse as sp
     rng = np.random.default_rng(3)
-    n, d = 300, 64
+    n, m, d = 300, 600, 64
     rows, cols = [], []
     for r in range(n):
         deg = 0 if r % 7 == 0 else (n if r == 5 else int(rng.integers(1, 40)))
         c = rng.choice(n, size=deg, replace=False)
         rows += [r] * deg; cols += c.tolist()
-    A = sp.csr_matrix((rng.standard_normal(len(rows)).astype(np.float32), (rows, cols)), shape=(n, n))
+    boundary = (1, 3, 4, 5, 8, 9, 15, 16, 17, 31, 32, 33, 0, 600)
+    for k, deg in enumerate(boundary):
+        rows += [n + k] * deg; cols += rng.choice(m, size=deg, replace=False).tolist()
+    nr = n + len(boundary)
+    A = sp.csr_matrix((rng.standard_normal(len(rows)).astype(np.float32), (rows, cols)), shape=(nr, m))
     A.sort_indices()
-    X = rng.standard_normal((n, d)).astype(np.float32)
-    Y = torch.full((n, d), 7.0, device='cuda')
+    X = rng.standard_normal((m, d)).astype(np.float32)
+    Y = torch.full((nr, d), 7.0, device='cuda')
     E.spmm_csr(_dev(torch, A.indptr.astype(np.int64)), _dev(torch, A.indices), _dev(torch, A.data), _dev(torch, X), Y,
                rowsplit=rowsplit)
     np.testing.assert_allclose(Y.cpu().numpy(), A.astype(np.float64) @ X, rtol=1e-4, atol=1e-5)
-    assert bool((Y[0] == 0).all())       # empty row is written as zeros, not left stale
+    assert bool((Y[0] == 0).all()) and bool((Y[n + 12] == 0).all())    # empty rows are written as zeros, not left stale
 
 
 def test_spmm_power_law_rows_split_across_chunks(torch, E):

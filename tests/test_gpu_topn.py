@@ -21,12 +21,6 @@ def E():
     return engine
 
 
-def _maybe_skip_tc(tc):
-    import os
-    if tc and os.environ.get('QREC_SKIP_TC') == '1':      # set by a run script after the tensor-core tests failed on their own
-        pytest.skip('tensor-core K8 tests disabled for this run (QREC_SKIP_TC=1)')
-
-
 def _reference(P, Q, users, rp, co, N, rated_value=0.0):
     ids, vals = [], []
     for u in users:
@@ -51,7 +45,6 @@ def _csr(rng, nu, ni, max_deg):
                                                  (300, 20000, 64, 20, False, True), (129, 257, 32, 100, True, True), (90, 700, 52, 30, True, True), (40, 300, 8, 20, False, True),
                                                  (1000, 5000, 64, 100, True, True)])
 def test_topn_equals_reference_flow(torch, E, nu, ni, d, N, signed, tc):
-    _maybe_skip_tc(tc)
     rng = np.random.default_rng(nu * 7 + ni)
     P = (rng.standard_normal((nu, d)) if signed else rng.random((nu, d))).astype(np.float32)
     Q = (rng.standard_normal((ni, d)) if signed else rng.random((ni, d))).astype(np.float32)
@@ -78,7 +71,6 @@ def test_topn_equals_reference_flow(torch, E, nu, ni, d, N, signed, tc):
 
 @pytest.mark.parametrize('tc', [False, True])
 def test_topn_ties_and_rated_zeros_outrank_negative_scores(torch, E, tc):
-    _maybe_skip_tc(tc)
     """All unrated scores negative, so the rated items (score 0) must fill the top of the list (the reference
     writes 0, it does not remove them -- SURVEY A7); exact ties are ordered by ascending item id."""
     nu, ni, d, N = 3, 400, (32 if tc else 4), 12
@@ -111,7 +103,6 @@ def test_topn_bad_arguments(torch, E):
 
 
 def test_topn_tensor_core_kernel_agrees_with_simt_kernel(torch, E):
-    _maybe_skip_tc(True)
     """Both kernels on one larger block (2048 users x 30000 items, d = 64, N = 100): identical index lists wherever the
     SIMT scores are separated by more than fp32 summation noise, scores within 2e-5."""
     g = torch.Generator(device='cuda'); g.manual_seed(5)

@@ -249,8 +249,6 @@ def test_device_csr_split_row_issues_one_launch_per_half_with_the_same_result(mo
     nnz_u = int(whole.rowptr[nu])
     assert calls == [(nu, 0, nnz_u, True), (ni, nnz_u, A.nnz, True)]
     assert torch.allclose(Y0, ref, atol=1e-6) and torch.equal(Y1, Y0) and torch.equal(acc1, acc0)
-    # out-of-range split rows and the experiment switch leave the single launch
+    # out-of-range split rows leave the single launch
     assert DeviceCSR.from_tensors(A.shape, whole.rowptr, whole.cols, whole.vals, split_row=0).split_row is None
     assert DeviceCSR.from_tensors(A.shape, whole.rowptr, whole.cols, whole.vals, split_row=nu + ni).split_row is None
-    monkeypatch.setenv('QREC_SPMM_SPLIT', '0')
-    assert DeviceCSR.from_tensors(A.shape, whole.rowptr, whole.cols, whole.vals, split_row=nu).split_row is None

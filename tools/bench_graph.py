@@ -62,12 +62,6 @@ def main():
                           'rows': N, 'nnz': nnz, 'd': D, 'ms': ms, 'algorithmic_GB': algo / 1e9,
                           'achieved_GBs': algo / ms / 1e6, 'frac_of_measured_hbm': algo / ms / 1e6 / peak,
                           'compulsory_GB': floor / 1e9, 'zipf': args.zipf}))
-    if D == 64:   # experiment configurations, csrc/spmm_variants.cu
-        for variant in range(7):
-            ms = timed(lambda: E.spmm_csr_rowsplit_variant(variant, rowptr, cols, vals, X, Y, acc=acc, acc_scale=0.25),
-                       args.steps, args.warmup)
-            print(json.dumps({'kernel': 'spmm_csr_rowsplit_var_f32', 'variant': variant, 'ms': ms,
-                              'achieved_GBs': algo / ms / 1e6, 'zipf': args.zipf}))
     if args.spmm_only:
         return
     # full LightGCN steps through the drop-in class's step function

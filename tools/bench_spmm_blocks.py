@@ -2,8 +2,8 @@
 """K2 decomposed on the bipartite blocks of the benchmark graph (1M users x 100K items x 50M edges, d=64): the user-side
 product A_ui E_i (gathers from the 25.6 MB item block), the item-side product A_iu E_u (gathers from the 256 MB user
 block) and the item side cut into column blocks of users so that one block of E_u fits the L2
-(parallel.split_csr_columns / blocked_spmm), each with the plain kernel (variant 0) and with the L2 residency hints
-(variant 6: (col, val) stream evict_first, gathered rows evict_last).  One JSON line per measurement.
+(parallel.split_csr_columns / blocked_spmm), each with the row-split product spmm_csr(..., rowsplit=True).  One JSON
+line per measurement.
 
   python tools/bench_spmm_blocks.py [--blocks 2 3 4 6 8] [--steps 10]
 """
@@ -19,7 +19,6 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--blocks', type=int, nargs='+', default=[2, 3, 4, 6, 8])
-    ap.add_argument('--variants', type=int, nargs='+', default=[0, 6])
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
     args = ap.parse_args()
@@ -49,23 +48,23 @@ def main():
         torch.cuda.synchronize()
         return a.elapsed_time(b) / args.steps
 
+    def spmm(A, X, Y, acc=None, s=0.0):
+        return E.spmm_csr(A[0], A[1], A[2], X, Y, acc=acc, acc_scale=s, rowsplit=True)
+
     nnz = int(A_ui[1].numel())
-    for var in args.variants:
-        ms_u = timed(lambda: E.spmm_csr_rowsplit_variant(var, A_ui[0], A_ui[1], A_ui[2], Ei, Yu))
-        print(json.dumps({'product': 'user side A_ui E_i', 'variant': var, 'rows': U, 'nnz': nnz, 'ms': ms_u,
-                          'G_gathers_per_s': nnz / ms_u / 1e6}), flush=True)
-        ms_i = timed(lambda: E.spmm_csr_rowsplit_variant(var, A_iu[0], A_iu[1], A_iu[2], Eu, Yi))
-        print(json.dumps({'product': 'item side A_iu E_u', 'variant': var, 'blocks': 1, 'rows': I, 'nnz': nnz, 'ms': ms_i,
-                          'G_gathers_per_s': nnz / ms_i / 1e6}), flush=True)
+    ms_u = timed(lambda: spmm(A_ui, Ei, Yu))
+    print(json.dumps({'product': 'user side A_ui E_i', 'rows': U, 'nnz': nnz, 'ms': ms_u,
+                      'G_gathers_per_s': nnz / ms_u / 1e6}), flush=True)
+    ms_i = timed(lambda: spmm(A_iu, Eu, Yi))
+    print(json.dumps({'product': 'item side A_iu E_u', 'blocks': 1, 'rows': I, 'nnz': nnz, 'ms': ms_i,
+                      'G_gathers_per_s': nnz / ms_i / 1e6}), flush=True)
     ref = Yi.clone()
     for nb in args.blocks:
         blocks = parallel.split_csr_columns(A_iu, U, nb)
-        for var in args.variants:
-            spmm = lambda A, X, Y, acc, s: E.spmm_csr_rowsplit_variant(var, A[0], A[1], A[2], X, Y, acc=acc, acc_scale=s)   # noqa: E731
-            ms = timed(lambda: parallel.blocked_spmm(spmm, blocks, Eu, Yi, Si, None, 0.0))
-            err = float((Yi - ref).abs().max() / ref.abs().max())
-            print(json.dumps({'product': 'item side A_iu E_u', 'variant': var, 'blocks': nb, 'block_MB': U / nb * D * 4 / 1e6,
-                              'ms': ms, 'G_gathers_per_s': nnz / ms / 1e6, 'rel_err_vs_unblocked': err}), flush=True)
+        ms = timed(lambda: parallel.blocked_spmm(spmm, blocks, Eu, Yi, Si, None, 0.0))
+        err = float((Yi - ref).abs().max() / ref.abs().max())
+        print(json.dumps({'product': 'item side A_iu E_u', 'blocks': nb, 'block_MB': U / nb * D * 4 / 1e6,
+                          'ms': ms, 'G_gathers_per_s': nnz / ms / 1e6, 'rel_err_vs_unblocked': err}), flush=True)
         del blocks
         torch.cuda.empty_cache()
 

@@ -121,7 +121,6 @@ def main():
         E.table_delta(Q.view(-1), Bt.view(-1), Dt, St)
         E.table_reduce_scatter_p2p([Dt.data_ptr(), Dt.data_ptr()], 1, St, Dt.numel())
         E.table_gather_merge_p2p([St.data_ptr(), St.data_ptr()], Q.view(-1), Bt.view(-1), Dt)
-        E.table_all_gather_p2p([St.data_ptr(), St.data_ptr()], Dt)
         E.table_merge(Q.view(-1), Bt.view(-1), Dt, St)
         E.ubench_row_ops(torch.rand(1000, 64, device='cuda'), 5000, 2)
         cnt, snd = torch.empty(2, dtype=torch.int32, device='cuda'), torch.empty(2 * 900, dtype=torch.int32, device='cuda')
