@@ -21,6 +21,7 @@
 
 #include "common.h"
 #include "device.cuh"
+#include "lane_shape.h"
 #include "philox.cuh"
 #include "bpr_step.cuh"
 #include "um_waves.cuh"
@@ -643,7 +644,6 @@ int launch_ordered(T* P, T* Q, int d, long long n, const int* u, const int* i, c
   QREC_REQUIRE(n >= 0, "bpr_sgd_ordered: n < 0");
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && j && wu && wi && wj, "bpr_sgd_ordered: null index pointer");
-  const int e = (d + 31) / 32;
   // 2 CTAs of 8 warps per SM: enough warps to cover the dependency DAG's width at the
   // synthetic scale (~25 independent triples per level in user-major order) without
   // drowning the LSU in pollers.
@@ -651,14 +651,10 @@ int launch_ordered(T* P, T* Q, int d, long long n, const int* u, const int* i, c
   // for about that many pollers -- thousands of idle warps hammering the version counters slow the
   // few that can make progress (1.4 independent triples per level on FilmTrust, ~25 at SYN scale)
   const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
-#define QREC_ORD(E)                                                                              \
-  bpr_sgd_ordered_kernel<T, E><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, j, wu, wi, wj, ver_p,     \
-                                                     ver_q, ticket, lr, reg_u, reg_i, loss)
-  if (e <= 1) QREC_ORD(1);
-  else if (e <= 2) QREC_ORD(2);
-  else if (e <= 4) QREC_ORD(4);
-  else QREC_ORD(8);
-#undef QREC_ORD
+  with_lane_elems(d, [&](auto e) {
+    bpr_sgd_ordered_kernel<T, decltype(e)::E><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, j, wu, wi, wj, ver_p, ver_q,
+                                                                    ticket, lr, reg_u, reg_i, loss);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -678,15 +674,11 @@ int launch_bpr_batch(float* P, float* Q, int d, long long n, const int* u, const
   const int nvec = d / 4;
   const long long warps_needed = (n + 31) / 32;
   const int grid = capped_grid((warps_needed + 7) / 8, 8);  // 8 CTAs x 8 warps per SM, grid-stride beyond
-#define QREC_BATCH(LPR, VPL, UN)                                                                \
-  bpr_sgd_batch_kernel<LPR, VPL, UN><<<grid, 256, 0, st>>>(P, Q, nvec, n, u, i, j, lr, reg_u,   \
-                                                           reg_i, loss)
-  if (nvec <= 4) QREC_BATCH(4, 1, 2);
-  else if (nvec <= 8) QREC_BATCH(8, 1, 4);
-  else if (nvec <= 16) QREC_BATCH(16, 1, 4);
-  else if (nvec <= 32) QREC_BATCH(32, 1, 4);
-  else QREC_BATCH(32, 2, 2);
-#undef QREC_BATCH
+  with_row_shape<256>(nvec, [&](auto s) {
+    using S = decltype(s);
+    bpr_sgd_batch_kernel<S::LPR, S::VPL, S::UNROLL><<<grid, 256, 0, st>>>(P, Q, nvec, n, u, i, j, lr, reg_u, reg_i,
+                                                                          loss);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -751,13 +743,11 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
   FusedSampler fs = {reinterpret_cast<const long long*>(rated_rowptr), rated_cols, num_items, (uint32_t)seed,
                      (uint32_t)(seed >> 32), epoch, j_out};
   const int nvec = d / 4;
-  const int lpr = nvec <= 4 ? 4 : nvec <= 8 ? 8 : nvec <= 16 ? 16 : 32;
+  const int lpr = row_lpr(nvec);
   const bool sig = sample && rated_sig != nullptr;
-  const UserMajorKernel kernel = tma        ? bpr_sgd_usermajor_tma_kernel
-                                 : lpr == 4  ? usermajor_kernel<4>(nvec, sample, sig)
-                                 : lpr == 8  ? usermajor_kernel<8>(nvec, sample, sig)
-                                 : lpr == 16 ? usermajor_kernel<16>(nvec, sample, sig)
-                                             : usermajor_kernel<32>(nvec, sample, sig);
+  const UserMajorKernel kernel =
+      tma ? bpr_sgd_usermajor_tma_kernel
+          : with_row_shape<128>(nvec, [&](auto s) { return usermajor_kernel<decltype(s)::LPR>(nvec, sample, sig); });
   const int smem = tma ? UM_STAGE_SMEM : 0;
   if (tma) QREC_CUDA(allow_dynamic_smem((const void*)kernel, smem));
   // Grid = exactly the CTAs that are resident at once (occupancy API per instantiation); the stream is swept in
@@ -900,18 +890,12 @@ int qrec_bpr_sgd_staged_f32(float* P, int32_t d, int64_t n, const int32_t* u, co
   QREC_REQUIRE(P && u && pos_i && pos_j && R && D && loss, "qrec_bpr_sgd_staged_f32: null pointer");
   const int nvec = d / 4;
   cudaStream_t st = (cudaStream_t)stream;
-#define QREC_STAGED(LPR)                                                                        \
-  {                                                                                             \
-    const long long per_block = 8 * (32 / LPR);                                                 \
-    const int grid = capped_grid((n + per_block - 1) / per_block, 8);                           \
-    bpr_sgd_staged_kernel<LPR><<<grid, 256, 0, st>>>(P, nvec, n, u, pos_i, pos_j, R, D,         \
-                                                     lr, reg_u, reg_i, loss);                   \
-  }
-  if (nvec <= 4) QREC_STAGED(4)
-  else if (nvec <= 8) QREC_STAGED(8)
-  else if (nvec <= 16) QREC_STAGED(16)
-  else QREC_STAGED(32)
-#undef QREC_STAGED
+  with_row_shape<128>(nvec, [&](auto s) {
+    constexpr int LPR = decltype(s)::LPR;
+    const long long per_block = 8 * (32 / LPR);
+    const int grid = capped_grid((n + per_block - 1) / per_block, 8);
+    bpr_sgd_staged_kernel<LPR><<<grid, 256, 0, st>>>(P, nvec, n, u, pos_i, pos_j, R, D, lr, reg_u, reg_i, loss);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }

@@ -18,6 +18,7 @@
 
 #include "common.h"
 #include "device.cuh"
+#include "lane_shape.h"
 
 namespace {
 
@@ -567,6 +568,22 @@ axpby_kernel(float* __restrict__ dst, const float* __restrict__ a, const float* 
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// K3's launch, shared by its four entry points (MODE as in bpr_grad_scatter_kernel); they check the arguments.
+template <int MODE>
+int launch_k3(const float* U, const float* V, int d, long long n, const int* u, const int* i, const int* j, float eps,
+              float reg, float* gU, float* gV, double* loss, float* y_buf, float log_weight, const float* y_scale,
+              cudaStream_t st) {
+  const int nvec = d / 4;
+  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
+  with_row_shape<256>(nvec, [&](auto s) {
+    using S = decltype(s);
+    bpr_grad_scatter_kernel<S::LPR, S::VPL, S::UNROLL, MODE><<<grid, 256, 0, st>>>(
+        U, V, nvec, n, u, i, j, eps, reg, gU, gV, loss, y_buf, log_weight, y_scale);
+  });
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -586,19 +603,13 @@ int qrec_spmm_csr_f32(int32_t n_rows, int64_t nnz, const int64_t* rowptr, const 
   QREC_REQUIRE(cols && vals, "qrec_spmm_csr_f32: null cols/vals");
   const int nvec = d / 4;
   constexpr int QN = 1024;
-#define QREC_SPMMB(LPR, VPL)                                                                     \
-  {                                                                                              \
-    const long long groups_per_block = 8 * (32 / LPR);                                           \
-    const int grid = capped_grid(((nnz + QN - 1) / QN + groups_per_block - 1) / groups_per_block, 8); \
-    spmm_csr_balanced_kernel<LPR, VPL, QN><<<grid, 256, 0, st>>>(                                \
-        n_rows, nnz, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale); \
-  }
-  if (nvec <= 4) QREC_SPMMB(4, 1)
-  else if (nvec <= 8) QREC_SPMMB(8, 1)
-  else if (nvec <= 16) QREC_SPMMB(16, 1)
-  else if (nvec <= 32) QREC_SPMMB(32, 1)
-  else QREC_SPMMB(32, 2)
-#undef QREC_SPMMB
+  with_row_shape<256>(nvec, [&](auto s) {
+    using S = decltype(s);
+    const long long groups_per_block = 8 * (32 / S::LPR);
+    const int grid = capped_grid(((nnz + QN - 1) / QN + groups_per_block - 1) / groups_per_block, 8);
+    spmm_csr_balanced_kernel<S::LPR, S::VPL, QN><<<grid, 256, 0, st>>>(
+        n_rows, nnz, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -621,19 +632,13 @@ int qrec_spmm_csr_rowsplit_f32(int32_t n_rows, int64_t nnz, const int64_t* rowpt
     return QREC_OK;
   }
   const int nvec = d / 4;
-#define QREC_SPMM(LPR, VPL)                                                                      \
-  {                                                                                              \
-    const long long groups_per_block = 8 * (32 / LPR);                                           \
-    const int grid = capped_grid((n_rows + groups_per_block - 1) / groups_per_block, 8);         \
-    spmm_csr_kernel<LPR, VPL><<<grid, 256, 0, st>>>(                                             \
-        n_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale); \
-  }
-  if (nvec <= 4) QREC_SPMM(4, 1)
-  else if (nvec <= 8) QREC_SPMM(8, 1)
-  else if (nvec <= 16) QREC_SPMM(16, 1)
-  else if (nvec <= 32) QREC_SPMM(32, 1)
-  else QREC_SPMM(32, 2)
-#undef QREC_SPMM
+  with_row_shape<256>(nvec, [&](auto s) {
+    using S = decltype(s);
+    const long long groups_per_block = 8 * (32 / S::LPR);
+    const int grid = capped_grid((n_rows + groups_per_block - 1) / groups_per_block, 8);
+    spmm_csr_kernel<S::LPR, S::VPL><<<grid, 256, 0, st>>>(
+        n_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -652,18 +657,13 @@ int qrec_spmm_csr_scatter_rows_f32(int32_t n_rows, int32_t n_src, const int32_t*
   if (n_src == 0) return QREC_OK;
   QREC_REQUIRE(src_rows && cols && vals, "qrec_spmm_csr_scatter_rows_f32: null index pointer");
   const int nvec = d / 4;
-#define QREC_SCAT(LPR)                                                                           \
-  {                                                                                              \
-    const long long per_block = 8 * (32 / LPR);                                                  \
-    const int grid = capped_grid(((long long)n_src * 64 + per_block - 1) / per_block, 8);        \
-    spmm_scatter_rows_kernel<LPR><<<grid, 256, 0, st>>>(                                         \
-        n_src, src_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale); \
-  }
-  if (nvec <= 4) QREC_SCAT(4)
-  else if (nvec <= 8) QREC_SCAT(8)
-  else if (nvec <= 16) QREC_SCAT(16)
-  else QREC_SCAT(32)
-#undef QREC_SCAT
+  with_row_shape<128>(nvec, [&](auto s) {
+    constexpr int LPR = decltype(s)::LPR;
+    const long long per_block = 8 * (32 / LPR);
+    const int grid = capped_grid(((long long)n_src * 64 + per_block - 1) / per_block, 8);
+    spmm_scatter_rows_kernel<LPR><<<grid, 256, 0, st>>>(
+        n_src, src_rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, nvec, acc, acc_scale);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -680,14 +680,10 @@ int qrec_spmm_csr_rows_f32(int32_t n_list, const int32_t* rows, const int64_t* r
   const int nvec = d / 4;
   const int grid = capped_grid(((long long)n_list + 7) / 8, 8);   // one warp per listed row, 8 warps per block
   cudaStream_t st = (cudaStream_t)stream;
-#define QREC_LIST(LPR)                                                                                     \
-  spmm_list_rows_kernel<LPR><<<grid, 256, 0, st>>>(n_list, rows, reinterpret_cast<const long long*>(rowptr), \
-                                                   cols, vals, X, Y, compact, nvec, acc, acc_scale)
-  if (nvec <= 4) QREC_LIST(4);
-  else if (nvec <= 8) QREC_LIST(8);
-  else if (nvec <= 16) QREC_LIST(16);
-  else QREC_LIST(32);
-#undef QREC_LIST
+  with_row_shape<128>(nvec, [&](auto s) {
+    spmm_list_rows_kernel<decltype(s)::LPR><<<grid, 256, 0, st>>>(
+        n_list, rows, reinterpret_cast<const long long*>(rowptr), cols, vals, X, Y, compact, nvec, acc, acc_scale);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -701,20 +697,7 @@ int qrec_bpr_grad_scatter_f32(const float* U, const float* V, int32_t d, int64_t
   QREC_REQUIRE(U && V && u && i && j && gU && gV && loss, "qrec_bpr_grad_scatter_f32: null pointer");
   QREC_REQUIRE(aligned16(U) && aligned16(V) && aligned16(gU) && aligned16(gV),
                "qrec_bpr_grad_scatter_f32: tables must be 16-byte aligned");
-  const int nvec = d / 4;
-  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-#define QREC_K3(LPR, VPL, UN)                                                                    \
-  bpr_grad_scatter_kernel<LPR, VPL, UN><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, eps, reg,  \
-                                                              gU, gV, loss)
-  if (nvec <= 4) QREC_K3(4, 1, 2);
-  else if (nvec <= 8) QREC_K3(8, 1, 4);
-  else if (nvec <= 16) QREC_K3(16, 1, 4);
-  else if (nvec <= 32) QREC_K3(32, 1, 4);
-  else QREC_K3(32, 2, 2);
-#undef QREC_K3
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_k3<0>(U, V, d, n, u, i, j, eps, reg, gU, gV, loss, nullptr, 1.f, nullptr, (cudaStream_t)stream);
 }
 
 int qrec_bpr_grad_scatter_scaled_f32(const float* U, const float* V, int32_t d, int64_t n,
@@ -726,20 +709,7 @@ int qrec_bpr_grad_scatter_scaled_f32(const float* U, const float* V, int32_t d, 
   QREC_REQUIRE(U && V && u && i && j && y_scale && gU && gV && loss, "qrec_bpr_grad_scatter_scaled_f32: null pointer");
   QREC_REQUIRE(aligned16(U) && aligned16(V) && aligned16(gU) && aligned16(gV),
                "qrec_bpr_grad_scatter_scaled_f32: tables must be 16-byte aligned");
-  const int nvec = d / 4;
-  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-#define QREC_K3S(LPR, VPL, UN)                                                                      \
-  bpr_grad_scatter_kernel<LPR, VPL, UN><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, eps, reg, gU, \
-                                                              gV, loss, nullptr, 1.f, y_scale)
-  if (nvec <= 4) QREC_K3S(4, 1, 2);
-  else if (nvec <= 8) QREC_K3S(8, 1, 4);
-  else if (nvec <= 16) QREC_K3S(16, 1, 4);
-  else if (nvec <= 32) QREC_K3S(32, 1, 4);
-  else QREC_K3S(32, 2, 2);
-#undef QREC_K3S
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_k3<0>(U, V, d, n, u, i, j, eps, reg, gU, gV, loss, nullptr, 1.f, y_scale, (cudaStream_t)stream);
 }
 
 int qrec_bpr_partial_scores_f32(const float* U, const float* V, int32_t d, int64_t n, const int32_t* u, const int32_t* i,
@@ -749,19 +719,7 @@ int qrec_bpr_partial_scores_f32(const float* U, const float* V, int32_t d, int64
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(U && V && u && i && j && y_part && loss, "qrec_bpr_partial_scores_f32: null pointer");
   QREC_REQUIRE(aligned16(U) && aligned16(V), "qrec_bpr_partial_scores_f32: tables must be 16-byte aligned");
-  const int nvec = d / 4;
-  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-#define QREC_K3P(LPR, VPL, UN)                                                                   \
-  bpr_grad_scatter_kernel<LPR, VPL, UN, 1><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, 0.f, reg, nullptr, nullptr, loss, y_part, 0.f)
-  if (nvec <= 4) QREC_K3P(4, 1, 2);
-  else if (nvec <= 8) QREC_K3P(8, 1, 4);
-  else if (nvec <= 16) QREC_K3P(16, 1, 4);
-  else if (nvec <= 32) QREC_K3P(32, 1, 4);
-  else QREC_K3P(32, 2, 2);
-#undef QREC_K3P
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_k3<1>(U, V, d, n, u, i, j, 0.f, reg, nullptr, nullptr, loss, y_part, 0.f, nullptr, (cudaStream_t)stream);
 }
 
 int qrec_bpr_grad_from_scores_f32(const float* U, const float* V, int32_t d, int64_t n, const int32_t* u, const int32_t* i,
@@ -773,20 +731,8 @@ int qrec_bpr_grad_from_scores_f32(const float* U, const float* V, int32_t d, int
   QREC_REQUIRE(U && V && u && i && j && y_full && gU && gV && loss, "qrec_bpr_grad_from_scores_f32: null pointer");
   QREC_REQUIRE(aligned16(U) && aligned16(V) && aligned16(gU) && aligned16(gV),
                "qrec_bpr_grad_from_scores_f32: tables must be 16-byte aligned");
-  const int nvec = d / 4;
-  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* yb = const_cast<float*>(y_full);
-#define QREC_K3A(LPR, VPL, UN)                                                                   \
-  bpr_grad_scatter_kernel<LPR, VPL, UN, 2><<<grid, 256, 0, st>>>(U, V, nvec, n, u, i, j, eps, reg, gU, gV, loss, yb, log_weight)
-  if (nvec <= 4) QREC_K3A(4, 1, 2);
-  else if (nvec <= 8) QREC_K3A(8, 1, 4);
-  else if (nvec <= 16) QREC_K3A(16, 1, 4);
-  else if (nvec <= 32) QREC_K3A(32, 1, 4);
-  else QREC_K3A(32, 2, 2);
-#undef QREC_K3A
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_k3<2>(U, V, d, n, u, i, j, eps, reg, gU, gV, loss, const_cast<float*>(y_full), log_weight, nullptr,
+                      (cudaStream_t)stream);
 }
 
 int qrec_adam_dense_tf1_f32(float* var, float* m, float* v, const float* g, int64_t n, float lr,

@@ -24,6 +24,7 @@
 //     rating_performance of iterativeRecommender.py:104-113 without moving the tables).
 #include "common.h"
 #include "device.cuh"
+#include "lane_shape.h"
 #include "mf_step.cuh"
 
 namespace {
@@ -223,24 +224,15 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
   QREC_REQUIRE(n >= 0, "mf_sgd_ordered: n < 0");
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && r && wu && wi, "mf_sgd_ordered: null entry pointer");
-  const int e = (d + 31) / 32;
   const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
-#define QREC_MFO(E, K)                                                                                 \
-  mf_sgd_ordered_kernel<T, E, K><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, r, wu, wi, ver_p, ver_q,      \
-                                                       ticket, lr, reg_u, reg_i, Bu, Bi, reg_b,        \
-                                                       global_mean, loss)
-#define QREC_MFO_K(E)            \
-  do {                           \
-    if (kind == 0) QREC_MFO(E, 0); \
-    else if (kind == 1) QREC_MFO(E, 1); \
-    else QREC_MFO(E, 2);         \
-  } while (0)
-  if (e <= 1) QREC_MFO_K(1);
-  else if (e <= 2) QREC_MFO_K(2);
-  else if (e <= 4) QREC_MFO_K(4);
-  else QREC_MFO_K(8);
-#undef QREC_MFO_K
-#undef QREC_MFO
+  with_lane_elems(d, [&](auto e) {
+    constexpr int E = decltype(e)::E;
+    const auto kernel = kind == 0   ? mf_sgd_ordered_kernel<T, E, 0>
+                        : kind == 1 ? mf_sgd_ordered_kernel<T, E, 1>
+                                    : mf_sgd_ordered_kernel<T, E, 2>;
+    kernel<<<grid, 256, 0, st>>>(P, Q, d, n, u, i, r, wu, wi, ver_p, ver_q, ticket, lr, reg_u, reg_i, Bu, Bi, reg_b,
+                                 global_mean, loss);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
@@ -297,27 +289,18 @@ int qrec_mf_sgd_batch_f32(int32_t kind, float* P, float* Q, int32_t d, int64_t n
   if (max_inflight > 0) {
     // a lane group has UNROLL = 4 entries between their row reads and their reductions: bound the
     // number of such entries across the grid (the staleness window of the Hogwild update)
-    const int lpr = nvec <= 4 ? 4 : (nvec <= 8 ? 8 : (nvec <= 16 ? 16 : 32));
-    const long long per_block = 8LL * (32 / lpr) * 4;
+    const long long per_block = 8LL * (32 / row_lpr(nvec)) * 4;
     long long want = (max_inflight + per_block - 1) / per_block;
     if (want < 1) want = 1;
     if (blocks > want) blocks = want;
   }
-#define QREC_MFB(LPR, K)                                                                                  \
-  mf_sgd_batch_kernel<LPR, K, 4><<<(int)blocks, 256, 0, st>>>(P, Q, nvec, n, u, i, r, lr, reg_u, reg_i,   \
-                                                              Bu, Bi, reg_b, global_mean, loss)
-#define QREC_MFB_K(LPR)              \
-  do {                               \
-    if (kind == 0) QREC_MFB(LPR, 0); \
-    else if (kind == 1) QREC_MFB(LPR, 1); \
-    else QREC_MFB(LPR, 2);           \
-  } while (0)
-  if (nvec <= 4) QREC_MFB_K(4);
-  else if (nvec <= 8) QREC_MFB_K(8);
-  else if (nvec <= 16) QREC_MFB_K(16);
-  else QREC_MFB_K(32);
-#undef QREC_MFB_K
-#undef QREC_MFB
+  with_row_shape<128>(nvec, [&](auto s) {
+    constexpr int LPR = decltype(s)::LPR;
+    const auto kernel = kind == 0   ? mf_sgd_batch_kernel<LPR, 0, 4>
+                        : kind == 1 ? mf_sgd_batch_kernel<LPR, 1, 4>
+                                    : mf_sgd_batch_kernel<LPR, 2, 4>;
+    kernel<<<(int)blocks, 256, 0, st>>>(P, Q, nvec, n, u, i, r, lr, reg_u, reg_i, Bu, Bi, reg_b, global_mean, loss);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }

@@ -16,6 +16,7 @@
 //     reads of Q[i_t], Bi[i_t], Y[i_t] run kPrefetch steps ahead of the writes of the steps before.
 #include "common.h"
 #include "device.cuh"
+#include "lane_shape.h"
 #include "svdpp_step.cuh"
 
 namespace {
@@ -286,20 +287,15 @@ int qrec_svdpp_epoch_usermajor_f32(float* P, float* Q, float* Y, float* Bu, floa
   QREC_REQUIRE(row_order && rowptr && cols && vals, "svdpp_epoch_usermajor: null CSR pointer");
   cudaStream_t st = (cudaStream_t)stream;
   const int nvec = d / 4;
-  const int lpr = nvec <= 4 ? 4 : (nvec <= 8 ? 8 : (nvec <= 16 ? 16 : 32));
-  const long long per_block = kThreads / lpr;
+  const long long per_block = kThreads / row_lpr(nvec);
   long long groups = max_users_in_flight > 0 && max_users_in_flight < n_rows ? max_users_in_flight : n_rows;
   const int blocks = capped_grid((groups + per_block - 1) / per_block, 8);
   if (groups > (long long)blocks * per_block) groups = (long long)blocks * per_block;
-#define QREC_SVDPP_UM(LPR)                                                                                      \
-  svdpp_usermajor_kernel<LPR><<<blocks, kThreads, 0, st>>>(P, Q, Y, Bu, Bi, nvec, n_rows, row_order,             \
-                                                            (const long long*)rowptr, cols, vals, lr, reg_u,     \
-                                                            reg_i, reg_b, reg_y, global_mean, groups, loss)
-  if (lpr == 4) QREC_SVDPP_UM(4);
-  else if (lpr == 8) QREC_SVDPP_UM(8);
-  else if (lpr == 16) QREC_SVDPP_UM(16);
-  else QREC_SVDPP_UM(32);
-#undef QREC_SVDPP_UM
+  with_row_shape<128>(nvec, [&](auto s) {
+    svdpp_usermajor_kernel<decltype(s)::LPR><<<blocks, kThreads, 0, st>>>(
+        P, Q, Y, Bu, Bi, nvec, n_rows, row_order, (const long long*)rowptr, cols, vals, lr, reg_u, reg_i, reg_b, reg_y,
+        global_mean, groups, loss);
+  });
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
