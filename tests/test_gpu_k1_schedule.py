@@ -2,15 +2,16 @@
 
 The epoch's launches run in waves (qrec_b200/csrc/um_waves.cuh).  Before a wave the item table is snapshotted; every
 user of the wave runs its triples in order with P[u] updated after each one, reading item rows only from the snapshot;
-the item-row deltas of the whole wave are summed into the table.  The oracle below does exactly that in float64, with
+the item-row deltas of the whole wave are summed into the table.  k1_wave_oracle.py does exactly that in float64, with
 the negatives the GPU drew.  What is left between the two is fp32 rounding and the summation order of the
 scatter-adds, far below the difference that one triple in a different wave would make."""
 import numpy as np
 import pytest
 
+from k1_wave_oracle import CH, check_against, pipeline_launches, wave_chunks, wave_oracle  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
-CH = 32
 LR, REG = 0.01, 0.001          # bench.py's learning rate and regularisation
 USERS, ITEMS, D, MAXDEG = 50_000, 5_000, 64, 120
 SEED, EPOCH = 0x5eed, 4
@@ -29,48 +30,6 @@ def E():
     return engine
 
 
-def wave_chunks(n, num_items, d):
-    """launch_usermajor's wave length in chunks of CH triples (um_wave_chunks)."""
-    copy_bytes = 2 * num_items * d * 4
-    copy_floor = 8 * copy_bytes // (24 * d + 12) if copy_bytes > (8 << 20) else 0
-    return max(min(max(n // 64, copy_floor), 4 * num_items) // CH, 1)
-
-
-def wave_oracle(P0, Q0, rowptr, i, j, launches, lr, reg, shift=0):
-    """float64 epoch: launches = [(ua, ub)], each a separate launch over users [ua, ub) with its own waves.  shift
-    moves every wave boundary `shift` triples earlier."""
-    from scipy import sparse
-    P, Q = P0.astype(np.float64), Q0.astype(np.float64)
-    a = lr * reg
-    loss = 0.0
-    for ua, ub in launches:
-        start = rowptr[ua:ub] - rowptr[ua]
-        deg = np.diff(rowptr[ua:ub + 1])
-        wave_of = (start + shift) // (wave_chunks(int(rowptr[ub] - rowptr[ua]), Q.shape[0], Q.shape[1]) * CH)
-        users = np.arange(ua, ub)
-        for w in np.unique(wave_of[deg > 0]):
-            sel = (wave_of == w) & (deg > 0)
-            uu, first, dg = users[sel], rowptr[ua:ub][sel], deg[sel]
-            Qw = Q.copy()
-            rows, deltas = [], []
-            for k in range(int(dg.max())):
-                on = dg > k
-                u, t = uu[on], first[on] + k
-                p, qi, qj = P[u], Qw[i[t]], Qw[j[t]]
-                x = np.einsum('ij,ij->i', p, qi - qj)
-                s = 1.0 / (1.0 + np.exp(-x))
-                g = (lr * (1.0 - s))[:, None]
-                loss += float(-np.log(s).sum())
-                pn = p + g * (qi - qj)
-                rows += [i[t], j[t]]
-                deltas += [g * (1 - a) * pn - a * qi, -g * (1 - a) * pn - a * qj]
-                P[u] = (1 - a) * pn
-            r = np.concatenate(rows)
-            S = sparse.csr_matrix((np.ones(len(r)), (r, np.arange(len(r)))), shape=(Q.shape[0], len(r)))
-            Q += S @ np.concatenate(deltas)
-    return P, Q, loss
-
-
 @pytest.fixture(scope='module')
 def case(torch, E):
     rng = np.random.default_rng(2024)
@@ -86,22 +45,6 @@ def case(torch, E):
     Q0 = (rng.random((ITEMS, D)) / 3).astype(np.float32)
     Po, Qo, lo = wave_oracle(P0, Q0, rowptr, i, j, [(0, USERS)], LR, REG)
     return dict(rowptr=rowptr, u=u, i=i, j=j, rrp=rrp, rc=rc, P0=P0, Q0=Q0, oracle=(Po, Qo, lo), dev=dev)
-
-
-def check_against(got_P, got_Q, got_loss, P0, Q0, oracle):
-    """fp32 tables and an fp32 loss per lane against float64: at this shape the rounding alone is about 3e-5 of the
-    update on P.  Users run one wave early or late move the tables by far more (test_oracle_resolves_wave_membership)."""
-    Po, Qo, lo = oracle
-    errs = {}
-    for got, ref, init, name in ((got_P, Po, P0, 'P'), (got_Q, Qo, Q0, 'Q')):
-        update = np.abs(ref - init).max()
-        err = np.abs(got.astype(np.float64) - ref).max()
-        print('%s: max-abs error %.3g of an update of %.3g (ratio %.3g)' % (name, err, update, err / update))
-        assert update > 0
-        errs[name] = err / update
-    print('loss: relative error %.3g' % (abs(got_loss - lo) / lo))
-    assert errs['P'] <= 1e-4 and errs['Q'] <= 1e-4, errs
-    assert abs(got_loss - lo) <= 1e-5 * lo
 
 
 def test_oracle_resolves_wave_membership(case):
@@ -137,12 +80,7 @@ def test_host_pipeline_matches_wave_oracle(torch, E, case):
     """Small staging chunks: every chunk of whole users is a launch of its own, with waves sized for it."""
     c = case
     rowptr, chunk = c['rowptr'], 200_000
-    launches, ua = [], 0
-    while ua < USERS:                                   # the pipeline's cut: the most whole users within `chunk` triples
-        ub = int(np.searchsorted(rowptr, rowptr[ua] + chunk, side='right')) - 1
-        ub = min(max(ub, ua + 1), USERS, ua + chunk)
-        launches.append((ua, ub))
-        ua = ub
+    launches = pipeline_launches(rowptr, chunk)
     assert len(launches) > 10
     oracle = wave_oracle(c['P0'], c['Q0'], rowptr, c['i'], c['j'], launches, LR, REG)
     P, Q = c['dev'](c['P0']), c['dev'](c['Q0'])
