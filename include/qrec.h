@@ -234,18 +234,6 @@ int qrec_bpr_epoch_usermajor_f32(float* dev_P, float* dev_Q, int32_t d, int32_t 
                                  int32_t num_items, uint64_t seed, uint32_t epoch, int32_t* dev_j_out,
                                  float lr, float reg_u, float reg_i, double* dev_loss, void* stream);
 
-/* The fused epoch with the item rows staged through shared memory by the bulk-copy (TMA) engine: one
- * cp.async.bulk (256 bytes) per row into a per-lane-group staging slot, completion on an mbarrier, lanes read their
- * slices with LDS.128; two slots per group, so the next 4 triples' rows are in flight while 4 are computed.  The
- * same kernel body, chunking, waves and wave snapshot of the item table as qrec_bpr_epoch_usermajor_f32, so it
- * draws the same negatives and gives the same result up to the summation order of the scatter-adds.  d = 64 only;
- * dev_Q 16-byte aligned. */
-int qrec_bpr_epoch_usermajor_tma_f32(float* dev_P, float* dev_Q, int32_t d, int32_t n_users, int64_t n,
-                                     const int64_t* dev_rowptr, const int32_t* dev_i,
-                                     const int64_t* dev_rated_rowptr, const int32_t* dev_rated_cols,
-                                     int32_t num_items, uint64_t seed, uint32_t epoch, int32_t* dev_j_out,
-                                     float lr, float reg_u, float reg_i, double* dev_loss, void* stream);
-
 /* The fused epoch with a pre-test in the sampler: rated_sig holds 16 words per user, bit (c & 511) set
  * for every rated column c (qrec_rated_signature_build; static per data set).  A clear bit proves a
  * draw is not rated, so about 1 - deg/512 of the draws skip the binary search -- the dependent-load

@@ -102,8 +102,6 @@ SIGNATURES = {
                                              C.c_float, C.c_float, vp, vp]),
     'qrec_bpr_epoch_usermajor_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_int32,
                                                C.c_uint64, C.c_uint32, vp, C.c_float, C.c_float, C.c_float, vp, vp]),
-    'qrec_bpr_epoch_usermajor_tma_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_int32,
-                                                   C.c_uint64, C.c_uint32, vp, C.c_float, C.c_float, C.c_float, vp, vp]),
     'qrec_bpr_sgd_staged_f32': (C.c_int, [vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_float, C.c_float,
                                           C.c_float, vp, vp]),
     'qrec_ubench_row_ops_f32': (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int32, C.c_uint32, vp, vp]),

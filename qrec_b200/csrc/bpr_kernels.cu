@@ -367,31 +367,15 @@ bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long
 // the same Philox counter as the stand-alone sampler, so both give identical j) instead of being
 // read from j[] (FusedSampler, philox.cuh); they are optionally written to j_out.
 // SIG: the sampler pre-tests every draw against the user's 512-bit rated signature (philox.cuh).
-// TMA (d = 64 only): the item rows reach the lane group through shared memory instead of one LDG.128 per lane
-// and row.  One lane per row issues a 256-byte cp.async.bulk from Qr into the group's staging slot, completion is
-// signalled on the slot's mbarrier and the lanes read their slices with LDS.128, so the gathers leave the
-// LSU/L1TEX path, which then carries only the scatter-adds.  Two slots per lane group: the rows of the next G
-// triples are requested while the current G are computed.
-constexpr int UM_STAGE_FLOATS = 2 * 4 * 64;                  // one slot: the 2 x G rows of G = 4 triples, d = 64
-constexpr int UM_STAGE_GROUPS = 16;                          // lane groups of 16 lanes in a 256-thread CTA
-constexpr int UM_STAGE_SMEM = UM_STAGE_GROUPS * 2 * (UM_STAGE_FLOATS * 4 + 8);   // two slots + two mbarriers per group
-
-// one 256-byte row: global -> this CTA's shared memory, completion counted on `bar`
-__device__ __forceinline__ void bulk_row_load(float* smem_dst, const float* gsrc, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 256, [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(smem_u32(bar)) : "memory");
-}
-
-template <int LPR, int G, bool FULL, bool SAMPLE, bool SIG, bool TMA>   // FULL: d == 4*LPR (every lane owns a slice)
-__device__ __forceinline__ void
-usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, long long n,
-                const int* __restrict__ wave_user, const long long* __restrict__ rowptr, const int* __restrict__ i,
-                const int* __restrict__ j, float lr, float reg_u, float reg_i, double* loss, FusedSampler fs,
-                long long trip_off, const uint32_t* __restrict__ rated_sig) {
+template <int LPR, int G, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>   // FULL: d == 4*LPR (every lane owns a slice)
+__global__ void __launch_bounds__(256, MINB)
+bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, long long n,
+                         const int* __restrict__ wave_user, const long long* __restrict__ rowptr,
+                         const int* __restrict__ i, const int* __restrict__ j, float lr, float reg_u, float reg_i,
+                         double* loss, FusedSampler fs, long long trip_off, const uint32_t* __restrict__ rated_sig) {
   // rowptr holds GLOBAL triple offsets; i/j are indexed relative to trip_off (a chunk of users of a
   // larger epoch: the host pipeline stages one chunk at a time).  Philox counters use global indices.
   // wave_user[0 .. 1]: the wave's users [ua, ub).
-  static_assert(!TMA || (LPR == 16 && G == 4 && FULL), "the TMA fetch is laid out for d = 64, G = 4");
   constexpr int GPW = 32 / LPR;
   const int lane = threadIdx.x & 31;
   const int sub = lane / LPR, l = lane % LPR;
@@ -407,21 +391,6 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
   // launched now, and this wave reads neither Q nor Qr, nor writes anything, before pdl_wait() (`waited`)
   qrec::pdl_launch_dependents();
   bool waited = false;
-  float* stage = nullptr;                                    // TMA: this group's two slots and their mbarriers
-  uint64_t* bar = nullptr;
-  uint32_t phase0 = 0, phase1 = 0;
-  if constexpr (TMA) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    float* stage_all = reinterpret_cast<float*>(smem_raw);                                         // [GROUPS][2][8][64]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stage_all + UM_STAGE_GROUPS * 2 * UM_STAGE_FLOATS);  // [GROUPS][2]
-    const int g_in_cta = (threadIdx.x >> 5) * GPW + sub;
-    stage = stage_all + (size_t)g_in_cta * 2 * UM_STAGE_FLOATS;
-    bar = bars + g_in_cta * 2;
-    if (l == 0) { mbar_init(bar, 1); mbar_init(bar + 1, 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-  }
   const int ub = __ldg(wave_user + 1);
   for (int uu = __ldg(wave_user) + group; uu < ub; uu += ngroups) {
     // the launch's first and last users are cut where the caller cut the launch
@@ -438,7 +407,7 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
     }
     for (long long base = lo; base < hi; base += LPR) {
       const int m = (hi - base) < LPR ? (int)(hi - base) : LPR;
-      int mi = 0, mj = 0;
+      int mj = 0, mi = 0;
       if (l < m) {
         mi = __ldg(i + base + l);
         if (SAMPLE) {
@@ -458,26 +427,7 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
         waited = true;
       }
       if (SAMPLE && l < m && fs.j_out != nullptr) fs.j_out[base + l] = mj;
-      // TMA: request the rows of triples t0 .. t0+G-1 into slot (t0 / G) & 1: lane 2f -> Qr[i_f], lane 2f+1 -> Qr[j_f]
-      auto issue = [&](int t0) {
-        const int src = sub * LPR + ((t0 + (l >> 1)) & (LPR - 1));
-        const int idi = __shfl_sync(gmask, mi, src), idj = __shfl_sync(gmask, mj, src);
-        const int rows_now = 2 * ((m - t0) < G ? (m - t0) : G);
-        uint64_t* bb = bar + ((t0 / G) & 1);
-        if (l == 0) mbar_expect_tx(bb, 256u * rows_now);
-        __syncwarp(gmask);
-        if (l < rows_now) bulk_row_load(stage + ((t0 / G) & 1) * UM_STAGE_FLOATS + l * 64, Qr + (size_t)((l & 1) ? idj : idi) * d, bb);
-      };
-      if constexpr (TMA) issue(0);
       for (int t0 = 0; t0 < m; t0 += G) {
-        const float* slot = nullptr;
-        if constexpr (TMA) {
-          if (t0 + G < m) issue(t0 + G);
-          const int s = (t0 / G) & 1;
-          mbar_wait(bar + s, s ? phase1 : phase0);
-          if (s) phase1 ^= 1u; else phase0 ^= 1u;
-          slot = stage + s * UM_STAGE_FLOATS;
-        }
         float4 qi[G], qj[G];
         int ri[G], rj[G];
 #pragma unroll
@@ -485,19 +435,13 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
           ri[f] = __shfl_sync(gmask, mi, sub * LPR + ((t0 + f) & (LPR - 1)));
           rj[f] = __shfl_sync(gmask, mj, sub * LPR + ((t0 + f) & (LPR - 1)));
           if (t0 + f < m && act) {
-            if constexpr (TMA) {
-              qi[f] = *reinterpret_cast<const float4*>(slot + (2 * f) * 64 + l * 4);
-              qj[f] = *reinterpret_cast<const float4*>(slot + (2 * f + 1) * 64 + l * 4);
-            } else {
-              // not through L1: the previous wave's rows of Qr may still sit there (launch_usermajor)
-              qi[f] = qrec::ldg_no_l1_v4(reinterpret_cast<const float4*>(Qr + (size_t)ri[f] * d + l * 4));
-              qj[f] = qrec::ldg_no_l1_v4(reinterpret_cast<const float4*>(Qr + (size_t)rj[f] * d + l * 4));
-            }
+            // not through L1: the previous wave's rows of Qr may still sit there (launch_usermajor)
+            qi[f] = qrec::ldg_no_l1_v4(reinterpret_cast<const float4*>(Qr + (size_t)ri[f] * d + l * 4));
+            qj[f] = qrec::ldg_no_l1_v4(reinterpret_cast<const float4*>(Qr + (size_t)rj[f] * d + l * 4));
           } else {
             qi[f] = qj[f] = make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
-        if constexpr (TMA) __syncwarp(gmask);         // the slot may be requested again G triples on
 #pragma unroll
         for (int f = 0; f < G; ++f) {
           if (t0 + f < m) {                              // uniform inside the lane group
@@ -526,27 +470,7 @@ usermajor_epoch(float* __restrict__ P, float* __restrict__ Q, const float* __res
   block_add_loss(lsum, loss);
 }
 
-template <int LPR, int G, bool FULL, bool SAMPLE, int MINB = 3, bool SIG = false>
-__global__ void __launch_bounds__(256, MINB)
-bpr_sgd_usermajor_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec, long long n,
-                         const int* __restrict__ wave_user, const long long* __restrict__ rowptr,
-                         const int* __restrict__ i, const int* __restrict__ j, float lr, float reg_u, float reg_i,
-                         double* loss, FusedSampler fs, long long trip_off, const uint32_t* __restrict__ rated_sig) {
-  usermajor_epoch<LPR, G, FULL, SAMPLE, SIG, false>(P, Q, Qr, nvec, n, wave_user, rowptr, i, j, lr, reg_u, reg_i, loss, fs,
-                                                    trip_off, rated_sig);
-}
-
-// d = 64 with fused sampling, item rows staged in shared memory (UM_STAGE_SMEM bytes of dynamic shared memory)
-__global__ void __launch_bounds__(256, 3)
-bpr_sgd_usermajor_tma_kernel(float* __restrict__ P, float* __restrict__ Q, const float* __restrict__ Qr, int nvec,
-                             long long n, const int* __restrict__ wave_user, const long long* __restrict__ rowptr,
-                             const int* __restrict__ i, const int* __restrict__ j, float lr, float reg_u, float reg_i,
-                             double* loss, FusedSampler fs, long long trip_off, const uint32_t* __restrict__ rated_sig) {
-  usermajor_epoch<16, 4, true, true, false, true>(P, Q, Qr, nvec, n, wave_user, rowptr, i, j, lr, reg_u, reg_i, loss, fs,
-                                                  trip_off, rated_sig);
-}
-
-using UserMajorKernel = decltype(&bpr_sgd_usermajor_tma_kernel);
+using UserMajorKernel = decltype(&bpr_sgd_usermajor_kernel<16, 4, true, false>);
 
 // The instantiation for lane groups of LPR lanes: FULL when d = 4 LPR; the signature pre-test only then.  With FULL
 // fused sampling, G = 2 triples in flight fit 64 registers, so four 256-thread CTAs are resident per SM instead of
@@ -736,24 +660,20 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
                      const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i, double* loss,
                      bool sample, const int64_t* rated_rowptr, const int32_t* rated_cols, int32_t num_items,
                      uint64_t seed, uint32_t epoch, int32_t* j_out, long long trip_off, cudaStream_t st,
-                     const uint32_t* rated_sig, bool tma) {
+                     const uint32_t* rated_sig) {
   if (n <= 0) return QREC_OK;
   QREC_REQUIRE(num_items >= 1, "qrec user-major epoch: num_items=%d (the item table's rows) must be given", num_items);
-  QREC_REQUIRE(!tma || (d == 64 && sample), "qrec user-major epoch: the TMA fetch needs d = 64 and fused sampling");
   FusedSampler fs = {reinterpret_cast<const long long*>(rated_rowptr), rated_cols, num_items, (uint32_t)seed,
                      (uint32_t)(seed >> 32), epoch, j_out};
   const int nvec = d / 4;
   const int lpr = row_lpr(nvec);
   const bool sig = sample && rated_sig != nullptr;
   const UserMajorKernel kernel =
-      tma ? bpr_sgd_usermajor_tma_kernel
-          : with_row_shape<128>(nvec, [&](auto s) { return usermajor_kernel<decltype(s)::LPR>(nvec, sample, sig); });
-  const int smem = tma ? UM_STAGE_SMEM : 0;
-  if (tma) QREC_CUDA(allow_dynamic_smem((const void*)kernel, smem));
+      with_row_shape<128>(nvec, [&](auto s) { return usermajor_kernel<decltype(s)::LPR>(nvec, sample, sig); });
   // Grid = exactly the CTAs that are resident at once (occupancy API per instantiation); the stream is swept in
   // waves (um_waves.cuh), each reading the item table as the previous waves left it (a snapshot copied on the stream).
   int occ = 3;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, 256, smem) != cudaSuccess || occ < 1) occ = 3;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, 256, 0) != cudaSuccess || occ < 1) occ = 3;
   const long long per_block = 8 * (32 / lpr);                                 // lane groups per CTA
   const long long max_users = n < n_users ? n : n_users;                      // users with triples in the launch
   const int grid = capped_grid((max_users + per_block - 1) / per_block, occ);
@@ -781,11 +701,10 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
     cudaLaunchAttribute pdl;
     pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     pdl.val.programmaticStreamSerializationAllowed = 1;
-    const auto launch = [&](auto* fn, dim3 g, dim3 b, size_t shm, bool chained, auto... args) {
+    const auto launch = [&](auto* fn, dim3 g, dim3 b, bool chained, auto... args) {
       cudaLaunchConfig_t cfg = {};
       cfg.gridDim = g;
       cfg.blockDim = b;
-      cfg.dynamicSmemBytes = shm;
       cfg.stream = st;
       cfg.attrs = chained ? &pdl : nullptr;
       cfg.numAttrs = chained ? 1 : 0;
@@ -794,10 +713,10 @@ int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, 
     const long long n4 = (long long)(q_bytes / sizeof(float4));
     const int copy_grid = sm_count() * UM_SNAPSHOT_CTAS_PER_SM;
     for (long long w = 0; w < nwaves; ++w) {
-      QREC_CUDA(launch(um_snapshot_kernel, dim3(copy_grid), dim3(UM_SNAPSHOT_THREADS), 0, w > 0,
+      QREC_CUDA(launch(um_snapshot_kernel, dim3(copy_grid), dim3(UM_SNAPSHOT_THREADS), w > 0,
                        reinterpret_cast<const float4*>(Q), reinterpret_cast<float4*>(Qr), n4));
       count_launch();
-      QREC_CUDA(launch(kernel, dim3(grid), dim3(256), (size_t)smem, true, P, Q, static_cast<const float*>(Qr), nvec,
+      QREC_CUDA(launch(kernel, dim3(grid), dim3(256), true, P, Q, static_cast<const float*>(Qr), nvec,
                        (long long)n, static_cast<const int*>(wave_user + w), reinterpret_cast<const long long*>(rowptr), i, j,
                        lr, reg_u, reg_i, loss, fs, trip_off, rated_sig));
       if (w + 1 < nwaves) count_launch();
@@ -823,7 +742,7 @@ int qrec_bpr_sgd_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users, i
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && j, "qrec_bpr_sgd_usermajor_f32: null index pointer");
   return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, j, lr, reg_u, reg_i, loss, false, nullptr, nullptr, num_items,
-                                0, 0, nullptr, 0, (cudaStream_t)stream, nullptr, false);
+                                0, 0, nullptr, 0, (cudaStream_t)stream, nullptr);
 }
 
 int qrec_bpr_epoch_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
@@ -836,7 +755,7 @@ int qrec_bpr_epoch_usermajor_f32(float* P, float* Q, int32_t d, int32_t n_users,
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols, "qrec_bpr_epoch_usermajor_f32: null index pointer");
   return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, nullptr, lr, reg_u, reg_i, loss, true, rated_rowptr,
-                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, nullptr, false);
+                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, nullptr);
 }
 
 int qrec_rated_signature_build(int32_t n_users, const int64_t* rated_rowptr, const int32_t* rated_cols,
@@ -863,22 +782,7 @@ int qrec_bpr_epoch_usermajor_sig_f32(float* P, float* Q, int32_t d, int32_t n_us
   if (n_users == 0 || n == 0) return QREC_OK;
   QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols && rated_sig, "qrec_bpr_epoch_usermajor_sig_f32: null index pointer");
   return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, nullptr, lr, reg_u, reg_i, loss, true, rated_rowptr,
-                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, rated_sig, false);
-}
-
-int qrec_bpr_epoch_usermajor_tma_f32(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
-                                     const int32_t* i, const int64_t* rated_rowptr, const int32_t* rated_cols,
-                                     int32_t num_items, uint64_t seed, uint32_t epoch, int32_t* j_out, float lr,
-                                     float reg_u, float reg_i, double* loss, void* stream) {
-  QREC_REQUIRE(P && Q && loss, "qrec_bpr_epoch_usermajor_tma_f32: null pointer");
-  QREC_REQUIRE(d == 64, "qrec_bpr_epoch_usermajor_tma_f32: d=%d unsupported (64 only: one 256-byte bulk copy per row); use "
-                        "qrec_bpr_epoch_usermajor_f32", d);
-  QREC_REQUIRE(n_users >= 0 && n >= 0 && num_items >= 1, "qrec_bpr_epoch_usermajor_tma_f32: bad size");
-  if (n_users == 0 || n == 0) return QREC_OK;
-  QREC_REQUIRE(rowptr && i && rated_rowptr && rated_cols, "qrec_bpr_epoch_usermajor_tma_f32: null index pointer");
-  QREC_REQUIRE((reinterpret_cast<uintptr_t>(Q) & 15) == 0, "qrec_bpr_epoch_usermajor_tma_f32: Q must be 16-byte aligned");
-  return qrec::launch_usermajor(P, Q, d, n_users, n, rowptr, i, nullptr, lr, reg_u, reg_i, loss, true, rated_rowptr,
-                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, nullptr, true);
+                                rated_cols, num_items, seed, epoch, j_out, 0, (cudaStream_t)stream, rated_sig);
 }
 
 int qrec_bpr_sgd_staged_f32(float* P, int32_t d, int64_t n, const int32_t* u, const int32_t* pos_i,

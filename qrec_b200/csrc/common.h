@@ -27,12 +27,12 @@ int launch_bpr_batch(float* P, float* Q, int d, long long n, const int* u, const
                      float reg_u, float reg_i, double* loss, cudaStream_t st);
 // launch_usermajor: the user-major epoch over a CSR of whole users.  rowptr holds global triple offsets, i / j are
 // indexed from trip_off.  sample: draw the negatives in the kernel (FusedSampler) instead of reading j; rated_sig
-// (may be null) adds the signature pre-test; tma (d = 64, sample) stages the item rows with bulk copies.
+// (may be null) adds the signature pre-test.
 int launch_usermajor(float* P, float* Q, int32_t d, int32_t n_users, int64_t n, const int64_t* rowptr,
                      const int32_t* i, const int32_t* j, float lr, float reg_u, float reg_i, double* loss,
                      bool sample, const int64_t* rated_rowptr, const int32_t* rated_cols, int32_t num_items,
                      uint64_t seed, uint32_t epoch, int32_t* j_out, long long trip_off, cudaStream_t st,
-                     const uint32_t* rated_sig, bool tma);
+                     const uint32_t* rated_sig);
 
 inline int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
   set_error("%s failed at %s:%d: %s", what, file, line, cudaGetErrorString(e));

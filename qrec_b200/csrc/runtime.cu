@@ -145,7 +145,7 @@ int qrec_bpr_epoch_usermajor_host(qrec_ctx* c, float* P, float* Q, int32_t d, in
       const int rc = qrec::launch_usermajor(P + (size_t)ua * d, Q, d, ub - ua, m, c->rp_slot[r], c->slot[r], nullptr, lr,
                                             reg_u, reg_i, c->dev_loss, true, dev_rated_rowptr + ua, dev_rated_cols,
                                             num_items, seed, epoch, nullptr, t0, c->compute,
-                                            c->rated_sig ? c->rated_sig + (size_t)ua * 16 : nullptr, false);
+                                            c->rated_sig ? c->rated_sig + (size_t)ua * 16 : nullptr);
       if (rc != QREC_OK) return rc;
     }
     QREC_CUDA(cudaEventRecord(c->freed[r], c->compute));

@@ -343,20 +343,6 @@ def bpr_epoch_usermajor(P, Q, rowptr, i, rated_rowptr, rated_cols, num_items, se
     return loss
 
 
-def bpr_epoch_usermajor_tma(P, Q, rowptr, i, rated_rowptr, rated_cols, num_items, seed, epoch, lr, reg_u, reg_i, loss,
-                            j_out=None):
-    """bpr_epoch_usermajor with the item rows staged through shared memory by bulk (TMA) copies; d = 64."""
-    torch = _torch()
-    check(lib.qrec_bpr_epoch_usermajor_tma_f32(_dev(P, torch.float32, 'P'), _dev(Q, torch.float32, 'Q'), P.shape[1],
-                                               rowptr.shape[0] - 1, int(i.shape[0]), _dev(rowptr, torch.int64, 'rowptr'),
-                                               _dev(i, torch.int32, 'i'), _dev(rated_rowptr, torch.int64, 'rated_rowptr'),
-                                               _dev(rated_cols, torch.int32, 'rated_cols'), int(num_items), int(seed),
-                                               int(epoch), _dev(j_out, torch.int32, 'j_out') if j_out is not None else None,
-                                               float(lr), float(reg_u), float(reg_i), _dev(loss, torch.float64, 'loss'),
-                                               _stream()), 'qrec_bpr_epoch_usermajor_tma_f32')
-    return loss
-
-
 def rated_signature(rated_rowptr, rated_cols):
     """512-bit rated-set signature per user ([n_users, 16] int32 storage of uint32 words) for the
     pre-testing sampler of bpr_epoch_usermajor_sig; static per data set."""

@@ -116,7 +116,7 @@ def pipeline_launches(rowptr, chunk):
 #          ('sparse', m)     one user in fifty has 1 .. m triples, the others none
 #          ('long',)         users of 3 triples; two of 5 000 and 1 000 with an empty user between them, whose items
 #                            repeat; one whose rated row holds every item
-# entries: 'given' (negatives passed in), 'plain' / 'sig' / 'tma' (fused sampling), 'nojout' (plain, j_out absent),
+# entries: 'given' (negatives passed in), 'plain' / 'sig' (fused sampling), 'nojout' (plain, j_out absent),
 #          'pipe' / 'pipe_sig' (HostPipeline with `chunk` triples per launch, without / with the rated signature)
 # key:     (seed, epoch) of the Philox sampler
 # tol, loss_tol: check_against's bounds (P, Q) and loss, each at most 3 x the ratio observed on an H100 80GB HBM3 (700 W
@@ -139,16 +139,15 @@ TOL, LOSS_TOL = (5e-5, 2e-5), 3e-7             # (P, Q) and the loss
 
 
 def _width(d):
-    entries = ('given', 'plain') + (('sig',) if d in (16, 32, 64, 128) else ()) + (('tma',) if d == 64 else ()) \
-        + (('nojout',) if d == 52 else ())
+    entries = ('given', 'plain') + (('sig',) if d in (16, 32, 64, 128) else ()) + (('nojout',) if d == 52 else ())
     return Case('w%d' % d, 8_000, 3_000, d, ('tails',), 100 + d, entries, BIG_KEY, 0, TOL, LOSS_TOL)
 
 
 CASES = [_width(d) for d in (4, 12, 16, 20, 32, 48, 52, 64, 100, 128)] + [
     Case('long16', 300, 40, 16, ('long',), 16, ('given', 'plain', 'sig'), SMALL_KEY, 0, (9e-5, 7e-5), 3e-6),
-    Case('long64', 300, 40, 64, ('long',), 64, ('given', 'plain', 'sig', 'tma'), BIG_KEY, 0, (1.2e-4, 3e-5), 1e-5),
+    Case('long64', 300, 40, 64, ('long',), 64, ('given', 'plain', 'sig'), BIG_KEY, 0, (1.2e-4, 3e-5), 1e-5),
     Case('capped128', 8_000, 300, 128, ('uniform', 100), 7, ('given', 'plain', 'sig'), SMALL_KEY, 0, (5e-5, 3e-5), LOSS_TOL),
-    Case('large64', 25_000, 40_000, 64, ('uniform', 120), 8, ('given', 'plain', 'tma'), BIG_KEY, 0, (7e-5, 2e-5), LOSS_TOL),
+    Case('large64', 25_000, 40_000, 64, ('uniform', 120), 8, ('given', 'plain'), BIG_KEY, 0, (7e-5, 2e-5), LOSS_TOL),
     Case('sparse32', 200_000, 3_000, 32, ('sparse', 40), 9, ('given', 'plain', 'sig'), BIG_KEY, 0, TOL, LOSS_TOL),
     Case('pipe48', 8_000, 3_000, 48, ('tails',), 10, ('pipe', 'pipe_sig'), BIG_KEY, 20_000, TOL, LOSS_TOL),
     Case('pipe128', 8_000, 3_000, 128, ('tails',), 11, ('pipe', 'pipe_sig'), BIG_KEY, 40_000, TOL, LOSS_TOL),

@@ -1,7 +1,7 @@
 """Every instantiation of the user-major BPR epoch against the float64 wave oracle (k1_wave_oracle.py).
 
-usermajor_epoch<LPR, G, FULL, SAMPLE, SIG, TMA> (bpr_kernels.cu) is compiled for four lane-group sizes, each with and
-without idle lanes, with the negatives given or drawn in the kernel (plain, signature pre-test, TMA staging), and
+bpr_sgd_usermajor_kernel<LPR, G, FULL, SAMPLE, MINB, SIG> (bpr_kernels.cu) is compiled for four lane-group sizes, each
+with and without idle lanes, with the negatives given or drawn in the kernel (plain, signature pre-test), and
 launch_usermajor sizes its waves by three rules.  The cases of k1_wave_oracle.CASES reach all of them
 (test_k1_wave_oracle_cpu.py proves that without a GPU): ragged degrees around the lane-group size and the number of
 triples in flight, users longer than a wave whose items repeat, a saturated user, the 4 x items cap and the snapshot-copy
@@ -81,7 +81,7 @@ def test_epoch_matches_wave_oracle(torch, E, case, entry):
     seed, epoch = case.key
     P, Q = dev(c['P0']), dev(c['Q0'])
     loss = torch.zeros(1, dtype=torch.float64, device='cuda')
-    jo = torch.full((len(c['i']),), -1, dtype=torch.int32, device='cuda') if entry in ('plain', 'sig', 'tma') else None
+    jo = torch.full((len(c['i']),), -1, dtype=torch.int32, device='cuda') if entry in ('plain', 'sig') else None
     if entry in ('pipe', 'pipe_sig'):
         pipe = E.HostPipeline(0, chunk_triples=case.chunk)
         if entry == 'pipe_sig':
@@ -99,8 +99,6 @@ def test_epoch_matches_wave_oracle(torch, E, case, entry):
         elif entry == 'sig':
             E.bpr_epoch_usermajor_sig(*args, E.rated_signature(c['rrp'], c['rc']), case.items, seed, epoch, LR, REG_U, REG_I,
                                       loss, j_out=jo)
-        elif entry == 'tma':
-            E.bpr_epoch_usermajor_tma(*args, case.items, seed, epoch, LR, REG_U, REG_I, loss, j_out=jo)
         else:
             E.bpr_epoch_usermajor(*args, case.items, seed, epoch, LR, REG_U, REG_I, loss, j_out=jo)
         torch.cuda.synchronize()

@@ -57,7 +57,7 @@ def test_oracle_resolves_wave_membership(case):
         assert np.abs(got - ref).max() > 1e-3 * np.abs(ref - init).max()
 
 
-@pytest.mark.parametrize('entry', ['plain', 'sig', 'tma'])
+@pytest.mark.parametrize('entry', ['plain', 'sig'])
 def test_fused_epoch_matches_wave_oracle(torch, E, case, entry):
     c = case
     dev = c['dev']
@@ -67,10 +67,8 @@ def test_fused_epoch_matches_wave_oracle(torch, E, case, entry):
     args = (P, Q, dev(c['rowptr']), dev(c['i']), c['rrp'], c['rc'])
     if entry == 'plain':
         E.bpr_epoch_usermajor(*args, ITEMS, SEED, EPOCH, LR, REG, REG, loss, j_out=jo)
-    elif entry == 'sig':
-        E.bpr_epoch_usermajor_sig(*args, E.rated_signature(c['rrp'], c['rc']), ITEMS, SEED, EPOCH, LR, REG, REG, loss, j_out=jo)
     else:
-        E.bpr_epoch_usermajor_tma(*args, ITEMS, SEED, EPOCH, LR, REG, REG, loss, j_out=jo)
+        E.bpr_epoch_usermajor_sig(*args, E.rated_signature(c['rrp'], c['rc']), ITEMS, SEED, EPOCH, LR, REG, REG, loss, j_out=jo)
     torch.cuda.synchronize()
     assert np.array_equal(jo.cpu().numpy(), c['j']), 'fused sampler != stand-alone Philox sampler'
     check_against(P.cpu().numpy(), Q.cpu().numpy(), loss.item(), c['P0'], c['Q0'], c['oracle'])

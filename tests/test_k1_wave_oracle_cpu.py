@@ -1,7 +1,7 @@
 """The float64 wave oracle (k1_wave_oracle.py) checked without a GPU.
 
 The GPU tests of the user-major BPR epoch compare the kernel with wave_oracle, which is vectorised over the users of a
-wave.  Here it must equal a loop written straight from the comment above usermajor_epoch (bpr_kernels.cu) and the
+wave.  Here it must equal a loop written straight from the comment above bpr_sgd_usermajor_kernel (bpr_kernels.cu) and the
 chunk rule of um_waves.cuh, on small epochs built to hit what vectorising could get wrong; and every case of
 test_gpu_k1_matrix.py must reach the branch of the wave rule, the degrees and the lane shape it is named for."""
 import math
@@ -104,7 +104,7 @@ def test_the_widths_cover_every_lane_shape():
     shapes = {(row_lpr(c.d // 4), c.d == 4 * row_lpr(c.d // 4)) for c in CASES if c.name.startswith('w')}
     assert shapes == {(lpr, full) for lpr in (4, 8, 16, 32) for full in (False, True)}
     for c in CASES:
-        assert c.d % 4 == 0 and ('sig' not in c.entries or c.d in (16, 32, 64, 128)) and ('tma' not in c.entries or c.d == 64)
+        assert c.d % 4 == 0 and ('sig' not in c.entries or c.d in (16, 32, 64, 128))
 
 
 @pytest.mark.parametrize('case', CASES, ids=lambda c: c.name)

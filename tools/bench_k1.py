@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""K1 variants on the benchmark workload (50 M shuffled triples, 1M x 100K, d=64): REDG scatter vs
+"""K1 variants on the benchmark workload (50 M triples, 1M x 100K, d=64): the user-major epoch with given and with
+fused-sampled negatives, the stand-alone sampler, and the batch kernel on shuffled triples with REDG scatter vs
 bulk-copy-engine (TMA) scatter.  One JSON line each."""
 import json
 import os
@@ -45,10 +46,6 @@ def main():
         sig = E.rated_signature(data['sorted_rowptr'], data['sorted_cols'])
         fused.append(('fused sampling + signature pre-test',
                       lambda: E.bpr_epoch_usermajor_sig(P, Q, rowptr, data['i'], data['sorted_rowptr'], data['sorted_cols'], sig,
-                                                        I, 1, next(seeds), 0.01, 0.001, 0.001, loss)))
-    if True:
-        fused.append(('fused sampling, item rows staged by bulk (TMA) copies',
-                      lambda: E.bpr_epoch_usermajor_tma(P, Q, rowptr, data['i'], data['sorted_rowptr'], data['sorted_cols'],
                                                         I, 1, next(seeds), 0.01, 0.001, 0.001, loss)))
     for name, fn in fused:
         for _ in range(3):

@@ -112,8 +112,6 @@ def main():
         from qrec_b200.graph_build import JointAdjacency
         E.bpr_epoch_usermajor(P, Q, dev(csr.pos_rowptr), dev(csr.pos_cols), dev(csr.sorted_rowptr), dev(csr.sorted_cols), ni, 5, 0,
                               0.01, 0.001, 0.001, loss)
-        E.bpr_epoch_usermajor_tma(P, Q, dev(csr.pos_rowptr), dev(csr.pos_cols), dev(csr.sorted_rowptr), dev(csr.sorted_cols), ni, 5, 0,
-                                  0.01, 0.001, 0.001, loss)
         ids, vals = E.score_topn(P, Q, dev(np.arange(nu, dtype=np.int32)), dev(csr.sorted_rowptr), dev(csr.sorted_cols), 10)
         J = JointAdjacency(dev(u.astype(np.int64)), dev(i.astype(np.int64)), nu, ni, device='cuda')
         J.full(); J.edge_dropout(0.3, 1, 2, 3)
