@@ -699,6 +699,47 @@ int qrec_svdpp_epoch_usermajor_f32(float* dev_P, float* dev_Q, float* dev_Y, flo
                                    float reg_b, float reg_y, float global_mean, double* dev_loss,
                                    int64_t max_users_in_flight, void* stream);
 
+/* =====================================================================================
+ * K12 -- CoFactor (model/ranking/CoFactor.py): WRMF plus a co-factorisation of the item-item SPPMI matrix.  The user
+ * half-epoch is K10's qrec_als_solve_rows_*; the SPPMI's co-occurrence counts and the item half-epoch are here.
+ * ===================================================================================== */
+/* Co-occurrence counts of the eligible items (at least `filter` distinct users): for each listed row i and each
+ * eligible j != i, the number of users of both, kept when > filter.  item_rowptr / item_users: every item's DISTINCT
+ * users; user_rowptr / user_items: its transpose, each user's items in ascending order.  One CTA per row, rows taken
+ * from row_order[0..n_rows) (eligible items only; longest first balances the grid).  Two passes:
+ *   out_rowptr == NULL: row_nnz[i] = number of kept entries of each listed row (other rows untouched);
+ *   out_rowptr != NULL: the kept columns of row i, ascending, go to out_cols[out_rowptr[i]..] with their counts.
+ * Exact integer counts, the same on every run. */
+int qrec_cooc_count(int32_t n_items, const int64_t* dev_item_rowptr, const int32_t* dev_item_users,
+                    const int64_t* dev_user_rowptr, const int32_t* dev_user_items, int32_t n_rows,
+                    const int32_t* dev_row_order, int32_t filter, const int64_t* dev_out_rowptr, int64_t* dev_row_nnz,
+                    int32_t* dev_out_cols, int32_t* dev_out_counts, void* stream);
+/* One item half-epoch in item-id order, in place (tables Y, G [n_items][d], w, c [n_items]; X [num_users][d] only
+ * read; XtX = X^T X from qrec_als_gram_*).  Item i's users are item_users[item_rowptr[i]..] with ratings item_vals,
+ * its SPPMI contexts sppmi_cols[sppmi_rowptr[i]..] with values sppmi_vals (the SPPMI must be symmetric):
+ *   Y_i = (XtX + alpha*sum r x x^T + lambda*I + sum_c G_c G_c^T)^-1 (sum (1 + alpha*r) x + sum_c ((m - w_i) - c_c) G_c)
+ *   and, for an item with contexts, G_i = (sum_c Y_c Y_c^T + gamma*I)^-1 sum_c ((m - w_c) - c_i) Y_c,
+ *   w_i = mean_c ((m - Y_i.G_c) - c_c), c_i = mean_c ((m - Y_c.G_i) - w_c)  with item i's values from before it.
+ * Contexts c < i are read after their update in this sweep, c > i before it, as in the sequential loop: CTAs take
+ * items in id order from dev_ticket (uint64[1], zero on entry) and wait until every smaller context's stamp
+ * (dev_stamps int32[n_items], all sweep - 1 on entry) equals `sweep`; each item then adds 1 to its stamp.  A and b
+ * are float64; the result is bitwise reproducible.  A system that is not positive definite leaves its row unchanged
+ * and is counted in dev_n_failed (optional, int32[1]).  d: 1..128. */
+int qrec_cofactor_item_sweep_f32(float* dev_Y, float* dev_G, float* dev_w, float* dev_c, const float* dev_X,
+                                 const double* dev_XtX, int32_t d, int32_t n_items, const int64_t* dev_item_rowptr,
+                                 const int32_t* dev_item_users, const float* dev_item_vals,
+                                 const int64_t* dev_sppmi_rowptr, const int32_t* dev_sppmi_cols,
+                                 const float* dev_sppmi_vals, double lambda, double gamma, double alpha,
+                                 int32_t* dev_stamps, int32_t sweep, unsigned long long* dev_ticket,
+                                 int32_t* dev_n_failed, void* stream);
+int qrec_cofactor_item_sweep_f64(double* dev_Y, double* dev_G, double* dev_w, double* dev_c, const double* dev_X,
+                                 const double* dev_XtX, int32_t d, int32_t n_items, const int64_t* dev_item_rowptr,
+                                 const int32_t* dev_item_users, const double* dev_item_vals,
+                                 const int64_t* dev_sppmi_rowptr, const int32_t* dev_sppmi_cols,
+                                 const double* dev_sppmi_vals, double lambda, double gamma, double alpha,
+                                 int32_t* dev_stamps, int32_t sweep, unsigned long long* dev_ticket,
+                                 int32_t* dev_n_failed, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,6 +87,11 @@ SIGNATURES = {
                                           vp, vp, vp]),
     'qrec_als_solve_rows_f64': (C.c_int, [vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double,
                                           vp, vp, vp]),
+    'qrec_cooc_count': (C.c_int, [C.c_int32, vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp, vp, vp, vp]),
+    'qrec_cofactor_item_sweep_f32': (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp,
+                                               C.c_double, C.c_double, C.c_double, vp, C.c_int32, vp, vp, vp]),
+    'qrec_cofactor_item_sweep_f64': (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp,
+                                               C.c_double, C.c_double, C.c_double, vp, C.c_int32, vp, vp, vp]),
     'qrec_svdpp_sgd_ordered_f64': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_double,
                                              C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
     'qrec_svdpp_sgd_ordered_f32': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_float,

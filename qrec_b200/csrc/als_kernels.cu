@@ -12,9 +12,15 @@
 //     feeds four FMAs), factors A in shared memory (als_step.cuh) and substitutes with one warp.  The grid is
 //     persistent and walks the caller's row order (longest rows first keeps one long row from becoming the tail).
 //     Nothing depends on scheduling, so the solved tables are bitwise reproducible.
+//
+//   CoFactor (model/ranking/CoFactor.py): the user half-epoch is WRMF's; the item half-epoch adds the item-item SPPMI
+//   co-factorisation (cofactor_step.cuh) and runs in item-id order, updating in place.
+//   * cofactor_item_sweep_kernel -- one CTA per item, on the same staging, tiles and Cholesky as the row solve; the
+//     in-order dataflow is kept with per-item stamps (see the kernel's comment).
 #include "common.h"
 #include "device.cuh"
 #include "als_step.cuh"
+#include "cofactor_step.cuh"
 
 namespace {
 
@@ -106,8 +112,9 @@ struct Tiles {
 };
 
 // Stages rows row_of(k) of Z (k < cnt) as float64 with zero columns up to dp.  Each warp gathers its kStage/8 rows
-// into registers first, so all of a thread's loads are in flight together, then stores them.
-template <typename T, class RowOf>
+// into registers first, so all of a thread's loads are in flight together, then stores them.  kCoherent: Z is written
+// by other CTAs of the same launch, so its rows are read from L2 (__ldcg) instead of the read-only path.
+template <typename T, bool kCoherent = false, class RowOf>
 __device__ __forceinline__ void stage_rows(double* Zs, const T* __restrict__ Z, int d, int dp, int cnt, RowOf row_of) {
   constexpr int kWarps = kThreads / 32, R = kStage / kWarps, C = kMaxD / 32;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -119,7 +126,7 @@ __device__ __forceinline__ void stage_rows(double* Zs, const T* __restrict__ Z, 
 #pragma unroll
     for (int e = 0; e < C; ++e) {
       const int c = e * 32 + lane;
-      v[m][e] = k < cnt && c < d ? (double)__ldg(z + c) : 0.0;
+      v[m][e] = k < cnt && c < d ? (double)(kCoherent ? __ldcg(z + c) : __ldg(z + c)) : 0.0;
     }
   }
 #pragma unroll
@@ -129,6 +136,58 @@ __device__ __forceinline__ void stage_rows(double* Zs, const T* __restrict__ Z, 
     for (int e = 0; e < C; ++e)
       if (k < cnt && e * 32 + lane < dp) Zs[k * dp + e * 32 + lane] = v[m][e];
   }
+}
+
+// Factors the upper triangle of A (d x d, leading dimension ld) in place with the whole CTA (als_step.cuh) and solves
+// A x = bv with warp 0, which stores x to out: the steps of als_solve_rows_kernel's tail, for the item sweep's two
+// solves (WRMF's kernel keeps its own inline copy, so its code stays as it was).  Entered after a barrier that
+// published A and bv.  Returns false on every thread when a pivot is not positive and finite; out is then untouched.
+template <typename T>
+__device__ __forceinline__ bool chol_solve(double* A, int d, int ld, double* sd, const double* bv, T* out) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  for (int j = 0; j < d; ++j) {
+    const double p = A[j * ld + j];
+    if (!als_pivot_ok(p)) return false;                // uniform: every thread reads the same pivot
+    const double s = als_pivot_scale(p);
+    if (t == 0) sd[j] = s;
+    als_chol_step(A, d, ld, j, s, t, kThreads);
+    __syncthreads();
+  }
+  als_chol_scale_rows(A, d, ld, sd, t, kThreads);
+  __syncthreads();
+  if (warp == 0) {                                      // U^T y = b, U x = y (als_solve, one warp)
+    double y[kMaxD / 32];
+#pragma unroll
+    for (int e = 0; e < kMaxD / 32; ++e) y[e] = e * 32 + lane < d ? bv[e * 32 + lane] : 0.0;
+    for (int j = 0; j < d; ++j) {
+      double v = 0.0;
+#pragma unroll
+      for (int e = 0; e < kMaxD / 32; ++e) if (e == (j >> 5)) v = y[e];
+      const double yj = __shfl_sync(0xffffffffu, v, j & 31) * sd[j];
+#pragma unroll
+      for (int e = 0; e < kMaxD / 32; ++e) {
+        const int i = e * 32 + lane;
+        if (i == j) y[e] = yj;
+        else if (i > j && i < d) y[e] = als_sub(y[e], A[j * ld + i], yj);
+      }
+    }
+    for (int i = d - 1; i >= 0; --i) {
+      double v = 0.0;
+#pragma unroll
+      for (int e = 0; e < kMaxD / 32; ++e) if (e == (i >> 5)) v = y[e];
+      const double xi = __shfl_sync(0xffffffffu, v, i & 31) * sd[i];
+#pragma unroll
+      for (int e = 0; e < kMaxD / 32; ++e) {
+        const int m = e * 32 + lane;
+        if (m == i) y[e] = xi;
+        else if (m < i) y[e] = als_sub(y[e], A[m * ld + i], xi);
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < kMaxD / 32; ++e)
+      if (e * 32 + lane < d) out[e * 32 + lane] = (T)y[e];
+  }
+  return true;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -295,6 +354,178 @@ als_solve_rows_kernel(T* __restrict__ X, const T* __restrict__ Z, const double* 
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// CoFactor item sweep
+// ------------------------------------------------------------------------------------------
+// Shared-memory carve-up (doubles): A, Zs [kStage][dp], W / M / O [kStage] (tile weight, SPPMI value, the context's
+// c or w), y_old, g_old, b, s [dp].
+inline size_t cof_smem_bytes(int d) {
+  return sizeof(double) * ((size_t)a_words(d) + (size_t)(kStage + 4) * pad4(d) + 3 * kStage);
+}
+
+__device__ __forceinline__ void wait_stamp(const int* p, int sweep) {
+  unsigned backoff = 32, polls = 0;
+  while (ld_acquire_gpu(p) != sweep) {
+    __nanosleep(backoff);
+    if (backoff < 256) backoff <<= 1;
+    // as in the ordered SGD kernels: ~10 s of polling means the stamps do not belong to this sweep -- abort the
+    // launch instead of hanging the GPU
+    if (++polls > (1u << 25)) __trap();
+  }
+}
+
+// One in-order item sweep (CoFactor.py, trainModel, item loop; arithmetic in cofactor_step.cuh).  For item i:
+//   A_Y = XtX + sum_u alpha*r x x^T + lambda*I + sum_c G_c G_c^T  -> Y_i      (X rows weight alpha*r, G rows weight 1)
+//   A_G = sum_c Y_c Y_c^T + gamma*I                               -> G_i, then w_i, c_i   (items with contexts only)
+// A and b are float64; a system that is not positive definite leaves its row unchanged and is counted in n_failed.
+//
+// Order.  The reference updates in place in item-id order, so a context c < i is read after its own update in this
+// sweep and c > i before it.  CTAs take items from `ticket` in id order.  Before reading its contexts a CTA waits
+// (acquire) until the stamp of every context c < i equals `sweep`; after writing Y_i, G_i, w_i, c_i it publishes its
+// own stamp (release add).  The SPPMI is symmetric, so a context c > i has i among its own contexts and waits for
+// i's stamp before it reads anything of i or writes its own rows: i reads c's values from before the sweep.
+// No deadlock: a CTA takes a ticket only while it runs and holds one at a time, and it waits only on smaller tickets,
+// which running CTAs hold; the CTA with the smallest unfinished ticket waits on nobody, so it always finishes.  Every
+// CTA of the persistent grid is resident at once (persistent_grid sizes it by occupancy), so no waiting CTA keeps
+// another from being scheduled.  Rows other CTAs write (Y, G, w, c) are read through L2.  The schedule only changes
+// when a value is computed, never from what, so the result is bitwise the same on every run.
+template <typename T, int NT>
+__global__ void __launch_bounds__(kThreads, NT == 1 ? 2 : 1)
+cofactor_item_sweep_kernel(T* Y, T* G, T* wb, T* cb, const T* __restrict__ X, const double* __restrict__ XtX, int d,
+                           int n_items, const long long* __restrict__ irp, const int* __restrict__ icol,
+                           const T* __restrict__ ival, const long long* __restrict__ srp, const int* __restrict__ scol,
+                           const T* __restrict__ sval, double lambda, double gamma, double alpha, int* stamps,
+                           int sweep, unsigned long long* ticket, int* n_failed) {
+  extern __shared__ __align__(16) double smem[];
+  __shared__ long long s_item;
+  __shared__ double part[2][kThreads / 32];
+  const int dp = pad4(d), ld = dp + 1;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  double* A = smem;
+  double* Zs = A + a_words(d);
+  double* W = Zs + kStage * dp;
+  double* M = W + kStage;
+  double* O = M + kStage;
+  double* yo = O + kStage;
+  double* go = yo + dp;
+  double* bv = go + dp;
+  double* sd = bv + dp;
+  Tiles<NT> tl;
+  tl.setup(d);
+  while (true) {
+    __syncthreads();                                   // the previous item is done with the buffers and s_item
+    if (t == 0) s_item = (long long)atomicAdd(ticket, 1ULL);
+    __syncthreads();
+    if (s_item >= n_items) break;
+    const int i = (int)s_item;
+    const long long ub = __ldg(irp + i), ue = __ldg(irp + i + 1), cbeg = __ldg(srp + i), cend = __ldg(srp + i + 1);
+    const int nctx = (int)(cend - cbeg);
+    T* yi = Y + (size_t)i * d;
+    T* gi = G + (size_t)i * d;
+    const double w_i = (double)__ldcg(wb + i), c_i = (double)__ldcg(cb + i);
+    for (int c = t; c < dp; c += kThreads) {
+      yo[c] = c < d ? (double)__ldcg(yi + c) : 0.0;
+      go[c] = c < d ? (double)__ldcg(gi + c) : 0.0;
+    }
+    // users: X rows with weight alpha*r (X is not written in this sweep; nothing to wait for)
+    tl.zero();
+    double bx = 0.0;
+    for (long long k0 = ub; k0 < ue; k0 += kStage) {
+      const int cnt = (int)(ue - k0 < kStage ? ue - k0 : kStage);
+      __syncthreads();
+      stage_rows<T>(Zs, X, d, dp, cnt, [=](int k) { return __ldg(icol + k0 + k); });
+      for (int k = t; k < cnt; k += kThreads) W[k] = als_conf<T>(__ldg(ival + k0 + k), alpha);
+      __syncthreads();
+      tl.accumulate(Zs, W, dp, cnt);
+      if (t < d)
+        for (int k = 0; k < cnt; ++k) bx = fma(als_rhs_weight(W[k]), Zs[k * dp + t], bx);
+    }
+    for (long long k = cbeg + t; k < cend; k += kThreads) {
+      const int c = __ldg(scol + k);
+      if (c < i) wait_stamp(stamps + c, sweep);
+    }
+    __syncthreads();
+    // contexts, first pass: G rows with weight 1 into A_Y and b_Y, and w_i's sum
+    double bg = 0.0, wsum = 0.0;
+    for (long long k0 = cbeg; k0 < cend; k0 += kStage) {
+      const int cnt = (int)(cend - k0 < kStage ? cend - k0 : kStage);
+      __syncthreads();
+      stage_rows<T, true>(Zs, G, d, dp, cnt, [=](int k) { return __ldg(scol + k0 + k); });
+      for (int k = t; k < cnt; k += kThreads) {
+        W[k] = 1.0;
+        M[k] = (double)__ldg(sval + k0 + k);
+        O[k] = (double)__ldcg(cb + __ldg(scol + k0 + k));
+      }
+      __syncthreads();
+      tl.accumulate(Zs, W, dp, cnt);
+      if (t < d)
+        for (int k = 0; k < cnt; ++k) bg = fma(cof_rhs_y_coef(M[k], w_i, O[k]), Zs[k * dp + t], bg);
+      for (int k = warp; k < cnt; k += kThreads / 32) {
+        double yg = 0.0;
+        for (int c = lane; c < d; c += 32) yg = fma(yo[c], Zs[k * dp + c], yg);
+        yg = warp_sum(yg);
+        if (lane == 0) wsum += cof_w_term(M[k], yg, O[k]);
+      }
+    }
+    __syncthreads();
+    tl.reduce_into(A, d, ld);
+    for (int e = t; e < d * d; e += kThreads) {
+      const int a = e / d, b = e % d;
+      if (a <= b) A[a * ld + b] = (__ldg(XtX + e) + A[a * ld + b]) + (a == b ? lambda : 0.0);
+    }
+    if (t < d) bv[t] = bx + bg;
+    __syncthreads();
+    if (!chol_solve<T>(A, d, ld, sd, bv, yi) && t == 0 && n_failed != nullptr) atomicAdd(n_failed, 1);
+    if (nctx > 0) {
+      // contexts, second pass: Y rows into A_G and b_G, and c_i's sum
+      tl.zero();
+      double by = 0.0, csum = 0.0;
+      for (long long k0 = cbeg; k0 < cend; k0 += kStage) {
+        const int cnt = (int)(cend - k0 < kStage ? cend - k0 : kStage);
+        __syncthreads();
+        stage_rows<T, true>(Zs, Y, d, dp, cnt, [=](int k) { return __ldg(scol + k0 + k); });
+        for (int k = t; k < cnt; k += kThreads) {
+          W[k] = 1.0;
+          M[k] = (double)__ldg(sval + k0 + k);
+          O[k] = (double)__ldcg(wb + __ldg(scol + k0 + k));
+        }
+        __syncthreads();
+        tl.accumulate(Zs, W, dp, cnt);
+        if (t < d)
+          for (int k = 0; k < cnt; ++k) by = fma(cof_rhs_g_coef(M[k], O[k], c_i), Zs[k * dp + t], by);
+        for (int k = warp; k < cnt; k += kThreads / 32) {
+          double yg = 0.0;
+          for (int c = lane; c < d; c += 32) yg = fma(go[c], Zs[k * dp + c], yg);
+          yg = warp_sum(yg);
+          if (lane == 0) csum += cof_c_term(M[k], yg, O[k]);
+        }
+      }
+      __syncthreads();
+      tl.reduce_into(A, d, ld);
+      for (int a = t; a < d; a += kThreads) A[a * ld + a] += gamma;
+      if (t < d) bv[t] = by;
+      if (lane == 0) {
+        part[0][warp] = wsum;
+        part[1][warp] = csum;
+      }
+      __syncthreads();
+      if (!chol_solve<T>(A, d, ld, sd, bv, gi) && t == 0 && n_failed != nullptr) atomicAdd(n_failed, 1);
+      if (t == 0) {
+        double sw = 0.0, sc = 0.0;
+        for (int w = 0; w < kThreads / 32; ++w) {
+          sw += part[0][w];
+          sc += part[1][w];
+        }
+        wb[i] = (T)cof_mean(sw, nctx);
+        cb[i] = (T)cof_mean(sc, nctx);
+      }
+    }
+    __threadfence();
+    __syncthreads();
+    if (t == 0) red_release_gpu_add(stamps + i, 1);
+  }
+}
+
 // persistent grid: as many CTAs as fit on the GPU at `bytes` of dynamic shared memory, at most `work`
 template <class K>
 int persistent_grid(K kernel, size_t bytes, long long work, int* grid) {
@@ -363,6 +594,37 @@ int launch_solve(T* X, const T* Z, const double* G, int d, long long n_order, co
   return QREC_OK;
 }
 
+template <typename T>
+int launch_cofactor(T* Y, T* G, T* w, T* c, const T* X, const double* XtX, int d, int n_items, const long long* irp,
+                    const int* icol, const T* ival, const long long* srp, const int* scol, const T* sval, double lambda,
+                    double gamma, double alpha, int* stamps, int sweep, unsigned long long* ticket, int* n_failed,
+                    cudaStream_t st) {
+  QREC_REQUIRE(d >= 1 && d <= kMaxD, "cofactor_item_sweep: d=%d unsupported (1..%d)", d, kMaxD);
+  QREC_REQUIRE(n_items >= 0, "cofactor_item_sweep: n_items < 0");
+  if (n_items == 0) return QREC_OK;
+  QREC_REQUIRE(Y && G && w && c && X && XtX && irp && srp && stamps && ticket, "cofactor_item_sweep: null pointer");
+  QREC_REQUIRE((const void*)Y != (const void*)G && (const void*)Y != (const void*)X && (const void*)G != (const void*)X,
+               "cofactor_item_sweep: Y, G and X must be different tables");
+  QREC_REQUIRE(sweep >= 1, "cofactor_item_sweep: sweep=%d (stamps count sweeps from 1)", sweep);
+  const size_t bytes = cof_smem_bytes(d);
+  int grid = 0;
+  if (tiles_of(d) <= kThreads) {
+    const int rc = persistent_grid(cofactor_item_sweep_kernel<T, 1>, bytes, n_items, &grid);
+    if (rc) return rc;
+    cofactor_item_sweep_kernel<T, 1><<<grid, kThreads, bytes, st>>>(Y, G, w, c, X, XtX, d, n_items, irp, icol, ival,
+                                                                     srp, scol, sval, lambda, gamma, alpha, stamps,
+                                                                     sweep, ticket, n_failed);
+  } else {
+    const int rc = persistent_grid(cofactor_item_sweep_kernel<T, 3>, bytes, n_items, &grid);
+    if (rc) return rc;
+    cofactor_item_sweep_kernel<T, 3><<<grid, kThreads, bytes, st>>>(Y, G, w, c, X, XtX, d, n_items, irp, icol, ival,
+                                                                     srp, scol, sval, lambda, gamma, alpha, stamps,
+                                                                     sweep, ticket, n_failed);
+  }
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -394,6 +656,26 @@ int qrec_als_solve_rows_f64(double* X, const double* Z, const double* G, int32_t
                             double lambda, double alpha, double* loss, int32_t* n_failed, void* stream) {
   return launch_solve<double>(X, Z, G, d, n_rows, row_order, (const long long*)rowptr, cols, vals, lambda, alpha,
                               loss, n_failed, (cudaStream_t)stream);
+}
+
+int qrec_cofactor_item_sweep_f32(float* Y, float* G, float* w, float* c, const float* X, const double* XtX, int32_t d,
+                                 int32_t n_items, const int64_t* item_rowptr, const int32_t* item_users,
+                                 const float* item_vals, const int64_t* sppmi_rowptr, const int32_t* sppmi_cols,
+                                 const float* sppmi_vals, double lambda, double gamma, double alpha, int32_t* stamps,
+                                 int32_t sweep, unsigned long long* ticket, int32_t* n_failed, void* stream) {
+  return launch_cofactor<float>(Y, G, w, c, X, XtX, d, n_items, (const long long*)item_rowptr, item_users, item_vals,
+                                (const long long*)sppmi_rowptr, sppmi_cols, sppmi_vals, lambda, gamma, alpha, stamps,
+                                sweep, ticket, n_failed, (cudaStream_t)stream);
+}
+
+int qrec_cofactor_item_sweep_f64(double* Y, double* G, double* w, double* c, const double* X, const double* XtX,
+                                 int32_t d, int32_t n_items, const int64_t* item_rowptr, const int32_t* item_users,
+                                 const double* item_vals, const int64_t* sppmi_rowptr, const int32_t* sppmi_cols,
+                                 const double* sppmi_vals, double lambda, double gamma, double alpha, int32_t* stamps,
+                                 int32_t sweep, unsigned long long* ticket, int32_t* n_failed, void* stream) {
+  return launch_cofactor<double>(Y, G, w, c, X, XtX, d, n_items, (const long long*)item_rowptr, item_users, item_vals,
+                                 (const long long*)sppmi_rowptr, sppmi_cols, sppmi_vals, lambda, gamma, alpha, stamps,
+                                 sweep, ticket, n_failed, (cudaStream_t)stream);
 }
 
 }  // extern "C"

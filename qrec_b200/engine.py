@@ -6,6 +6,7 @@ sm_90a kernels.  There is no CPU path here: device entry points raise if a tenso
 CUDA device.
 """
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -1030,6 +1031,125 @@ def als_solve_rows(X, Z, G, rowptr, cols, vals, lam, alpha, row_order, loss=None
             raise QRecError('als_solve_rows: %d row(s) with normal equations that are not positive definite were '
                             'left unchanged' % bad)
     return X
+
+
+# =============================================================================================
+# K12: CoFactor -- SPPMI co-occurrence counts and the in-order item sweep
+# =============================================================================================
+def cooc_count(item_rowptr, item_users, num_users, filt):
+    """Co-occurrence counts of CoFactor's SPPMI (CoFactor.py, initModel) on the device.  item_rowptr (int64
+    [num_items + 1]) / item_users (int32): every item's DISTINCT users (Rating.rating_csr('item')).  Items with at
+    least `filt` users are eligible; for eligible i != j the count of common users is kept when > filt.
+    Returns the CSR (rowptr int64, cols int32 ascending per row, counts int32), symmetric."""
+    torch = _torch()
+    n_items = item_rowptr.shape[0] - 1
+    _dev(item_rowptr, torch.int64, 'item_rowptr')
+    _dev(item_users, torch.int32, 'item_users')
+    dev = item_rowptr.device
+    nnz = item_users.shape[0]
+    if nnz == 0:                                  # no ratings: no pairs
+        return (torch.zeros(n_items + 1, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev),
+                torch.empty(0, dtype=torch.int32, device=dev))
+    if int(item_users.min()) < 0 or int(item_users.max()) >= num_users:
+        raise QRecError('cooc_count: a user id is outside [0, %d)' % num_users)
+    deg = item_rowptr[1:] - item_rowptr[:-1]
+    item_of = torch.repeat_interleave(torch.arange(n_items, dtype=torch.int32, device=dev), deg, output_size=nnz)
+    # user-major transpose with ascending items: the item-major entries are in item order, the sort is stable
+    user_items = item_of[torch.sort(item_users, stable=True).indices].contiguous()
+    udeg = torch.bincount(item_users, minlength=num_users)
+    user_rowptr = torch.zeros(num_users + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(udeg, 0, out=user_rowptr[1:])
+    # eligible rows, the most user-item steps first (sum over the row's users of their degrees)
+    work = torch.zeros(n_items, dtype=torch.int64, device=dev).index_add_(0, item_of.long(), udeg[item_users.long()])
+    elig = torch.nonzero(deg >= filt).flatten()
+    order = elig[torch.argsort(work[elig], descending=True, stable=True)].to(torch.int32).contiguous()
+    row_nnz = torch.zeros(n_items, dtype=torch.int64, device=dev)
+    args = (n_items, item_rowptr.data_ptr(), item_users.data_ptr(), user_rowptr.data_ptr(), user_items.data_ptr(),
+            order.shape[0], order.data_ptr(), int(filt))
+    check(lib.qrec_cooc_count(*args, None, row_nnz.data_ptr(), None, None, _stream()), 'qrec_cooc_count')
+    rowptr = torch.zeros(n_items + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(row_nnz, 0, out=rowptr[1:])
+    total = int(rowptr[-1])
+    cols = torch.empty(total, dtype=torch.int32, device=dev)
+    counts = torch.empty(total, dtype=torch.int32, device=dev)
+    if total:
+        check(lib.qrec_cooc_count(*args, rowptr.data_ptr(), None, cols.data_ptr(), counts.data_ptr(), _stream()),
+              'qrec_cooc_count')
+    return rowptr, cols, counts
+
+
+def sppmi_csr(item_rowptr, item_users, num_users, k, filt, dtype=None):
+    """CoFactor's SPPMI matrix (CoFactor.py, initModel) as a device CSR (rowptr int64, cols int32 ascending, vals):
+    with f_i the sum of row i's kept counts and D the sum of all f, the value of a pair is
+    max(log((count*D) / (f_i*f_j)) - log(k), 0) in float64, kept when > 0, then divided by the largest value.
+    k < 1 counts as 1.  vals are float64, or `dtype`."""
+    torch = _torch()
+    rowptr, cols, counts = cooc_count(item_rowptr, item_users, num_users, filt)
+    n_items = rowptr.shape[0] - 1
+    dev = rowptr.device
+    rows = torch.repeat_interleave(torch.arange(n_items, device=dev), rowptr[1:] - rowptr[:-1], output_size=cols.shape[0])
+    cnt = counts.to(torch.float64)
+    f = torch.zeros(n_items, dtype=torch.float64, device=dev).index_add_(0, rows, cnt)   # integer sums: exact
+    D = f.sum()
+    val = torch.log((cnt * D) / (f[rows] * f[cols.long()])) - math.log(max(int(k), 1))
+    keep = val > 0
+    val, cols, rows = val[keep], cols[keep].contiguous(), rows[keep]
+    out_rowptr = torch.zeros(n_items + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(torch.bincount(rows, minlength=n_items), 0, out=out_rowptr[1:])
+    if val.numel():
+        val = val / val.max()
+    return out_rowptr, cols, val.to(dtype or torch.float64).contiguous()
+
+
+def cofactor_item_sweep(Y, G, w, c, X, XtX, item_csr, sppmi, lam, gamma, alpha, n_failed=None, stamps=None,
+                        sweep=1):
+    """One in-order item half-epoch of CoFactor (CoFactor.py, trainModel, item loop) on the device, in place on Y, G
+    (float32 / float64 [num_items, d]) and w, c ([num_items], like Y); X ([num_users, d], like Y) is only read and
+    XtX = X^T X is float64 (als_gram).  item_csr: (rowptr int64, users int32, ratings like Y), rating_csr('item');
+    sppmi: (rowptr int64, cols int32, vals like Y), symmetric (sppmi_csr).  lam regularises Y, gamma G, alpha is the
+    confidence scale.  Contexts c < i are read after their own update, c > i before it, as in the sequential loop.
+    stamps (int32 [num_items], all sweep - 1) lets a caller reuse one stamp array across sweeps 1, 2, ...; without
+    it a zeroed array is used for sweep 1.  n_failed: optional int32 CUDA tensor counting systems that were not
+    positive definite (their rows left unchanged); when it is not given, the count is read back here and a failed
+    system raises QRecError."""
+    torch = _torch()
+    dt = Y.dtype
+    if dt not in (torch.float32, torch.float64):
+        raise QRecError('Y must be float32 or float64, got %s' % dt)
+    n_items, d = Y.shape
+    if G.shape != Y.shape or X.dim() != 2 or X.shape[1] != d:
+        raise QRecError('cofactor_item_sweep: G must have the shape of Y and X its width')
+    if w.shape != (n_items,) or c.shape != (n_items,):
+        raise QRecError('cofactor_item_sweep: w and c need one entry per item')
+    if tuple(XtX.shape) != (d, d):
+        raise QRecError('cofactor_item_sweep: XtX must be [%d, %d]' % (d, d))
+    irp, icol, ival = item_csr
+    srp, scol, sval = sppmi
+    if irp.shape[0] != n_items + 1 or srp.shape[0] != n_items + 1:
+        raise QRecError('cofactor_item_sweep: item and SPPMI rowptrs need %d entries' % (n_items + 1))
+    if icol.shape[0] != ival.shape[0] or scol.shape[0] != sval.shape[0]:
+        raise QRecError('cofactor_item_sweep: cols and vals differ in length')
+    if stamps is None:
+        stamps, sweep = torch.zeros(n_items, dtype=torch.int32, device=Y.device), 1
+    elif stamps.shape != (n_items,) or (n_items and not bool((stamps == sweep - 1).all())):
+        raise QRecError('cofactor_item_sweep: stamps must hold %d (sweep - 1) for every item' % (sweep - 1))
+    ticket = torch.zeros(1, dtype=torch.int64, device=Y.device)
+    own = n_failed is None
+    if own:
+        n_failed = torch.zeros(1, dtype=torch.int32, device=Y.device)
+    fn = lib.qrec_cofactor_item_sweep_f64 if dt == torch.float64 else lib.qrec_cofactor_item_sweep_f32
+    check(fn(_dev(Y, dt, 'Y'), _dev(G, dt, 'G'), _dev(w, dt, 'w'), _dev(c, dt, 'c'), _dev(X, dt, 'X'),
+             _dev(XtX, torch.float64, 'XtX'), d, n_items, _dev(irp, torch.int64, 'item rowptr'),
+             _dev(icol, torch.int32, 'item users'), _dev(ival, dt, 'item ratings'), _dev(srp, torch.int64, 'SPPMI rowptr'),
+             _dev(scol, torch.int32, 'SPPMI cols'), _dev(sval, dt, 'SPPMI vals'), float(lam), float(gamma),
+             float(alpha), _dev(stamps, torch.int32, 'stamps'), int(sweep), ticket.data_ptr(),
+             _dev(n_failed, torch.int32, 'n_failed'), _stream()), 'qrec_cofactor_item_sweep')
+    if own:
+        bad = int(n_failed.item())
+        if bad:
+            raise QRecError('cofactor_item_sweep: %d system(s) that are not positive definite left their rows '
+                            'unchanged' % bad)
+    return Y
 
 
 # =============================================================================================

@@ -157,6 +157,21 @@ def main():
                                         max_users_in_flight=k)
         torch.cuda.synchronize()
         print('sanitize_all: + K11, launched', E.launch_count(), 'kernels')
+        # K12 (CoFactor): both co-occurrence passes (and so the SPPMI), then the item sweep for both table types and
+        # both tile builds, over the SPPMI of the same interactions
+        pairs = np.unique(np.stack([i, u]), axis=1)                              # distinct (item, user), item-major
+        irp = torch.from_numpy(np.concatenate([[0], np.bincount(pairs[0], minlength=ni).cumsum()])).cuda()
+        icol = dev(pairs[1].astype(np.int32))
+        srp, scol, sval = E.sppmi_csr(irp, icol, nu, 5, 0)
+        for dd in (20, 128):
+            for dt in (torch.float64, torch.float32):
+                Y, G = torch.rand(ni, dd, device='cuda', dtype=dt), torch.rand(ni, dd, device='cuda', dtype=dt)
+                w, c = torch.rand(ni, device='cuda', dtype=dt), torch.rand(ni, device='cuda', dtype=dt)
+                Xs = torch.rand(nu, dd, device='cuda', dtype=dt)
+                E.cofactor_item_sweep(Y, G, w, c, Xs, E.als_gram(Xs), (irp, icol, torch.ones_like(icol, dtype=dt)),
+                                      (srp, scol, sval.to(dt)), 1.0, 1.0, 10.0)
+        torch.cuda.synchronize()
+        print('sanitize_all: + K12, launched', E.launch_count(), 'kernels', 'SPPMI nnz', scol.shape[0])
 
 
 if __name__ == '__main__':
