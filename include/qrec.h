@@ -740,6 +740,25 @@ int qrec_cofactor_item_sweep_f64(double* dev_Y, double* dev_G, double* dev_w, do
                                  int32_t* dev_stamps, int32_t sweep, unsigned long long* dev_ticket,
                                  int32_t* dev_n_failed, void* stream);
 
+/* =====================================================================================
+ * K13 -- ExpoMF (model/ranking/ExpoMF.py): implicit-feedback MF with an exposure posterior A per (user, item).  Every
+ * row's system weights every row of the other table by A, so there is no shared Gram.  Tables are float32.
+ * ===================================================================================== */
+/* One half-epoch over the rows row_order[0..n_rows) of X (a different table from Z[n_z][d]).  Row r's observed
+ * columns are cols[rowptr[r]..rowptr[r+1]) (rows of Z, any order).  With s = x_old.z and mu_k = mu[r] (mu_by_row != 0)
+ * or mu[k] (mu_by_row == 0, mu has n_z entries):
+ *   A_k = (p + 1e-8) / (p + 1e-8 + (1 - mu_k) / mu_k),  p = sqrt(lam_y/2/pi) exp(-lam_y s^2 / 2);  A_k = 1 if observed
+ *   X[r] = (sum_{k < n_z} A_k z_k z_k^T + lambda*I)^-1 sum_{observed k} z_k      (float64 system, float32 result)
+ * One CTA solves one row in place; every CTA reads only its own old row.  dev_mu_out (optional, float[n_rows of X],
+ * not dev_mu; mu then needs an entry per row of X): after the solve, mu_out[r] = (a + sum_k A_k - 1) / (a + b + n_z - 2)
+ * with A_k from the NEW x_r and mu[r] -- the exposure prior of the item half.  A row whose system is not positive
+ * definite is left unchanged and counted in dev_n_failed (optional, int32[1]).  max_ctas: 0 = fill the GPU, k > 0 = at
+ * most k CTAs; the result is bitwise the same for any grid.  d: 1..128. */
+int qrec_expomf_solve_rows_f32(float* dev_X, const float* dev_Z, int32_t d, int64_t n_z, int64_t n_rows,
+                               const int32_t* dev_row_order, const int64_t* dev_rowptr, const int32_t* dev_cols,
+                               const float* dev_mu, int32_t mu_by_row, float* dev_mu_out, double lambda, double lam_y,
+                               double a, double b, int32_t max_ctas, int32_t* dev_n_failed, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

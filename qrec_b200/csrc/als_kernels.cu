@@ -17,10 +17,18 @@
 //   co-factorisation (cofactor_step.cuh) and runs in item-id order, updating in place.
 //   * cofactor_item_sweep_kernel -- one CTA per item, on the same staging, tiles and Cholesky as the row solve; the
 //     in-order dataflow is kept with per-item stamps (see the kernel's comment).
+//
+//   ExpoMF (model/ranking/ExpoMF.py): every row's system weights EVERY row of the other table by an exposure
+//   posterior that depends on the row (expomf_step.cuh), so there is no shared Gram.
+//   * expomf_solve_rows_kernel -- one CTA solves one row completely: it streams the whole other table through shared
+//     memory, weights each staged row by its posterior, lifts the row's observed entries to 1 with a sparse correction
+//     pass, and solves on the same tiles and Cholesky.  Fused into the item half, it also sums the posteriors of the
+//     new row for the exposure prior.
 #include "common.h"
 #include "device.cuh"
 #include "als_step.cuh"
 #include "cofactor_step.cuh"
+#include "expomf_step.cuh"
 
 namespace {
 
@@ -526,6 +534,127 @@ cofactor_item_sweep_kernel(T* Y, T* G, T* wb, T* cb, const T* __restrict__ X, co
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// ExpoMF row solve
+// ------------------------------------------------------------------------------------------
+// Posteriors of the staged rows Zs[0..cnt) against x (shared, dp columns): one warp per staged row, the dot in float64
+// with the lanes along the row.  Each weight is expomf_exposure(s, mu_of(k)), or its lift 1 - A when kLift; it goes to
+// W[k] when W is given.  Returns the sum of the weights of the warp's rows on lane 0 (in k order).
+template <bool kLift, class MuOf>
+__device__ __forceinline__ double expomf_weights(const double* Zs, const double* x, double* W, int d, int dp, int cnt,
+                                                 double lam_y, MuOf mu_of) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double sum = 0.0;
+  for (int k = warp; k < cnt; k += kThreads / 32) {
+    double s = 0.0;
+    for (int c = lane; c < d; c += 32) s = fma(x[c], Zs[k * dp + c], s);
+    s = warp_sum(s);
+    const double A = expomf_exposure(s, mu_of(k), lam_y);
+    const double w = kLift ? expomf_lift(A) : A;
+    if (lane == 0) {
+      if (W != nullptr) W[k] = w;
+      sum += w;
+    }
+  }
+  return sum;
+}
+
+// One ExpoMF half-epoch (ExpoMF.py: recompute_factors / _solve, arithmetic in expomf_step.cuh).  For row r of X with
+// observed columns Y_r (CSR) against all n_z rows of Z:
+//   B = sum_k A_k z_k z_k^T + lambda*I,   A_k = posterior of (x_old.z_k, mu), 1 on Y_r;   x_r = B^-1 sum_{k in Y_r} z_k
+// mu is indexed by the row (mu_by_row) or by Z's row.  The dense pass weights every staged row of Z by its posterior;
+// the correction pass adds (1 - A) z z^T over Y_r, so the columns need not be sorted.  Every CTA reads only its own old
+// row, so X is written in place.  A system that is not positive definite leaves its row unchanged and is counted in
+// n_failed.  mu_out (item half): after the solve the CTA streams Z once more and writes
+//   mu_out[r] = prior(sum_k A_k)  with A_k from (x_new.z_k, mu[r]), 1 on Y_r   (ExpoMF.py: _update_expo)
+// -- never into mu, which other CTAs may still read.  Nothing depends on the grid, so X and mu_out are bitwise
+// reproducible.
+template <int NT>
+__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
+expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
+                         const int* __restrict__ order, const long long* __restrict__ rowptr,
+                         const int* __restrict__ cols, const float* __restrict__ mu, int mu_by_row,
+                         float* __restrict__ mu_out, double lambda, double lam_y, double a, double b, int* n_failed) {
+  extern __shared__ __align__(16) double smem[];
+  __shared__ double part[kThreads / 32];
+  const int dp = pad4(d), ld = dp + 1;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  double* A = smem;
+  double* Zs = A + a_words(d);
+  double* W = Zs + kStage * dp;
+  double* xo = W + kStage;
+  double* bv = xo + dp;
+  double* sd = bv + dp;
+  Tiles<NT> tl;
+  tl.setup(d);
+  for (long long q = blockIdx.x; q < n_order; q += gridDim.x) {
+    const int r = __ldg(order + q);
+    const long long beg = __ldg(rowptr + r), end = __ldg(rowptr + r + 1);
+    float* x = X + (size_t)r * d;
+    const double mu_r = mu_by_row || mu_out != nullptr ? (double)__ldg(mu + r) : 0.0;
+    tl.zero();
+    double bacc = 0.0;
+    __syncthreads();                                   // the previous row is done with the buffers
+    for (int c = t; c < dp; c += kThreads) xo[c] = c < d ? (double)x[c] : 0.0;
+    // every row of Z, weighted by its posterior
+    for (long long k0 = 0; k0 < n_z; k0 += kStage) {
+      const int cnt = (int)(n_z - k0 < kStage ? n_z - k0 : kStage);
+      __syncthreads();
+      stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return k0 + k; });
+      __syncthreads();
+      expomf_weights<false>(Zs, xo, W, d, dp, cnt, lam_y,
+                            [=](int k) { return mu_by_row ? mu_r : (double)__ldg(mu + k0 + k); });
+      __syncthreads();
+      tl.accumulate(Zs, W, dp, cnt);
+    }
+    // the observed entries: lifted to A = 1, and the right-hand side
+    for (long long k0 = beg; k0 < end; k0 += kStage) {
+      const int cnt = (int)(end - k0 < kStage ? end - k0 : kStage);
+      __syncthreads();
+      stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return __ldg(cols + k0 + k); });
+      __syncthreads();
+      expomf_weights<true>(Zs, xo, W, d, dp, cnt, lam_y,
+                           [=](int k) { return mu_by_row ? mu_r : (double)__ldg(mu + __ldg(cols + k0 + k)); });
+      __syncthreads();
+      tl.accumulate(Zs, W, dp, cnt);
+      if (t < d)
+        for (int k = 0; k < cnt; ++k) bacc += Zs[k * dp + t];
+    }
+    __syncthreads();
+    tl.reduce_into(A, d, ld);
+    for (int j = t; j < d; j += kThreads) A[j * ld + j] += lambda;     // ExpoMF.py: + lam * np.eye(f)
+    if (t < d) bv[t] = bacc;
+    __syncthreads();
+    if (!chol_solve<float>(A, d, ld, sd, bv, x) && t == 0 && n_failed != nullptr) atomicAdd(n_failed, 1);
+    if (mu_out == nullptr) continue;
+    // the exposure prior of this row with its new value (the old one if the solve failed)
+    __syncthreads();                                   // warp 0's store of x is visible to the CTA
+    for (int c = t; c < dp; c += kThreads) xo[c] = c < d ? (double)x[c] : 0.0;
+    double asum = 0.0;
+    for (long long k0 = 0; k0 < n_z; k0 += kStage) {
+      const int cnt = (int)(n_z - k0 < kStage ? n_z - k0 : kStage);
+      __syncthreads();
+      stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return k0 + k; });
+      __syncthreads();
+      asum += expomf_weights<false>(Zs, xo, nullptr, d, dp, cnt, lam_y, [=](int) { return mu_r; });
+    }
+    for (long long k0 = beg; k0 < end; k0 += kStage) {
+      const int cnt = (int)(end - k0 < kStage ? end - k0 : kStage);
+      __syncthreads();
+      stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return __ldg(cols + k0 + k); });
+      __syncthreads();
+      asum += expomf_weights<true>(Zs, xo, nullptr, d, dp, cnt, lam_y, [=](int) { return mu_r; });
+    }
+    if (lane == 0) part[warp] = asum;
+    __syncthreads();
+    if (t == 0) {
+      double s = 0.0;
+      for (int w = 0; w < kThreads / 32; ++w) s += part[w];
+      mu_out[r] = (float)expomf_prior(s, a, b, n_z);
+    }
+  }
+}
+
 // persistent grid: as many CTAs as fit on the GPU at `bytes` of dynamic shared memory, at most `work`
 template <class K>
 int persistent_grid(K kernel, size_t bytes, long long work, int* grid) {
@@ -625,6 +754,35 @@ int launch_cofactor(T* Y, T* G, T* w, T* c, const T* X, const double* XtX, int d
   return QREC_OK;
 }
 
+int launch_expomf(float* X, const float* Z, int d, long long n_z, long long n_order, const int* order,
+                  const long long* rowptr, const int* cols, const float* mu, int mu_by_row, float* mu_out,
+                  double lambda, double lam_y, double a, double b, int max_ctas, int* n_failed, cudaStream_t st) {
+  QREC_REQUIRE(d >= 1 && d <= kMaxD, "expomf_solve_rows: d=%d unsupported (1..%d)", d, kMaxD);
+  QREC_REQUIRE(n_order >= 0 && n_z >= 0, "expomf_solve_rows: n_rows=%lld n_z=%lld", n_order, n_z);
+  QREC_REQUIRE(max_ctas >= 0, "expomf_solve_rows: max_ctas=%d < 0", max_ctas);
+  if (n_order == 0) return QREC_OK;
+  QREC_REQUIRE(X && Z && order && rowptr && mu, "expomf_solve_rows: null pointer");
+  QREC_REQUIRE((const void*)X != (const void*)Z, "expomf_solve_rows: X and Z must be different tables");
+  QREC_REQUIRE((const void*)mu_out != (const void*)mu, "expomf_solve_rows: mu_out must not be mu");
+  const size_t bytes = smem_bytes(d);
+  int grid = 0;
+  if (tiles_of(d) <= kThreads) {
+    const int rc = persistent_grid(expomf_solve_rows_kernel<1>, bytes, n_order, &grid);
+    if (rc) return rc;
+    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+    expomf_solve_rows_kernel<1><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, mu,
+                                                                mu_by_row, mu_out, lambda, lam_y, a, b, n_failed);
+  } else {
+    const int rc = persistent_grid(expomf_solve_rows_kernel<3>, bytes, n_order, &grid);
+    if (rc) return rc;
+    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+    expomf_solve_rows_kernel<3><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, mu,
+                                                                mu_by_row, mu_out, lambda, lam_y, a, b, n_failed);
+  }
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -676,6 +834,14 @@ int qrec_cofactor_item_sweep_f64(double* Y, double* G, double* w, double* c, con
   return launch_cofactor<double>(Y, G, w, c, X, XtX, d, n_items, (const long long*)item_rowptr, item_users, item_vals,
                                  (const long long*)sppmi_rowptr, sppmi_cols, sppmi_vals, lambda, gamma, alpha, stamps,
                                  sweep, ticket, n_failed, (cudaStream_t)stream);
+}
+
+int qrec_expomf_solve_rows_f32(float* X, const float* Z, int32_t d, int64_t n_z, int64_t n_rows,
+                               const int32_t* row_order, const int64_t* rowptr, const int32_t* cols, const float* mu,
+                               int32_t mu_by_row, float* mu_out, double lambda, double lam_y, double a, double b,
+                               int32_t max_ctas, int32_t* n_failed, void* stream) {
+  return launch_expomf(X, Z, d, n_z, n_rows, row_order, (const long long*)rowptr, cols, mu, mu_by_row, mu_out, lambda,
+                       lam_y, a, b, max_ctas, n_failed, (cudaStream_t)stream);
 }
 
 }  // extern "C"

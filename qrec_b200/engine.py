@@ -1153,6 +1153,71 @@ def cofactor_item_sweep(Y, G, w, c, X, XtX, item_csr, sppmi, lam, gamma, alpha, 
 
 
 # =============================================================================================
+# K13: ExpoMF -- exposure posterior and weighted normal equations, fused per row
+# =============================================================================================
+def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, mu_out=None, a=1.0, b=99.0,
+                      n_failed=None, max_ctas=0):
+    """One ExpoMF half-epoch (ExpoMF.py: recompute_factors) in place on the rows `row_order` of X (float32 [n, d])
+    against every row of Z (float32 [m, d]): with s = x_old.z and the exposure posterior
+    A = (p + 1e-8) / (p + 1e-8 + (1 - mu) / mu), p = sqrt(lam_y/2/pi) exp(-lam_y s^2 / 2), set to 1 on row r's
+    observed columns (rowptr int64 [n + 1], cols int32 < m),
+        X[r] = (sum_k A_k z_k z_k^T + lam*I)^-1 sum_{observed k} z_k.
+    mu (float32) is indexed by X's row when mu_by_row ([n]), else by Z's row ([m]).  mu_out (float32 [n], item half):
+    also writes mu_out[r] = (a + sum_k A_k - 1) / (a + b + m - 2) with A from the new X[r] and mu[r] (mu then needs
+    n entries; mu_out must not be mu).  max_ctas > 0 caps the grid (the result does not depend on it).  n_failed:
+    optional int32 CUDA tensor counting rows whose system was not positive definite (left unchanged); when it is not
+    given, the count is read back here and a failed row raises QRecError."""
+    torch = _torch()
+    f32 = torch.float32
+    for t, name in ((X, 'X'), (Z, 'Z'), (mu, 'mu')):
+        if t.dtype != f32:
+            raise QRecError('expomf_half_epoch: %s must be float32, got %s' % (name, t.dtype))
+    if X.dim() != 2 or Z.dim() != 2 or Z.shape[1] != X.shape[1]:
+        raise QRecError('expomf_half_epoch: X and Z must be 2-D tables of one width')
+    n, d = X.shape
+    m = Z.shape[0]
+    if not 1 <= d <= 128:
+        raise QRecError('expomf_half_epoch: d=%d unsupported (1..128)' % d)
+    if X.data_ptr() == Z.data_ptr():
+        raise QRecError('expomf_half_epoch: X and Z must be different tables')
+    want = n if mu_by_row else m
+    if mu.shape != (want,):
+        raise QRecError('expomf_half_epoch: mu indexed by %s needs %d entries, got %s'
+                        % ('row' if mu_by_row else 'column', want, tuple(mu.shape)))
+    if mu_out is not None:
+        if mu_out.dtype != f32 or mu_out.shape != (n,) or mu.shape != (n,):
+            raise QRecError('expomf_half_epoch: mu_out and mu need one float32 entry per row (%d)' % n)
+        if mu_out.data_ptr() == mu.data_ptr():
+            raise QRecError('expomf_half_epoch: mu_out must be a buffer of its own, not mu')
+    if rowptr.shape != (n + 1,):
+        raise QRecError('expomf_half_epoch: rowptr needs %d entries' % (n + 1))
+    if row_order.dim() != 1 or row_order.shape[0] > n:
+        raise QRecError('expomf_half_epoch: row_order must be a list of at most %d rows' % n)
+    if row_order.numel() and (int(row_order.min()) < 0 or int(row_order.max()) >= n):
+        raise QRecError('expomf_half_epoch: a row of row_order is outside [0, %d)' % n)
+    nnz = cols.shape[0]
+    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
+        raise QRecError('expomf_half_epoch: rowptr must rise from 0 to len(cols) = %d' % nnz)
+    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= m):
+        raise QRecError('expomf_half_epoch: a column is outside [0, %d)' % m)
+    own = n_failed is None
+    if own:
+        n_failed = torch.zeros(1, dtype=torch.int32, device=X.device)
+    check(lib.qrec_expomf_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
+                                         _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
+                                         _dev(cols, torch.int32, 'cols'), _dev(mu, f32, 'mu'), int(bool(mu_by_row)),
+                                         _opt(mu_out, f32, 'mu_out'), float(lam), float(lam_y), float(a), float(b),
+                                         int(max_ctas), _dev(n_failed, torch.int32, 'n_failed'), _stream()),
+          'qrec_expomf_solve_rows_f32')
+    if own:
+        bad = int(n_failed.item())
+        if bad:
+            raise QRecError('expomf_half_epoch: %d row(s) with normal equations that are not positive definite were '
+                            'left unchanged' % bad)
+    return X
+
+
+# =============================================================================================
 # K11: SVD++ -- in-order parity epoch and user-major closed-form fast epoch
 # =============================================================================================
 def _svdpp_tables(P, Q, Y, Bu, Bi, dt):

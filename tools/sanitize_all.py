@@ -172,6 +172,16 @@ def main():
                                       (srp, scol, sval.to(dt)), 1.0, 1.0, 10.0)
         torch.cuda.synchronize()
         print('sanitize_all: + K12, launched', E.launch_count(), 'kernels', 'SPPMI nnz', scol.shape[0])
+        # K13 (ExpoMF): the user half (mu by column) and the item half with the prior (mu by row), for both tile
+        # builds, over the same interactions (users with no entries included)
+        for dd in (20, 128):
+            th, be = torch.rand(nu, dd, device='cuda') * 0.1, torch.rand(ni, dd, device='cuda') * 0.1
+            mu, mu_out = torch.full((ni,), 0.01, device='cuda'), torch.empty(ni, device='cuda')
+            E.expomf_half_epoch(th, be, rowptr, cols, mu, False, 1e-5, 1.0, order)
+            E.expomf_half_epoch(be, th, irp, icol, mu, True, 1e-5, 1.0, dev(E.als_row_order(irp.cpu().numpy())),
+                                mu_out=mu_out)
+        torch.cuda.synchronize()
+        print('sanitize_all: + K13, launched', E.launch_count(), 'kernels')
 
 
 if __name__ == '__main__':
