@@ -759,6 +759,27 @@ int qrec_expomf_solve_rows_f32(float* dev_X, const float* dev_Z, int32_t d, int6
                                const float* dev_mu, int32_t mu_by_row, float* dev_mu_out, double lambda, double lam_y,
                                double a, double b, int32_t max_ctas, int32_t* dev_n_failed, void* stream);
 
+/* =====================================================================================
+ * K14 -- SERec (model/ranking/SERec.py): ExpoMF with a social exposure prior per (user, item).  The reference's dense
+ * U x I prior is mu(u, i) = (a + A_i + (s-1)*deg_u*A_i - 1) / (a + b + (s-1)*deg_u*A_i + U - 2), with A_i the item's
+ * summed posterior and deg_u the user's number of followees, so the state is A (float64 [I]) and deg (int32 [U]).
+ * ===================================================================================== */
+/* One half-epoch over the rows row_order[0..n_rows) of X (a different table from Z[n_z][d]), as
+ * qrec_expomf_solve_rows_f32 with the prior of the pair (row r, column k) taken as:
+ *   dev_asum == NULL:  mu0 for every pair (the first epoch);
+ *   row_is_user != 0:  mu(r, k) = prior(A = asum[k], deg = deg[r])   (asum has n_z entries, deg one per row of X)
+ *   row_is_user == 0:  mu(k, r) = prior(A = asum[r], deg = deg[k])   (asum one per row of X, deg n_z entries)
+ * with the operand order above, s - 1 in double and U = n_users; deg_u * A_i is one float64 product.
+ * dev_asum_out (optional, double[n_rows of X], not dev_asum; asum then needs an entry per row of X and deg n_z
+ * entries): after the solve, asum_out[r] = sum_k A_k with A_k from the NEW x_r and prior(asum[r], deg[k]) (or mu0),
+ * 1 on the observed entries -- the summed posteriors of the item half, from which the next epoch's prior follows.
+ * n_failed, max_ctas and d as for qrec_expomf_solve_rows_f32; bitwise the same for any grid. */
+int qrec_serec_solve_rows_f32(float* dev_X, const float* dev_Z, int32_t d, int64_t n_z, int64_t n_rows,
+                              const int32_t* dev_row_order, const int64_t* dev_rowptr, const int32_t* dev_cols,
+                              const double* dev_asum, float mu0, const int32_t* dev_deg, int32_t row_is_user,
+                              double* dev_asum_out, double lambda, double lam_y, double a, double b, double s,
+                              int64_t n_users, int32_t max_ctas, int32_t* dev_n_failed, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

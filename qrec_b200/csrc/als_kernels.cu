@@ -24,11 +24,18 @@
 //     memory, weights each staged row by its posterior, lifts the row's observed entries to 1 with a sparse correction
 //     pass, and solves on the same tiles and Cholesky.  Fused into the item half, it also sums the posteriors of the
 //     new row for the exposure prior.
+//
+//   SERec (model/ranking/SERec.py): ExpoMF with a prior per (user, item) pair that grows with the user's number of
+//   followees (serec_step.cuh).  The reference's dense U x I prior has a closed form in one float64 sum per item and
+//   one degree per user, evaluated per pair inside the solve.
+//   * serec_solve_rows_kernel -- the same row solve as ExpoMF's (exposure_solve_rows, generic over the prior policy);
+//     fused into the item half, it writes each item's summed posterior for the next epoch's prior.
 #include "common.h"
 #include "device.cuh"
 #include "als_step.cuh"
 #include "cofactor_step.cuh"
 #include "expomf_step.cuh"
+#include "serec_step.cuh"
 
 namespace {
 
@@ -559,22 +566,86 @@ __device__ __forceinline__ double expomf_weights(const double* Zs, const double*
   return sum;
 }
 
-// One ExpoMF half-epoch (ExpoMF.py: recompute_factors / _solve, arithmetic in expomf_step.cuh).  For row r of X with
-// observed columns Y_r (CSR) against all n_z rows of Z:
-//   B = sum_k A_k z_k z_k^T + lambda*I,   A_k = posterior of (x_old.z_k, mu), 1 on Y_r;   x_r = B^-1 sum_{k in Y_r} z_k
-// mu is indexed by the row (mu_by_row) or by Z's row.  The dense pass weights every staged row of Z by its posterior;
-// the correction pass adds (1 - A) z z^T over Y_r, so the columns need not be sorted.  Every CTA reads only its own old
+// Prior policies of exposure_solve_rows (below).  A policy says what prior each (row r, column k) pair of the solve
+// uses, what prior the fused pass after the solve uses, and what that pass writes.  row(r) loads the row's own
+// state once; solve(p, k) and out(p, k) take the column as a functor, so that a policy that does not need it does not
+// load it.
+//
+// ExpoMF: one float32 prior per item, indexed by the row (by_row) or by the column.  The fused pass uses mu[r] and
+// writes the item's new prior to mu_out.
+struct ExpoPrior {
+  const float* __restrict__ mu;
+  int by_row;
+  float* __restrict__ mu_out;
+  double a, b;
+  long long n_z;
+  __device__ __forceinline__ bool has_out() const { return mu_out != nullptr; }
+  __device__ __forceinline__ double row(int r) const { return by_row || mu_out != nullptr ? (double)__ldg(mu + r) : 0.0; }
+  template <class Col>
+  __device__ __forceinline__ double solve(double mu_r, Col col) const { return by_row ? mu_r : (double)__ldg(mu + col()); }
+  template <class Col>
+  __device__ __forceinline__ double out(double mu_r, Col) const { return mu_r; }
+  __device__ __forceinline__ void write(int r, double asum) const { mu_out[r] = (float)expomf_prior(asum, a, b, n_z); }
+};
+
+// SERec: the prior of the pair (user u, item i) is serec_prior(A[i], deg[u]) (serec_step.cuh), or the uniform mu0
+// when A is null (the first epoch).  row_is_user says which of r and k is the user: the user half has user rows, the
+// item half item rows -- except when there are as many users as items, where the reference's item half takes the user
+// branch (SERec.py, _solve_batch: mu.shape[1] == X.shape[0]) and so reads mu[i, u].  The fused pass after the solve
+// always reads mu[u, i] with the item as the row (SERec.py: _update_expo) and writes the item's summed posterior
+// A itself to asum_out; the next epoch evaluates the prior from it.  The social term deg_u * A_i is one float64
+// product, where the reference's T.dot adds A_i to itself deg_u times: the two differ by a few ulps once deg_u >= 7
+// (about 1e-15 of the prior), far below the float32 rows the prior feeds.
+struct SocialPrior {
+  const double* __restrict__ A;
+  double mu0;
+  const int* __restrict__ deg;
+  int row_is_user;
+  double* __restrict__ asum_out;
+  double a, b, s, n_users;
+  struct Row {
+    double A;                                // A[r]: the row is the item of its pairs
+    int deg;                                 // deg[r]: the row is the user of its pairs
+  };
+  __device__ __forceinline__ bool has_out() const { return asum_out != nullptr; }
+  __device__ __forceinline__ Row row(int r) const {
+    Row p{0.0, 0};
+    if (A != nullptr) {
+      if (row_is_user) p.deg = __ldg(deg + r);
+      if (!row_is_user || asum_out != nullptr) p.A = __ldg(A + r);
+    }
+    return p;
+  }
+  template <class Col>
+  __device__ __forceinline__ double solve(const Row& p, Col col) const {
+    if (A == nullptr) return mu0;
+    const int k = col();
+    return row_is_user ? serec_prior(__ldg(A + k), p.deg, a, b, s, n_users)
+                       : serec_prior(p.A, __ldg(deg + k), a, b, s, n_users);
+  }
+  template <class Col>
+  __device__ __forceinline__ double out(const Row& p, Col col) const {
+    return A == nullptr ? mu0 : serec_prior(p.A, __ldg(deg + col()), a, b, s, n_users);
+  }
+  __device__ __forceinline__ void write(int r, double asum) const { asum_out[r] = asum; }
+};
+
+// One exposure-weighted half-epoch (ExpoMF.py / SERec.py: recompute_factors / _solve, arithmetic in expomf_step.cuh
+// and serec_step.cuh).  For row r of X with observed columns Y_r (CSR) against all n_z rows of Z:
+//   B = sum_k A_k z_k z_k^T + lambda*I,   A_k = posterior of (x_old.z_k, mu_rk), 1 on Y_r;   x_r = B^-1 sum_{k in Y_r} z_k
+// with the prior mu_rk from the policy P.  The dense pass weights every staged row of Z by its posterior; the
+// correction pass adds (1 - A) z z^T over Y_r, so the columns need not be sorted.  Every CTA reads only its own old
 // row, so X is written in place.  A system that is not positive definite leaves its row unchanged and is counted in
-// n_failed.  mu_out (item half): after the solve the CTA streams Z once more and writes
-//   mu_out[r] = prior(sum_k A_k)  with A_k from (x_new.z_k, mu[r]), 1 on Y_r   (ExpoMF.py: _update_expo)
-// -- never into mu, which other CTAs may still read.  Nothing depends on the grid, so X and mu_out are bitwise
-// reproducible.
-template <int NT>
-__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
-expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
-                         const int* __restrict__ order, const long long* __restrict__ rowptr,
-                         const int* __restrict__ cols, const float* __restrict__ mu, int mu_by_row,
-                         float* __restrict__ mu_out, double lambda, double lam_y, double a, double b, int* n_failed) {
+// n_failed.  Fused pass (item half, P::has_out): after the solve the CTA streams Z once more and sums
+//   sum_k A_k  with A_k from (x_new.z_k, the policy's out prior), 1 on Y_r   (_update_expo)
+// which P::write stores -- never into the prior being read, which other CTAs may still read.  Nothing depends on the
+// grid, so X and the fused output are bitwise reproducible.
+template <int NT, class P>
+__device__ __forceinline__ void exposure_solve_rows(float* X, const float* __restrict__ Z, int d, long long n_z,
+                                                    long long n_order, const int* __restrict__ order,
+                                                    const long long* __restrict__ rowptr,
+                                                    const int* __restrict__ cols, const P& prior, double lambda,
+                                                    double lam_y, int* n_failed) {
   extern __shared__ __align__(16) double smem[];
   __shared__ double part[kThreads / 32];
   const int dp = pad4(d), ld = dp + 1;
@@ -591,7 +662,7 @@ expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long
     const int r = __ldg(order + q);
     const long long beg = __ldg(rowptr + r), end = __ldg(rowptr + r + 1);
     float* x = X + (size_t)r * d;
-    const double mu_r = mu_by_row || mu_out != nullptr ? (double)__ldg(mu + r) : 0.0;
+    const auto pr = prior.row(r);
     tl.zero();
     double bacc = 0.0;
     __syncthreads();                                   // the previous row is done with the buffers
@@ -603,7 +674,7 @@ expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long
       stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return k0 + k; });
       __syncthreads();
       expomf_weights<false>(Zs, xo, W, d, dp, cnt, lam_y,
-                            [=](int k) { return mu_by_row ? mu_r : (double)__ldg(mu + k0 + k); });
+                            [=](int k) { return prior.solve(pr, [=] { return k0 + k; }); });
       __syncthreads();
       tl.accumulate(Zs, W, dp, cnt);
     }
@@ -614,7 +685,7 @@ expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long
       stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return __ldg(cols + k0 + k); });
       __syncthreads();
       expomf_weights<true>(Zs, xo, W, d, dp, cnt, lam_y,
-                           [=](int k) { return mu_by_row ? mu_r : (double)__ldg(mu + __ldg(cols + k0 + k)); });
+                           [=](int k) { return prior.solve(pr, [=] { return __ldg(cols + k0 + k); }); });
       __syncthreads();
       tl.accumulate(Zs, W, dp, cnt);
       if (t < d)
@@ -626,8 +697,8 @@ expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long
     if (t < d) bv[t] = bacc;
     __syncthreads();
     if (!chol_solve<float>(A, d, ld, sd, bv, x) && t == 0 && n_failed != nullptr) atomicAdd(n_failed, 1);
-    if (mu_out == nullptr) continue;
-    // the exposure prior of this row with its new value (the old one if the solve failed)
+    if (!prior.has_out()) continue;
+    // the summed posteriors of this row with its new value (the old one if the solve failed)
     __syncthreads();                                   // warp 0's store of x is visible to the CTA
     for (int c = t; c < dp; c += kThreads) xo[c] = c < d ? (double)x[c] : 0.0;
     double asum = 0.0;
@@ -636,23 +707,45 @@ expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long
       __syncthreads();
       stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return k0 + k; });
       __syncthreads();
-      asum += expomf_weights<false>(Zs, xo, nullptr, d, dp, cnt, lam_y, [=](int) { return mu_r; });
+      asum += expomf_weights<false>(Zs, xo, nullptr, d, dp, cnt, lam_y,
+                                    [=](int k) { return prior.out(pr, [=] { return k0 + k; }); });
     }
     for (long long k0 = beg; k0 < end; k0 += kStage) {
       const int cnt = (int)(end - k0 < kStage ? end - k0 : kStage);
       __syncthreads();
       stage_rows<float>(Zs, Z, d, dp, cnt, [=](int k) { return __ldg(cols + k0 + k); });
       __syncthreads();
-      asum += expomf_weights<true>(Zs, xo, nullptr, d, dp, cnt, lam_y, [=](int) { return mu_r; });
+      asum += expomf_weights<true>(Zs, xo, nullptr, d, dp, cnt, lam_y,
+                                   [=](int k) { return prior.out(pr, [=] { return __ldg(cols + k0 + k); }); });
     }
     if (lane == 0) part[warp] = asum;
     __syncthreads();
     if (t == 0) {
       double s = 0.0;
       for (int w = 0; w < kThreads / 32; ++w) s += part[w];
-      mu_out[r] = (float)expomf_prior(s, a, b, n_z);
+      prior.write(r, s);
     }
   }
+}
+
+// The two policies keep separate entry points.  ExpoMF's keeps its flat parameter list, so its kernels compile to the
+// code they had before the policy was factored out; SERec's takes its policy as one parameter.
+template <int NT>
+__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
+expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
+                         const int* __restrict__ order, const long long* __restrict__ rowptr,
+                         const int* __restrict__ cols, const float* __restrict__ mu, int mu_by_row,
+                         float* __restrict__ mu_out, double lambda, double lam_y, double a, double b, int* n_failed) {
+  exposure_solve_rows<NT>(X, Z, d, n_z, n_order, order, rowptr, cols, ExpoPrior{mu, mu_by_row, mu_out, a, b, n_z},
+                          lambda, lam_y, n_failed);
+}
+
+template <int NT>
+__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
+serec_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
+                        const int* __restrict__ order, const long long* __restrict__ rowptr,
+                        const int* __restrict__ cols, SocialPrior prior, double lambda, double lam_y, int* n_failed) {
+  exposure_solve_rows<NT>(X, Z, d, n_z, n_order, order, rowptr, cols, prior, lambda, lam_y, n_failed);
 }
 
 // persistent grid: as many CTAs as fit on the GPU at `bytes` of dynamic shared memory, at most `work`
@@ -783,6 +876,38 @@ int launch_expomf(float* X, const float* Z, int d, long long n_z, long long n_or
   return QREC_OK;
 }
 
+int launch_serec(float* X, const float* Z, int d, long long n_z, long long n_order, const int* order,
+                 const long long* rowptr, const int* cols, const double* asum, float mu0, const int* deg,
+                 int row_is_user, double* asum_out, double lambda, double lam_y, double a, double b, double s,
+                 long long n_users, int max_ctas, int* n_failed, cudaStream_t st) {
+  QREC_REQUIRE(d >= 1 && d <= kMaxD, "serec_solve_rows: d=%d unsupported (1..%d)", d, kMaxD);
+  QREC_REQUIRE(n_order >= 0 && n_z >= 0, "serec_solve_rows: n_rows=%lld n_z=%lld", n_order, n_z);
+  QREC_REQUIRE(max_ctas >= 0, "serec_solve_rows: max_ctas=%d < 0", max_ctas);
+  if (n_order == 0) return QREC_OK;
+  QREC_REQUIRE(X && Z && order && rowptr && deg, "serec_solve_rows: null pointer");
+  QREC_REQUIRE((const void*)X != (const void*)Z, "serec_solve_rows: X and Z must be different tables");
+  QREC_REQUIRE(asum_out == nullptr || (const void*)asum_out != (const void*)asum,
+               "serec_solve_rows: asum_out must not be asum");
+  const SocialPrior prior{asum, (double)mu0, deg, row_is_user, asum_out, a, b, s, (double)n_users};
+  const size_t bytes = smem_bytes(d);
+  int grid = 0;
+  if (tiles_of(d) <= kThreads) {
+    const int rc = persistent_grid(serec_solve_rows_kernel<1>, bytes, n_order, &grid);
+    if (rc) return rc;
+    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+    serec_solve_rows_kernel<1><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, prior,
+                                                               lambda, lam_y, n_failed);
+  } else {
+    const int rc = persistent_grid(serec_solve_rows_kernel<3>, bytes, n_order, &grid);
+    if (rc) return rc;
+    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+    serec_solve_rows_kernel<3><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, prior,
+                                                               lambda, lam_y, n_failed);
+  }
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -842,6 +967,15 @@ int qrec_expomf_solve_rows_f32(float* X, const float* Z, int32_t d, int64_t n_z,
                                int32_t max_ctas, int32_t* n_failed, void* stream) {
   return launch_expomf(X, Z, d, n_z, n_rows, row_order, (const long long*)rowptr, cols, mu, mu_by_row, mu_out, lambda,
                        lam_y, a, b, max_ctas, n_failed, (cudaStream_t)stream);
+}
+
+int qrec_serec_solve_rows_f32(float* X, const float* Z, int32_t d, int64_t n_z, int64_t n_rows,
+                              const int32_t* row_order, const int64_t* rowptr, const int32_t* cols,
+                              const double* asum, float mu0, const int32_t* deg, int32_t row_is_user,
+                              double* asum_out, double lambda, double lam_y, double a, double b, double s,
+                              int64_t n_users, int32_t max_ctas, int32_t* n_failed, void* stream) {
+  return launch_serec(X, Z, d, n_z, n_rows, row_order, (const long long*)rowptr, cols, asum, mu0, deg, row_is_user,
+                      asum_out, lambda, lam_y, a, b, s, n_users, max_ctas, n_failed, (cudaStream_t)stream);
 }
 
 }  // extern "C"

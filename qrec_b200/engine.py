@@ -1218,6 +1218,78 @@ def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, 
 
 
 # =============================================================================================
+# K14: SERec -- ExpoMF's fused row solve with the social exposure prior evaluated per pair
+# =============================================================================================
+def serec_half_epoch(X, Z, rowptr, cols, asum, deg, row_is_user, lam, lam_y, row_order, asum_out=None, mu0=0.01,
+                     a=1.0, b=99.0, s=2.2, n_failed=None, max_ctas=0):
+    """One SERec half-epoch (SERec.py: recompute_factors) in place on the rows `row_order` of X (float32 [n, d])
+    against every row of Z (float32 [m, d]), as expomf_half_epoch with the prior of each (user, item) pair
+        mu(u, i) = (a + A_i + (s-1)*deg_u*A_i - 1) / (a + b + (s-1)*deg_u*A_i + U - 2)
+    from asum (float64, A_i: each item's summed posterior) and deg (int32, each user's number of followees), or the
+    uniform mu0 for every pair when asum is None.  row_is_user: X's rows are the users (asum [m], deg [n], U = n) or
+    the items (asum [n], deg [m], U = m); the reference's item half takes the user branch when U == I.  asum_out
+    (float64 [n], item half, a buffer of its own): also writes asum_out[r] = sum_k A_k with A from the new X[r] and
+    mu(k, r), 1 on row r's observed columns -- asum then needs n entries and deg m.  max_ctas > 0 caps the grid (the
+    result does not depend on it).  n_failed: optional int32 CUDA tensor counting rows whose system was not positive
+    definite (left unchanged); when it is not given, the count is read back here and a failed row raises QRecError."""
+    torch = _torch()
+    f32, f64, i32 = torch.float32, torch.float64, torch.int32
+    for t, name in ((X, 'X'), (Z, 'Z')):
+        if t.dtype != f32:
+            raise QRecError('serec_half_epoch: %s must be float32, got %s' % (name, t.dtype))
+    if X.dim() != 2 or Z.dim() != 2 or Z.shape[1] != X.shape[1]:
+        raise QRecError('serec_half_epoch: X and Z must be 2-D tables of one width')
+    n, d = X.shape
+    m = Z.shape[0]
+    if not 1 <= d <= 128:
+        raise QRecError('serec_half_epoch: d=%d unsupported (1..128)' % d)
+    if X.data_ptr() == Z.data_ptr():
+        raise QRecError('serec_half_epoch: X and Z must be different tables')
+    n_users, n_items = (n, m) if row_is_user else (m, n)
+    if asum is not None and (asum.dtype != f64 or asum.shape != (n_items,)):
+        raise QRecError('serec_half_epoch: asum needs one float64 entry per item (%d), got %s %s'
+                        % (n_items, asum.dtype, tuple(asum.shape)))
+    if deg.dtype != i32 or deg.shape != (n_users,):
+        raise QRecError('serec_half_epoch: deg needs one int32 entry per user (%d), got %s %s'
+                        % (n_users, deg.dtype, tuple(deg.shape)))
+    if n_users and int(deg.min()) < 0:
+        raise QRecError('serec_half_epoch: deg must not be negative')
+    if asum_out is not None:
+        if asum_out.dtype != f64 or asum_out.shape != (n,) or n != n_items:
+            raise QRecError('serec_half_epoch: asum_out needs one float64 entry per row (%d), and the rows must be '
+                            'the items' % n)
+        if asum is not None and asum_out.data_ptr() == asum.data_ptr():
+            raise QRecError('serec_half_epoch: asum_out must be a buffer of its own, not asum')
+    if rowptr.shape != (n + 1,):
+        raise QRecError('serec_half_epoch: rowptr needs %d entries' % (n + 1))
+    if row_order.dim() != 1 or row_order.shape[0] > n:
+        raise QRecError('serec_half_epoch: row_order must be a list of at most %d rows' % n)
+    if row_order.numel() and (int(row_order.min()) < 0 or int(row_order.max()) >= n):
+        raise QRecError('serec_half_epoch: a row of row_order is outside [0, %d)' % n)
+    nnz = cols.shape[0]
+    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
+        raise QRecError('serec_half_epoch: rowptr must rise from 0 to len(cols) = %d' % nnz)
+    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= m):
+        raise QRecError('serec_half_epoch: a column is outside [0, %d)' % m)
+    own = n_failed is None
+    if own:
+        n_failed = torch.zeros(1, dtype=i32, device=X.device)
+    check(lib.qrec_serec_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
+                                        _dev(row_order, i32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
+                                        _dev(cols, i32, 'cols'), _opt(asum, f64, 'asum'), float(mu0),
+                                        _dev(deg, i32, 'deg'), int(bool(row_is_user)), _opt(asum_out, f64, 'asum_out'),
+                                        float(lam), float(lam_y), float(a), float(b), float(s), n_users,
+                                        int(max_ctas), _dev(n_failed, i32, 'n_failed'), _stream()),
+          'qrec_serec_solve_rows_f32')
+    if own:
+        bad = int(n_failed.item())
+        if bad:
+            raise QRecError('serec_half_epoch: %d row(s) with normal equations that are not positive definite were '
+                            'left unchanged' % bad)
+    return X
+
+
+# =============================================================================================
 # K11: SVD++ -- in-order parity epoch and user-major closed-form fast epoch
 # =============================================================================================
 def _svdpp_tables(P, Q, Y, Bu, Bi, dt):

@@ -182,6 +182,28 @@ def main():
                                 mu_out=mu_out)
         torch.cuda.synchronize()
         print('sanitize_all: + K13, launched', E.launch_count(), 'kernels')
+        # K14 (SERec): both halves with the uniform first-epoch prior and with the social prior from A and deg (users
+        # of degree 0 included), the item half with the fused sums, for both tile builds; then the square case, whose
+        # item half reads the prior with its rows as users, over the entries of the first nu items
+        deg = torch.randint(0, 40, (nu,), dtype=torch.int32, device='cuda') * (torch.rand(nu, device='cuda') < 0.5)
+        iord = dev(E.als_row_order(irp.cpu().numpy()))
+        for dd in (20, 128):
+            th, be = torch.rand(nu, dd, device='cuda') * 0.1, torch.rand(ni, dd, device='cuda') * 0.1
+            A, A_out = None, torch.empty(ni, dtype=torch.float64, device='cuda')
+            for _ in range(2):
+                E.serec_half_epoch(th, be, rowptr, cols, A, deg, True, 1e-3, 0.01, order)
+                E.serec_half_epoch(be, th, irp, icol, A, deg, False, 1e-3, 0.01, iord, asum_out=A_out)
+                A, A_out = A_out, torch.empty_like(A_out)
+        rp_h, col_h = rowptr.cpu().numpy(), cols.cpu().numpy()
+        keep = col_h < nu
+        sq_rp = np.concatenate([[0], np.cumsum(np.bincount(np.repeat(np.arange(nu), np.diff(rp_h))[keep], minlength=nu))])
+        sq_rp, sq_col = dev(sq_rp.astype(np.int64)), dev(col_h[keep].astype(np.int32))
+        sq = torch.rand(nu, 20, device='cuda') * 0.1
+        A_sq = torch.rand(nu, dtype=torch.float64, device='cuda') * 10
+        E.serec_half_epoch(sq, torch.rand(nu, 20, device='cuda') * 0.1, sq_rp, sq_col, A_sq, deg, True, 1e-3, 0.01,
+                           dev(E.als_row_order(sq_rp.cpu().numpy())), asum_out=torch.empty_like(A_sq))
+        torch.cuda.synchronize()
+        print('sanitize_all: + K14, launched', E.launch_count(), 'kernels')
 
 
 if __name__ == '__main__':

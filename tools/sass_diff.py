@@ -33,7 +33,7 @@ def sass(pkg):
             cur = m.group(1)
             kernels[cur] = []
         elif cur is not None and line.strip().startswith('/*'):
-            kernels[cur].append(line.strip())
+            kernels[cur].append(' '.join(line.split()))     # cuobjdump pads to the widest line of the ELF
     names = demangle(kernels)
     return {names[k]: v for k, v in kernels.items()}
 
