@@ -20,16 +20,18 @@
 //
 //   ExpoMF (model/ranking/ExpoMF.py): every row's system weights EVERY row of the other table by an exposure
 //   posterior that depends on the row (expomf_step.cuh), so there is no shared Gram.
-//   * expomf_solve_rows_kernel -- one CTA solves one row completely: it streams the whole other table through shared
-//     memory, weights each staged row by its posterior, lifts the row's observed entries to 1 with a sparse correction
-//     pass, and solves on the same tiles and Cholesky.  Fused into the item half, it also sums the posteriors of the
-//     new row for the exposure prior.
+//   * exposure_solve_rows_kernel<NT, ExpoPrior> -- one CTA solves one row completely: it streams the whole other
+//     table through shared memory, weights each staged row by its posterior, lifts the row's observed entries to 1
+//     with a sparse correction pass, and solves on the same tiles and Cholesky.  Fused into the item half, it also
+//     sums the posteriors of the new row for the exposure prior.
 //
 //   SERec (model/ranking/SERec.py): ExpoMF with a prior per (user, item) pair that grows with the user's number of
 //   followees (serec_step.cuh).  The reference's dense U x I prior has a closed form in one float64 sum per item and
 //   one degree per user, evaluated per pair inside the solve.
-//   * serec_solve_rows_kernel -- the same row solve as ExpoMF's (exposure_solve_rows, generic over the prior policy);
-//     fused into the item half, it writes each item's summed posterior for the next epoch's prior.
+//   * exposure_solve_rows_kernel<NT, SocialPrior> -- ExpoMF's row solve with the social prior policy; fused into the
+//     item half, it writes each item's summed posterior for the next epoch's prior.
+#include <type_traits>
+
 #include "common.h"
 #include "device.cuh"
 #include "als_step.cuh"
@@ -154,9 +156,9 @@ __device__ __forceinline__ void stage_rows(double* Zs, const T* __restrict__ Z, 
 }
 
 // Factors the upper triangle of A (d x d, leading dimension ld) in place with the whole CTA (als_step.cuh) and solves
-// A x = bv with warp 0, which stores x to out: the steps of als_solve_rows_kernel's tail, for the item sweep's two
-// solves (WRMF's kernel keeps its own inline copy, so its code stays as it was).  Entered after a barrier that
-// published A and bv.  Returns false on every thread when a pivot is not positive and finite; out is then untouched.
+// A x = bv with warp 0, which stores x to out: the tail of the item sweep's and the exposure kernel's solves (WRMF's
+// kernel writes the same steps out, see there).  Entered after a barrier that published A and bv.  Returns false on
+// every thread when a pivot is not positive and finite; out is then untouched.
 template <typename T>
 __device__ __forceinline__ bool chol_solve(double* A, int d, int ld, double* sd, const double* bv, T* out) {
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -203,6 +205,18 @@ __device__ __forceinline__ bool chol_solve(double* A, int d, int ld, double* sd,
       if (e * 32 + lane < d) out[e * 32 + lane] = (T)y[e];
   }
   return true;
+}
+
+// The CTA's sum of v as held by lane 0 of each warp: the lanes 0 store it to part (kThreads / 32 doubles) and, after
+// a barrier, thread 0 adds them from 0.0 in warp order, so the sum does not depend on scheduling.  Called by every
+// thread; returns the sum on thread 0 (0.0 elsewhere).  part must not be written again before the next barrier.
+__device__ __forceinline__ double cta_sum(double v, double* part) {
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < kThreads / 32; ++w) s += part[w];
+  return s;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -307,6 +321,7 @@ als_solve_rows_kernel(T* __restrict__ X, const T* __restrict__ Z, const double* 
     }
     if (t < d) bv[t] = bacc;
     __syncthreads();
+    // chol_solve's steps written out: called here, the NT = 1 kernels spill more and solve ~1% slower on an H100
     bool ok = true;
     for (int j = 0; j < d; ++j) {
       const double p = A[j * ld + j];
@@ -356,16 +371,9 @@ als_solve_rows_kernel(T* __restrict__ X, const T* __restrict__ Z, const double* 
     }
   }
   if (loss != nullptr) {
-    __shared__ double wsum[kThreads / 32];
-    lsum = warp_sum(lsum);
-    __syncthreads();
-    if (lane == 0) wsum[warp] = lsum;
-    __syncthreads();
-    if (t == 0) {
-      double s = 0.0;
-      for (int w = 0; w < kThreads / 32; ++w) s += wsum[w];
-      if (s != 0.0) atomicAdd(loss, s);
-    }
+    __shared__ double part[kThreads / 32];
+    const double s = cta_sum(lsum, part);
+    if (t == 0 && s != 0.0) atomicAdd(loss, s);
   }
 }
 
@@ -519,18 +527,10 @@ cofactor_item_sweep_kernel(T* Y, T* G, T* wb, T* cb, const T* __restrict__ X, co
       tl.reduce_into(A, d, ld);
       for (int a = t; a < d; a += kThreads) A[a * ld + a] += gamma;
       if (t < d) bv[t] = by;
-      if (lane == 0) {
-        part[0][warp] = wsum;
-        part[1][warp] = csum;
-      }
-      __syncthreads();
+      const double sw = cta_sum(wsum, part[0]);         // its barrier also publishes A and bv
+      const double sc = cta_sum(csum, part[1]);
       if (!chol_solve<T>(A, d, ld, sd, bv, gi) && t == 0 && n_failed != nullptr) atomicAdd(n_failed, 1);
       if (t == 0) {
-        double sw = 0.0, sc = 0.0;
-        for (int w = 0; w < kThreads / 32; ++w) {
-          sw += part[0][w];
-          sc += part[1][w];
-        }
         wb[i] = (T)cof_mean(sw, nctx);
         cb[i] = (T)cof_mean(sc, nctx);
       }
@@ -566,7 +566,7 @@ __device__ __forceinline__ double expomf_weights(const double* Zs, const double*
   return sum;
 }
 
-// Prior policies of exposure_solve_rows (below).  A policy says what prior each (row r, column k) pair of the solve
+// Prior policies of exposure_solve_rows_kernel (below).  A policy says what prior each (row r, column k) pair of the solve
 // uses, what prior the fused pass after the solve uses, and what that pass writes.  row(r) loads the row's own
 // state once; solve(p, k) and out(p, k) take the column as a functor, so that a policy that does not need it does not
 // load it.
@@ -641,15 +641,14 @@ struct SocialPrior {
 // which P::write stores -- never into the prior being read, which other CTAs may still read.  Nothing depends on the
 // grid, so X and the fused output are bitwise reproducible.
 template <int NT, class P>
-__device__ __forceinline__ void exposure_solve_rows(float* X, const float* __restrict__ Z, int d, long long n_z,
-                                                    long long n_order, const int* __restrict__ order,
-                                                    const long long* __restrict__ rowptr,
-                                                    const int* __restrict__ cols, const P& prior, double lambda,
-                                                    double lam_y, int* n_failed) {
+__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
+exposure_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
+                           const int* __restrict__ order, const long long* __restrict__ rowptr,
+                           const int* __restrict__ cols, P prior, double lambda, double lam_y, int* n_failed) {
   extern __shared__ __align__(16) double smem[];
   __shared__ double part[kThreads / 32];
   const int dp = pad4(d), ld = dp + 1;
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   double* A = smem;
   double* Zs = A + a_words(d);
   double* W = Zs + kStage * dp;
@@ -718,43 +717,35 @@ __device__ __forceinline__ void exposure_solve_rows(float* X, const float* __res
       asum += expomf_weights<true>(Zs, xo, nullptr, d, dp, cnt, lam_y,
                                    [=](int k) { return prior.out(pr, [=] { return __ldg(cols + k0 + k); }); });
     }
-    if (lane == 0) part[warp] = asum;
-    __syncthreads();
-    if (t == 0) {
-      double s = 0.0;
-      for (int w = 0; w < kThreads / 32; ++w) s += part[w];
-      prior.write(r, s);
-    }
+    const double s = cta_sum(asum, part);
+    if (t == 0) prior.write(r, s);
   }
 }
 
-// The two policies keep separate entry points.  ExpoMF's keeps its flat parameter list, so its kernels compile to the
-// code they had before the policy was factored out; SERec's takes its policy as one parameter.
-template <int NT>
-__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
-expomf_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
-                         const int* __restrict__ order, const long long* __restrict__ rowptr,
-                         const int* __restrict__ cols, const float* __restrict__ mu, int mu_by_row,
-                         float* __restrict__ mu_out, double lambda, double lam_y, double a, double b, int* n_failed) {
-  exposure_solve_rows<NT>(X, Z, d, n_z, n_order, order, rowptr, cols, ExpoPrior{mu, mu_by_row, mu_out, a, b, n_z},
-                          lambda, lam_y, n_failed);
-}
-
-template <int NT>
-__global__ void __launch_bounds__(kThreads, NT == 1 ? 3 : 1)
-serec_solve_rows_kernel(float* X, const float* __restrict__ Z, int d, long long n_z, long long n_order,
-                        const int* __restrict__ order, const long long* __restrict__ rowptr,
-                        const int* __restrict__ cols, SocialPrior prior, double lambda, double lam_y, int* n_failed) {
-  exposure_solve_rows<NT>(X, Z, d, n_z, n_order, order, rowptr, cols, prior, lambda, lam_y, n_failed);
-}
-
-// persistent grid: as many CTAs as fit on the GPU at `bytes` of dynamic shared memory, at most `work`
+// persistent grid: as many CTAs as fit on the GPU at `bytes` of dynamic shared memory, at most `work`, and at most
+// max_ctas when it is > 0.  Never more than fit at once: the CoFactor sweep needs every CTA of its grid resident.
 template <class K>
-int persistent_grid(K kernel, size_t bytes, long long work, int* grid) {
+int persistent_grid(K kernel, size_t bytes, long long work, int max_ctas, int* grid) {
   QREC_CUDA(allow_dynamic_smem((const void*)kernel, (int)bytes));
   int per_sm = 0;
   QREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, bytes));
   *grid = capped_grid(work, per_sm > 0 ? per_sm : 1);
+  if (max_ctas > 0 && *grid > max_ctas) *grid = max_ctas;
+  return QREC_OK;
+}
+
+// Launches kernel_of(std::integral_constant<int, NT>{})(args...) on its persistent grid, with the tile count NT of a
+// d-wide system: 1 when the upper triangle's 4x4 tiles fit one per thread, else 3 (d <= kMaxD).
+template <class KernelOf, class... Args>
+int launch_rows(KernelOf kernel_of, int d, size_t bytes, long long work, int max_ctas, cudaStream_t st,
+                Args... args) {
+  const auto kernel = tiles_of(d) <= kThreads ? kernel_of(std::integral_constant<int, 1>{})
+                                              : kernel_of(std::integral_constant<int, 3>{});
+  int grid = 0;
+  const int rc = persistent_grid(kernel, bytes, work, max_ctas, &grid);
+  if (rc) return rc;
+  kernel<<<grid, kThreads, bytes, st>>>(args...);
+  QREC_LAUNCH_CHECK();
   return QREC_OK;
 }
 
@@ -772,18 +763,9 @@ int launch_gram(const T* Z, long long n, int d, double* G, void* ws, long long w
                nchunks * d * d * (long long)sizeof(double));
   double* parts = (double*)ws;
   if (nchunks > 0) {
-    const size_t bytes = smem_bytes(d);
-    int grid = 0;
-    if (tiles_of(d) <= kThreads) {
-      const int rc = persistent_grid(als_gram_partial_kernel<T, 1>, bytes, nchunks, &grid);
-      if (rc) return rc;
-      als_gram_partial_kernel<T, 1><<<grid, kThreads, bytes, st>>>(Z, n, d, parts);
-    } else {
-      const int rc = persistent_grid(als_gram_partial_kernel<T, 3>, bytes, nchunks, &grid);
-      if (rc) return rc;
-      als_gram_partial_kernel<T, 3><<<grid, kThreads, bytes, st>>>(Z, n, d, parts);
-    }
-    QREC_LAUNCH_CHECK();
+    const int rc = launch_rows([](auto nt) { return als_gram_partial_kernel<T, decltype(nt)::value>; }, d,
+                               smem_bytes(d), nchunks, 0, st, Z, n, d, parts);
+    if (rc) return rc;
   }
   als_gram_sum_kernel<<<(d * d + kThreads - 1) / kThreads, kThreads, 0, st>>>(parts, nchunks, d * d, G);
   QREC_LAUNCH_CHECK();
@@ -799,21 +781,8 @@ int launch_solve(T* X, const T* Z, const double* G, int d, long long n_order, co
   if (n_order == 0) return QREC_OK;
   QREC_REQUIRE(X && Z && G && order && rowptr, "als_solve_rows: null pointer");
   QREC_REQUIRE((const void*)X != (const void*)Z, "als_solve_rows: X and Z must be different tables");
-  const size_t bytes = smem_bytes(d);
-  int grid = 0;
-  if (tiles_of(d) <= kThreads) {
-    const int rc = persistent_grid(als_solve_rows_kernel<T, 1>, bytes, n_order, &grid);
-    if (rc) return rc;
-    als_solve_rows_kernel<T, 1><<<grid, kThreads, bytes, st>>>(X, Z, G, d, n_order, order, rowptr, cols, vals,
-                                                                lambda, alpha, loss, n_failed);
-  } else {
-    const int rc = persistent_grid(als_solve_rows_kernel<T, 3>, bytes, n_order, &grid);
-    if (rc) return rc;
-    als_solve_rows_kernel<T, 3><<<grid, kThreads, bytes, st>>>(X, Z, G, d, n_order, order, rowptr, cols, vals,
-                                                                lambda, alpha, loss, n_failed);
-  }
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_rows([](auto nt) { return als_solve_rows_kernel<T, decltype(nt)::value>; }, d, smem_bytes(d),
+                     n_order, 0, st, X, Z, G, d, n_order, order, rowptr, cols, vals, lambda, alpha, loss, n_failed);
 }
 
 template <typename T>
@@ -828,23 +797,9 @@ int launch_cofactor(T* Y, T* G, T* w, T* c, const T* X, const double* XtX, int d
   QREC_REQUIRE((const void*)Y != (const void*)G && (const void*)Y != (const void*)X && (const void*)G != (const void*)X,
                "cofactor_item_sweep: Y, G and X must be different tables");
   QREC_REQUIRE(sweep >= 1, "cofactor_item_sweep: sweep=%d (stamps count sweeps from 1)", sweep);
-  const size_t bytes = cof_smem_bytes(d);
-  int grid = 0;
-  if (tiles_of(d) <= kThreads) {
-    const int rc = persistent_grid(cofactor_item_sweep_kernel<T, 1>, bytes, n_items, &grid);
-    if (rc) return rc;
-    cofactor_item_sweep_kernel<T, 1><<<grid, kThreads, bytes, st>>>(Y, G, w, c, X, XtX, d, n_items, irp, icol, ival,
-                                                                     srp, scol, sval, lambda, gamma, alpha, stamps,
-                                                                     sweep, ticket, n_failed);
-  } else {
-    const int rc = persistent_grid(cofactor_item_sweep_kernel<T, 3>, bytes, n_items, &grid);
-    if (rc) return rc;
-    cofactor_item_sweep_kernel<T, 3><<<grid, kThreads, bytes, st>>>(Y, G, w, c, X, XtX, d, n_items, irp, icol, ival,
-                                                                     srp, scol, sval, lambda, gamma, alpha, stamps,
-                                                                     sweep, ticket, n_failed);
-  }
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_rows([](auto nt) { return cofactor_item_sweep_kernel<T, decltype(nt)::value>; }, d,
+                     cof_smem_bytes(d), n_items, 0, st, Y, G, w, c, X, XtX, d, n_items, irp, icol, ival, srp, scol,
+                     sval, lambda, gamma, alpha, stamps, sweep, ticket, n_failed);
 }
 
 int launch_expomf(float* X, const float* Z, int d, long long n_z, long long n_order, const int* order,
@@ -857,23 +812,10 @@ int launch_expomf(float* X, const float* Z, int d, long long n_z, long long n_or
   QREC_REQUIRE(X && Z && order && rowptr && mu, "expomf_solve_rows: null pointer");
   QREC_REQUIRE((const void*)X != (const void*)Z, "expomf_solve_rows: X and Z must be different tables");
   QREC_REQUIRE((const void*)mu_out != (const void*)mu, "expomf_solve_rows: mu_out must not be mu");
-  const size_t bytes = smem_bytes(d);
-  int grid = 0;
-  if (tiles_of(d) <= kThreads) {
-    const int rc = persistent_grid(expomf_solve_rows_kernel<1>, bytes, n_order, &grid);
-    if (rc) return rc;
-    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-    expomf_solve_rows_kernel<1><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, mu,
-                                                                mu_by_row, mu_out, lambda, lam_y, a, b, n_failed);
-  } else {
-    const int rc = persistent_grid(expomf_solve_rows_kernel<3>, bytes, n_order, &grid);
-    if (rc) return rc;
-    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-    expomf_solve_rows_kernel<3><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, mu,
-                                                                mu_by_row, mu_out, lambda, lam_y, a, b, n_failed);
-  }
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  const ExpoPrior prior{mu, mu_by_row, mu_out, a, b, n_z};
+  return launch_rows([](auto nt) { return exposure_solve_rows_kernel<decltype(nt)::value, ExpoPrior>; }, d,
+                     smem_bytes(d), n_order, max_ctas, st, X, Z, d, n_z, n_order, order, rowptr, cols, prior, lambda,
+                     lam_y, n_failed);
 }
 
 int launch_serec(float* X, const float* Z, int d, long long n_z, long long n_order, const int* order,
@@ -889,23 +831,9 @@ int launch_serec(float* X, const float* Z, int d, long long n_z, long long n_ord
   QREC_REQUIRE(asum_out == nullptr || (const void*)asum_out != (const void*)asum,
                "serec_solve_rows: asum_out must not be asum");
   const SocialPrior prior{asum, (double)mu0, deg, row_is_user, asum_out, a, b, s, (double)n_users};
-  const size_t bytes = smem_bytes(d);
-  int grid = 0;
-  if (tiles_of(d) <= kThreads) {
-    const int rc = persistent_grid(serec_solve_rows_kernel<1>, bytes, n_order, &grid);
-    if (rc) return rc;
-    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-    serec_solve_rows_kernel<1><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, prior,
-                                                               lambda, lam_y, n_failed);
-  } else {
-    const int rc = persistent_grid(serec_solve_rows_kernel<3>, bytes, n_order, &grid);
-    if (rc) return rc;
-    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-    serec_solve_rows_kernel<3><<<grid, kThreads, bytes, st>>>(X, Z, d, n_z, n_order, order, rowptr, cols, prior,
-                                                               lambda, lam_y, n_failed);
-  }
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
+  return launch_rows([](auto nt) { return exposure_solve_rows_kernel<decltype(nt)::value, SocialPrior>; }, d,
+                     smem_bytes(d), n_order, max_ctas, st, X, Z, d, n_z, n_order, order, rowptr, cols, prior, lambda,
+                     lam_y, n_failed);
 }
 
 }  // namespace

@@ -5,6 +5,7 @@ streams, torch.distributed); every compute call below goes through ctypes into t
 sm_90a kernels.  There is no CPU path here: device entry points raise if a tensor is not on a
 CUDA device.
 """
+import contextlib
 import ctypes as C
 import math
 
@@ -976,6 +977,24 @@ def mf_predict_pairs(P, Q, u, i, Bu=None, Bi=None, global_mean=0.0, out=None):
 # =============================================================================================
 # K10: WRMF (implicit-feedback ALS) -- Gram matrix and per-row normal-equation solve
 # =============================================================================================
+_ROWS_FAILED = 'row(s) with normal equations that are not positive definite were left unchanged'
+
+
+@contextlib.contextmanager
+def _failures(n_failed, device, message):
+    """Yields the n_failed counter of one ALS-family launch: the caller's, or, when the caller gave none, a zeroed
+    one that is read back after the launch; a count above 0 in it raises QRecError(message % count)."""
+    own = n_failed is None
+    if own:
+        torch = _torch()
+        n_failed = torch.zeros(1, dtype=torch.int32, device=device)
+    yield n_failed
+    if own:
+        bad = int(n_failed.item())
+        if bad:
+            raise QRecError(message % bad)
+
+
 def als_row_order(rowptr):
     """Rows by decreasing entry count (ties by id): the order als_solve_rows hands rows to its persistent grid,
     so that one long row does not become the tail.  rowptr: host int64 array."""
@@ -1016,20 +1035,13 @@ def als_solve_rows(X, Z, G, rowptr, cols, vals, lam, alpha, row_order, loss=None
     dt = X.dtype
     if Z.shape[1] != d:
         raise QRecError('X and Z differ in width (%d, %d)' % (d, Z.shape[1]))
-    own = n_failed is None
-    if own:
-        n_failed = torch.zeros(1, dtype=torch.int32, device=X.device)
     fn = lib.qrec_als_solve_rows_f64 if dt == torch.float64 else lib.qrec_als_solve_rows_f32
-    check(fn(_dev(X, dt, 'X'), _dev(Z, dt, 'Z'), _dev(G, torch.float64, 'G'), d, row_order.shape[0],
-             _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
-             _dev(cols, torch.int32, 'cols'), _dev(vals, dt, 'vals'), float(lam), float(alpha),
-             _opt(loss, torch.float64, 'loss'), _dev(n_failed, torch.int32, 'n_failed'), _stream()),
-          'qrec_als_solve_rows')
-    if own:
-        bad = int(n_failed.item())
-        if bad:
-            raise QRecError('als_solve_rows: %d row(s) with normal equations that are not positive definite were '
-                            'left unchanged' % bad)
+    with _failures(n_failed, X.device, 'als_solve_rows: %d ' + _ROWS_FAILED) as n_failed:
+        check(fn(_dev(X, dt, 'X'), _dev(Z, dt, 'Z'), _dev(G, torch.float64, 'G'), d, row_order.shape[0],
+                 _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
+                 _dev(cols, torch.int32, 'cols'), _dev(vals, dt, 'vals'), float(lam), float(alpha),
+                 _opt(loss, torch.float64, 'loss'), _dev(n_failed, torch.int32, 'n_failed'), _stream()),
+              'qrec_als_solve_rows')
     return X
 
 
@@ -1134,27 +1146,51 @@ def cofactor_item_sweep(Y, G, w, c, X, XtX, item_csr, sppmi, lam, gamma, alpha, 
     elif stamps.shape != (n_items,) or (n_items and not bool((stamps == sweep - 1).all())):
         raise QRecError('cofactor_item_sweep: stamps must hold %d (sweep - 1) for every item' % (sweep - 1))
     ticket = torch.zeros(1, dtype=torch.int64, device=Y.device)
-    own = n_failed is None
-    if own:
-        n_failed = torch.zeros(1, dtype=torch.int32, device=Y.device)
     fn = lib.qrec_cofactor_item_sweep_f64 if dt == torch.float64 else lib.qrec_cofactor_item_sweep_f32
-    check(fn(_dev(Y, dt, 'Y'), _dev(G, dt, 'G'), _dev(w, dt, 'w'), _dev(c, dt, 'c'), _dev(X, dt, 'X'),
-             _dev(XtX, torch.float64, 'XtX'), d, n_items, _dev(irp, torch.int64, 'item rowptr'),
-             _dev(icol, torch.int32, 'item users'), _dev(ival, dt, 'item ratings'), _dev(srp, torch.int64, 'SPPMI rowptr'),
-             _dev(scol, torch.int32, 'SPPMI cols'), _dev(sval, dt, 'SPPMI vals'), float(lam), float(gamma),
-             float(alpha), _dev(stamps, torch.int32, 'stamps'), int(sweep), ticket.data_ptr(),
-             _dev(n_failed, torch.int32, 'n_failed'), _stream()), 'qrec_cofactor_item_sweep')
-    if own:
-        bad = int(n_failed.item())
-        if bad:
-            raise QRecError('cofactor_item_sweep: %d system(s) that are not positive definite left their rows '
-                            'unchanged' % bad)
+    with _failures(n_failed, Y.device, 'cofactor_item_sweep: %d system(s) that are not positive definite left their '
+                   'rows unchanged') as n_failed:
+        check(fn(_dev(Y, dt, 'Y'), _dev(G, dt, 'G'), _dev(w, dt, 'w'), _dev(c, dt, 'c'), _dev(X, dt, 'X'),
+                 _dev(XtX, torch.float64, 'XtX'), d, n_items, _dev(irp, torch.int64, 'item rowptr'),
+                 _dev(icol, torch.int32, 'item users'), _dev(ival, dt, 'item ratings'),
+                 _dev(srp, torch.int64, 'SPPMI rowptr'), _dev(scol, torch.int32, 'SPPMI cols'),
+                 _dev(sval, dt, 'SPPMI vals'), float(lam), float(gamma), float(alpha),
+                 _dev(stamps, torch.int32, 'stamps'), int(sweep), ticket.data_ptr(),
+                 _dev(n_failed, torch.int32, 'n_failed'), _stream()), 'qrec_cofactor_item_sweep')
     return Y
 
 
 # =============================================================================================
 # K13: ExpoMF -- exposure posterior and weighted normal equations, fused per row
 # =============================================================================================
+def _exposure_checks(name, X, Z, rowptr, cols, row_order):
+    """The checks expomf_half_epoch and serec_half_epoch (`name`) share: X [n, d] and Z [m, d] float32 and not one
+    table, 1 <= d <= 128, and a CSR of n rows into [0, m) with row_order a list of its rows.  Returns (n, d, m)."""
+    f32 = _torch().float32
+    for t, tname in ((X, 'X'), (Z, 'Z')):
+        if t.dtype != f32:
+            raise QRecError('%s: %s must be float32, got %s' % (name, tname, t.dtype))
+    if X.dim() != 2 or Z.dim() != 2 or Z.shape[1] != X.shape[1]:
+        raise QRecError('%s: X and Z must be 2-D tables of one width' % name)
+    n, d = X.shape
+    m = Z.shape[0]
+    if not 1 <= d <= 128:
+        raise QRecError('%s: d=%d unsupported (1..128)' % (name, d))
+    if X.data_ptr() == Z.data_ptr():
+        raise QRecError('%s: X and Z must be different tables' % name)
+    if rowptr.shape != (n + 1,):
+        raise QRecError('%s: rowptr needs %d entries' % (name, n + 1))
+    if row_order.dim() != 1 or row_order.shape[0] > n:
+        raise QRecError('%s: row_order must be a list of at most %d rows' % (name, n))
+    if row_order.numel() and (int(row_order.min()) < 0 or int(row_order.max()) >= n):
+        raise QRecError('%s: a row of row_order is outside [0, %d)' % (name, n))
+    nnz = cols.shape[0]
+    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
+        raise QRecError('%s: rowptr must rise from 0 to len(cols) = %d' % (name, nnz))
+    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= m):
+        raise QRecError('%s: a column is outside [0, %d)' % (name, m))
+    return n, d, m
+
+
 def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, mu_out=None, a=1.0, b=99.0,
                       n_failed=None, max_ctas=0):
     """One ExpoMF half-epoch (ExpoMF.py: recompute_factors) in place on the rows `row_order` of X (float32 [n, d])
@@ -1169,17 +1205,9 @@ def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, 
     given, the count is read back here and a failed row raises QRecError."""
     torch = _torch()
     f32 = torch.float32
-    for t, name in ((X, 'X'), (Z, 'Z'), (mu, 'mu')):
-        if t.dtype != f32:
-            raise QRecError('expomf_half_epoch: %s must be float32, got %s' % (name, t.dtype))
-    if X.dim() != 2 or Z.dim() != 2 or Z.shape[1] != X.shape[1]:
-        raise QRecError('expomf_half_epoch: X and Z must be 2-D tables of one width')
-    n, d = X.shape
-    m = Z.shape[0]
-    if not 1 <= d <= 128:
-        raise QRecError('expomf_half_epoch: d=%d unsupported (1..128)' % d)
-    if X.data_ptr() == Z.data_ptr():
-        raise QRecError('expomf_half_epoch: X and Z must be different tables')
+    n, d, m = _exposure_checks('expomf_half_epoch', X, Z, rowptr, cols, row_order)
+    if mu.dtype != f32:
+        raise QRecError('expomf_half_epoch: mu must be float32, got %s' % mu.dtype)
     want = n if mu_by_row else m
     if mu.shape != (want,):
         raise QRecError('expomf_half_epoch: mu indexed by %s needs %d entries, got %s'
@@ -1189,31 +1217,14 @@ def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, 
             raise QRecError('expomf_half_epoch: mu_out and mu need one float32 entry per row (%d)' % n)
         if mu_out.data_ptr() == mu.data_ptr():
             raise QRecError('expomf_half_epoch: mu_out must be a buffer of its own, not mu')
-    if rowptr.shape != (n + 1,):
-        raise QRecError('expomf_half_epoch: rowptr needs %d entries' % (n + 1))
-    if row_order.dim() != 1 or row_order.shape[0] > n:
-        raise QRecError('expomf_half_epoch: row_order must be a list of at most %d rows' % n)
-    if row_order.numel() and (int(row_order.min()) < 0 or int(row_order.max()) >= n):
-        raise QRecError('expomf_half_epoch: a row of row_order is outside [0, %d)' % n)
-    nnz = cols.shape[0]
-    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
-        raise QRecError('expomf_half_epoch: rowptr must rise from 0 to len(cols) = %d' % nnz)
-    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= m):
-        raise QRecError('expomf_half_epoch: a column is outside [0, %d)' % m)
-    own = n_failed is None
-    if own:
-        n_failed = torch.zeros(1, dtype=torch.int32, device=X.device)
-    check(lib.qrec_expomf_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
-                                         _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
-                                         _dev(cols, torch.int32, 'cols'), _dev(mu, f32, 'mu'), int(bool(mu_by_row)),
-                                         _opt(mu_out, f32, 'mu_out'), float(lam), float(lam_y), float(a), float(b),
-                                         int(max_ctas), _dev(n_failed, torch.int32, 'n_failed'), _stream()),
-          'qrec_expomf_solve_rows_f32')
-    if own:
-        bad = int(n_failed.item())
-        if bad:
-            raise QRecError('expomf_half_epoch: %d row(s) with normal equations that are not positive definite were '
-                            'left unchanged' % bad)
+    with _failures(n_failed, X.device, 'expomf_half_epoch: %d ' + _ROWS_FAILED) as n_failed:
+        check(lib.qrec_expomf_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
+                                             _dev(row_order, torch.int32, 'row_order'),
+                                             _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'),
+                                             _dev(mu, f32, 'mu'), int(bool(mu_by_row)), _opt(mu_out, f32, 'mu_out'),
+                                             float(lam), float(lam_y), float(a), float(b), int(max_ctas),
+                                             _dev(n_failed, torch.int32, 'n_failed'), _stream()),
+              'qrec_expomf_solve_rows_f32')
     return X
 
 
@@ -1234,17 +1245,7 @@ def serec_half_epoch(X, Z, rowptr, cols, asum, deg, row_is_user, lam, lam_y, row
     definite (left unchanged); when it is not given, the count is read back here and a failed row raises QRecError."""
     torch = _torch()
     f32, f64, i32 = torch.float32, torch.float64, torch.int32
-    for t, name in ((X, 'X'), (Z, 'Z')):
-        if t.dtype != f32:
-            raise QRecError('serec_half_epoch: %s must be float32, got %s' % (name, t.dtype))
-    if X.dim() != 2 or Z.dim() != 2 or Z.shape[1] != X.shape[1]:
-        raise QRecError('serec_half_epoch: X and Z must be 2-D tables of one width')
-    n, d = X.shape
-    m = Z.shape[0]
-    if not 1 <= d <= 128:
-        raise QRecError('serec_half_epoch: d=%d unsupported (1..128)' % d)
-    if X.data_ptr() == Z.data_ptr():
-        raise QRecError('serec_half_epoch: X and Z must be different tables')
+    n, d, m = _exposure_checks('serec_half_epoch', X, Z, rowptr, cols, row_order)
     n_users, n_items = (n, m) if row_is_user else (m, n)
     if asum is not None and (asum.dtype != f64 or asum.shape != (n_items,)):
         raise QRecError('serec_half_epoch: asum needs one float64 entry per item (%d), got %s %s'
@@ -1260,32 +1261,15 @@ def serec_half_epoch(X, Z, rowptr, cols, asum, deg, row_is_user, lam, lam_y, row
                             'the items' % n)
         if asum is not None and asum_out.data_ptr() == asum.data_ptr():
             raise QRecError('serec_half_epoch: asum_out must be a buffer of its own, not asum')
-    if rowptr.shape != (n + 1,):
-        raise QRecError('serec_half_epoch: rowptr needs %d entries' % (n + 1))
-    if row_order.dim() != 1 or row_order.shape[0] > n:
-        raise QRecError('serec_half_epoch: row_order must be a list of at most %d rows' % n)
-    if row_order.numel() and (int(row_order.min()) < 0 or int(row_order.max()) >= n):
-        raise QRecError('serec_half_epoch: a row of row_order is outside [0, %d)' % n)
-    nnz = cols.shape[0]
-    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
-        raise QRecError('serec_half_epoch: rowptr must rise from 0 to len(cols) = %d' % nnz)
-    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= m):
-        raise QRecError('serec_half_epoch: a column is outside [0, %d)' % m)
-    own = n_failed is None
-    if own:
-        n_failed = torch.zeros(1, dtype=i32, device=X.device)
-    check(lib.qrec_serec_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
-                                        _dev(row_order, i32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
-                                        _dev(cols, i32, 'cols'), _opt(asum, f64, 'asum'), float(mu0),
-                                        _dev(deg, i32, 'deg'), int(bool(row_is_user)), _opt(asum_out, f64, 'asum_out'),
-                                        float(lam), float(lam_y), float(a), float(b), float(s), n_users,
-                                        int(max_ctas), _dev(n_failed, i32, 'n_failed'), _stream()),
-          'qrec_serec_solve_rows_f32')
-    if own:
-        bad = int(n_failed.item())
-        if bad:
-            raise QRecError('serec_half_epoch: %d row(s) with normal equations that are not positive definite were '
-                            'left unchanged' % bad)
+    with _failures(n_failed, X.device, 'serec_half_epoch: %d ' + _ROWS_FAILED) as n_failed:
+        check(lib.qrec_serec_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
+                                            _dev(row_order, i32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
+                                            _dev(cols, i32, 'cols'), _opt(asum, f64, 'asum'), float(mu0),
+                                            _dev(deg, i32, 'deg'), int(bool(row_is_user)),
+                                            _opt(asum_out, f64, 'asum_out'), float(lam), float(lam_y), float(a),
+                                            float(b), float(s), n_users, int(max_ctas), _dev(n_failed, i32, 'n_failed'),
+                                            _stream()),
+              'qrec_serec_solve_rows_f32')
     return X
 
 

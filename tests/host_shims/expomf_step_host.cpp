@@ -1,6 +1,6 @@
 // Host build of qrec_b200/csrc/expomf_step.cuh (with als_step.cuh): one ExpoMF row solve and one row's exposure
 // prior on the CPU with the headers' own posterior, lift, prior, factorization and substitution functions, in the
-// order expomf_solve_rows_kernel applies them (every row of Z weighted by its posterior, then the observed entries
+// order exposure_solve_rows_kernel applies them (every row of Z weighted by its posterior, then the observed entries
 // lifted to 1) -- so the CPU suite pins the device source to the float64 oracle.  (The kernel spreads the sums over
 // threads; only the grouping of the float64 sums differs.)
 #include <cstddef>
