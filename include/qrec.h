@@ -780,6 +780,56 @@ int qrec_serec_solve_rows_f32(float* dev_X, const float* dev_Z, int32_t d, int64
                               double* dev_asum_out, double lambda, double lam_y, double a, double b, double s,
                               int64_t n_users, int32_t max_ctas, int32_t* dev_n_failed, void* stream);
 
+/* =====================================================================================
+ * K15 -- UserKNN, ItemKNN and SlopeOne (model/rating/UserKNN.py, ItemKNN.py, SlopeOne.py, util/qmath.py): float64
+ * statistics over the keys two training rows share, each operation separately rounded, no floating-point atomics.
+ * Rows are one side's training rows in insertion order (users for UserKNN, items for ItemKNN and SlopeOne).
+ * ===================================================================================== */
+/* Neighbour lists.  rowptr[n_rows + 1] / cols / vals: the rows, entries in insertion order, columns < n_cols and
+ * distinct within a row; sq: each entry's square as CPython's `**` gives it -- (x - mean)**2 for metric 0 (pcc),
+ * x**2 for 1 (cos) and 2 (euclidean); means[n_rows]: the row means.  col_rowptr[n_cols + 1] / col_rows / col_entries:
+ * the same entries by column (their row, and their index in cols).  queries[n_queries]: the query list, a row id or
+ * -1 (cold); pos_of_row[n_rows]: each row's position in it, or -1.  Non-cold queries are distinct.
+ * For the query at position p the reference's candidate list is every earlier query at list position p' (cold ones
+ * with similarity 0; others with similarity(earlier row, query row)) and then every other training row v that is not
+ * an earlier query at position n_queries + v (similarity(query row, v)); a cold query lists every training row at
+ * n_queries + v with similarity 0.  Writes the first K entries of that list sorted by (similarity descending,
+ * position ascending): out_ids[n_queries][K] (a row id; -2 - p' for the cold earlier query p'; -1 for padding),
+ * out_sims[n_queries][K] and out_cnt[n_queries] = min(K, list length).  max_ctas > 0 caps the persistent grid; the
+ * result does not depend on it. */
+int qrec_knn_neighbours_f64(int32_t metric, const int64_t* dev_rowptr, const int32_t* dev_cols, const double* dev_vals,
+                            const double* dev_sq, const double* dev_means, int32_t n_rows, int32_t n_cols,
+                            const int64_t* dev_col_rowptr, const int32_t* dev_col_rows, const int64_t* dev_col_entries,
+                            const int32_t* dev_queries, const int32_t* dev_pos_of_row, int32_t n_queries, int32_t K,
+                            int32_t* dev_out_ids, double* dev_out_sims, int32_t* dev_out_cnt, int32_t max_ctas,
+                            void* stream);
+/* KNN predictions of n_lines test lines.  Line l belongs to the query at position line_qpos[l] and probes the other
+ * side's id line_probe[l] (-1 when cold) in the rows of its neighbours (qrec_knn_neighbours_f64's output, K wide):
+ * rowptr / sorted_cols / sorted_vals hold every row's columns ascending with their values.  Walking the neighbours in
+ * order, a neighbour row that holds the probe (and, with minus_one_unrated, whose value is not -1) adds
+ * sim*(r - means[n]) to sum and sim to denom.  pred[l] = mean + sum/denom with mean = means[query] (global_mean for a
+ * cold query), status[l] = 0; when sum == 0: pred = mean, status 1; when denom == 0 != sum: status 2 (the reference
+ * raises ZeroDivisionError), pred 0. */
+int qrec_knn_predict_f64(const int64_t* dev_rowptr, const int32_t* dev_sorted_cols, const double* dev_sorted_vals,
+                         const double* dev_means, double global_mean, const int32_t* dev_queries, int32_t K,
+                         const int32_t* dev_nbr_ids, const double* dev_nbr_sims, const int32_t* dev_nbr_cnt,
+                         int64_t n_lines, const int32_t* dev_line_qpos, const int32_t* dev_line_probe,
+                         int32_t minus_one_unrated, double* dev_pred, int32_t* dev_status, void* stream);
+/* SlopeOne predictions.  item_* / user_*: the item rows (users, values) and the user rows (items, values) of the
+ * training set, each in insertion order, with their means.  test_items[n_test_items]: item ids or -1 (cold); the test
+ * lines of test item p are line_rowptr[p] .. line_rowptr[p + 1]: user line_user[k] (-1 when cold), written to
+ * pred[line_out[k]] / status[line_out[k]].  For each test item the diff / count row against every item is built from
+ * its users in insertion order; a warm user's prediction is sum((r + diff/count) * count) / sum(count) over the user's
+ * rated items in insertion order, or the user's mean when the counts sum to 0 (status 1); a cold user gets the item's
+ * mean, or global_mean for a cold item (status 1).  max_ctas as for qrec_knn_neighbours_f64. */
+int qrec_slopeone_predict_f64(const int64_t* dev_item_rowptr, const int32_t* dev_item_users, const double* dev_item_vals,
+                              const double* dev_item_means, const int64_t* dev_user_rowptr,
+                              const int32_t* dev_user_items, const double* dev_user_vals, const double* dev_user_means,
+                              double global_mean, int32_t n_items, const int32_t* dev_test_items, int32_t n_test_items,
+                              const int64_t* dev_line_rowptr, const int32_t* dev_line_user,
+                              const int64_t* dev_line_out, double* dev_pred, int32_t* dev_status, int32_t max_ctas,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -97,6 +97,12 @@ SIGNATURES = {
     'qrec_serec_solve_rows_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, C.c_int64, vp, vp, vp, vp, C.c_float, vp,
                                             C.c_int32, vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
                                             C.c_int64, C.c_int32, vp, vp]),
+    'qrec_knn_neighbours_f64': (C.c_int, [C.c_int32, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp,
+                                          C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, vp]),
+    'qrec_knn_predict_f64': (C.c_int, [vp, vp, vp, vp, C.c_double, vp, C.c_int32, vp, vp, vp, C.c_int64, vp, vp,
+                                       C.c_int32, vp, vp, vp]),
+    'qrec_slopeone_predict_f64': (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, C.c_double, C.c_int32, vp, C.c_int32, vp,
+                                            vp, vp, vp, vp, C.c_int32, vp]),
     'qrec_svdpp_sgd_ordered_f64': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_double,
                                              C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
     'qrec_svdpp_sgd_ordered_f32': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_float,

@@ -1325,3 +1325,229 @@ def svdpp_epoch_usermajor(P, Q, Y, Bu, Bi, rowptr, cols, vals, row_order, lr, re
                                              _dev(loss, torch.float64, 'loss'), int(max_users_in_flight), _stream()),
           'qrec_svdpp_epoch_usermajor_f32')
     return loss
+
+
+# =============================================================================================
+# K15: UserKNN, ItemKNN and SlopeOne -- co-rated statistics, exact neighbour lists and predictions
+# =============================================================================================
+KNN_METRICS = ('pcc', 'cos', 'euclidean')
+KNN_COLD = -2          # neighbour ids <= KNN_COLD: the cold earlier query at list position KNN_COLD - id
+KNN_PAD = -1
+
+
+def knn_metric(similarity):
+    """The reference's choice (util/qmath.py: similarity): 'pcc' and 'euclidean' select themselves, anything else
+    cosine.  Returns 0 (pcc), 1 (cos) or 2 (euclidean)."""
+    return 0 if similarity == 'pcc' else 2 if similarity == 'euclidean' else 1
+
+
+def knn_squares(rowptr, vals, means, metric):
+    """The per-entry squares the similarities add, as CPython's float `**` gives them (glibc pow(x, 2.0), which is not
+    always the correctly rounded x*x -- nor numpy's square): (x - mean)**2 with the row's mean for pcc (metric 0),
+    x**2 for cos and euclidean.  Host arrays in, a float64 array parallel to vals out."""
+    vals = np.asarray(vals, dtype=np.float64)
+    if metric == 0:
+        lengths = np.diff(np.asarray(rowptr, dtype=np.int64))
+        m = np.repeat(np.asarray(means, dtype=np.float64), lengths).tolist()
+        return np.array([(x - mu) ** 2 for x, mu in zip(vals.tolist(), m)], dtype=np.float64)
+    return np.array([x ** 2 for x in vals.tolist()], dtype=np.float64)
+
+
+def _knn_csr(name, rowptr, cols, n_cols):
+    """Host checks of a CSR: rowptr int64 rising from 0 to len(cols), columns int32 in [0, n_cols), distinct within
+    each row.  Returns the number of rows."""
+    torch = _torch()
+    if rowptr.dtype != torch.int64 or rowptr.dim() != 1 or rowptr.shape[0] < 1:
+        raise QRecError('%s: rowptr must be a 1-D int64 tensor of n_rows + 1 entries' % name)
+    if cols.dtype != torch.int32 or cols.dim() != 1:
+        raise QRecError('%s: cols must be a 1-D int32 tensor' % name)
+    n, nnz = rowptr.shape[0] - 1, cols.shape[0]
+    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
+        raise QRecError('%s: rowptr must rise from 0 to len(cols) = %d' % (name, nnz))
+    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= n_cols):
+        raise QRecError('%s: a column is outside [0, %d)' % (name, n_cols))
+    if n + n_cols >= 2 ** 31:
+        raise QRecError('%s: %d rows and %d columns exceed the int32 ids' % (name, n, n_cols))
+    return n
+
+
+def _knn_sorted(rowptr, cols, n_cols, *payload):
+    """Every row's entries ordered by column (stable on device): (sorted cols, the payloads in the same permutation,
+    the permutation).  Raises QRecError when a row repeats a column."""
+    torch = _torch()
+    n = rowptr.shape[0] - 1
+    row = torch.repeat_interleave(torch.arange(n, device=cols.device), rowptr[1:] - rowptr[:-1])
+    order = torch.argsort(row * n_cols + cols.to(torch.int64), stable=True)
+    sc = cols[order].contiguous()
+    if sc.shape[0] > 1 and bool(((sc[1:] == sc[:-1]) & (row[order][1:] == row[order][:-1])).any()):
+        raise QRecError('knn: a row lists the same column twice')
+    return (sc,) + tuple(p[order].contiguous() for p in payload) + (order,)
+
+
+def _knn_queries(name, queries, n_rows):
+    torch = _torch()
+    if queries.dtype != torch.int32 or queries.dim() != 1:
+        raise QRecError('%s: queries must be a 1-D int32 tensor' % name)
+    if queries.numel() and (int(queries.min()) < -1 or int(queries.max()) >= n_rows):
+        raise QRecError('%s: a query is outside [0, %d) and not -1 (cold)' % (name, n_rows))
+    warm = queries[queries >= 0]
+    if warm.numel() != torch.unique(warm).numel():
+        raise QRecError('%s: a row is queried twice' % name)
+
+
+def _f64_vec(name, t, n):
+    torch = _torch()
+    if t.dtype != torch.float64 or t.shape != (n,):
+        raise QRecError('%s must be float64 [%d], got %s %s' % (name, n, t.dtype, tuple(t.shape)))
+
+
+def knn_neighbours(rowptr, cols, vals, sq, means, n_cols, queries, metric, K, max_ctas=0):
+    """UserKNN / ItemKNN computeSimilarities: the first K entries of every query's sorted candidate list.
+    rowptr (int64 [n + 1]) / cols (int32 < n_cols) / vals (float64): the training rows in insertion order
+    (Rating.rating_csr); sq (float64, parallel to vals): knn_squares; means (float64 [n]): the row means (userMeans /
+    itemMeans); queries (int32): the query list in the reference's order (testSet_u / testSet_i), a row id or -1 for a
+    query with no training row; metric: 0 pcc, 1 cos, 2 euclidean (knn_metric); K >= 0.  All CUDA tensors.
+    Returns (ids int32 [Q, K], sims float64 [Q, K], counts int32 [Q]): ids are row ids, KNN_COLD - p for the cold
+    earlier query at position p, KNN_PAD past counts[q] = min(K, list length).  The list of the query at position p is
+    every earlier query (similarity(earlier row, this row)) and then every other training row (similarity(this row,
+    it)) -- a cold query lists every training row with similarity 0 -- sorted by similarity descending, stably.
+    max_ctas > 0 caps the grid (the result does not depend on it).  The selected entries are ranked by counting:
+    the cost grows with K**2 per query, which is small at the models' num.neighbors and large when K spans the whole
+    list of a large set."""
+    torch = _torch()
+    i32, i64, f64 = torch.int32, torch.int64, torch.float64
+    if metric not in (0, 1, 2):
+        raise QRecError('knn_neighbours: metric must be 0 (pcc), 1 (cos) or 2 (euclidean), got %r' % (metric,))
+    if int(K) != K or K < 0:
+        raise QRecError('knn_neighbours: K must be an integer >= 0, got %r' % (K,))
+    n = _knn_csr('knn_neighbours', rowptr, cols, n_cols)
+    for t, name in ((vals, 'vals'), (sq, 'sq')):
+        _f64_vec('knn_neighbours: ' + name, t, cols.shape[0])
+    _f64_vec('knn_neighbours: means', means, n)
+    _knn_queries('knn_neighbours', queries, n)
+    Q, K = queries.shape[0], int(K)
+    if Q + n >= 2 ** 31:
+        raise QRecError('knn_neighbours: %d queries and %d rows exceed the int32 list positions' % (Q, n))
+    dev = cols.device
+    _knn_sorted(rowptr, cols, n_cols)
+    # the entries by column: their rows and their indices
+    ent = torch.argsort(cols, stable=True)
+    crows = torch.repeat_interleave(torch.arange(n, dtype=i32, device=dev), rowptr[1:] - rowptr[:-1])[ent].contiguous()
+    crowptr = torch.zeros(n_cols + 1, dtype=i64, device=dev)
+    crowptr[1:] = torch.cumsum(torch.bincount(cols.to(i64), minlength=n_cols), 0)
+    pos_of_row = torch.full((n,), -1, dtype=i32, device=dev)
+    warm = queries >= 0
+    pos_of_row[queries[warm].to(i64)] = torch.arange(Q, dtype=i32, device=dev)[warm]
+    ids = torch.empty((Q, K), dtype=i32, device=dev)
+    sims = torch.empty((Q, K), dtype=f64, device=dev)
+    cnt = torch.empty(Q, dtype=i32, device=dev)
+    check(lib.qrec_knn_neighbours_f64(int(metric), _dev(rowptr, i64, 'rowptr'), _dev(cols, i32, 'cols'),
+                                      _dev(vals, f64, 'vals'), _dev(sq, f64, 'sq'), _dev(means, f64, 'means'), n,
+                                      int(n_cols), crowptr.data_ptr(), crows.data_ptr(), ent.data_ptr(),
+                                      _dev(queries, i32, 'queries'), pos_of_row.data_ptr(),
+                                      Q, K, ids.data_ptr(), sims.data_ptr(), cnt.data_ptr(), int(max_ctas), _stream()),
+          'qrec_knn_neighbours_f64')
+    return ids, sims, cnt
+
+
+def knn_sorted_view(rowptr, cols, vals):
+    """The view of the rows knn_predict searches: every row's columns ascending (int32), with their values (float64)
+    in the same permutation.  Built once per model; a row that repeats a column raises QRecError."""
+    n_cols = int(cols.max()) + 1 if cols.numel() else 1
+    _knn_csr('knn_sorted_view', rowptr, cols, n_cols)
+    _f64_vec('knn_sorted_view: vals', vals, cols.shape[0])
+    scols, svals, _ = _knn_sorted(rowptr, cols, n_cols, vals)
+    return scols, svals
+
+
+def knn_predict(rowptr, sorted_cols, sorted_vals, means, global_mean, queries, ids, sims, counts, line_qpos,
+                line_probe, minus_one_unrated):
+    """UserKNN / ItemKNN predictForRating for a batch of test lines.  rowptr / means: the rows the neighbours were
+    chosen from (as knn_neighbours), sorted_cols / sorted_vals: their knn_sorted_view; queries, ids, sims, counts: the
+    query list and knn_neighbours' output; line_qpos (int32): each line's query position; line_probe (int32): the
+    line's id on the other side (the item for UserKNN, the user for ItemKNN), -1 when it has no training row.
+    minus_one_unrated: a stored rating of -1 counts as unrated (UserKNN).  Returns (pred float64, status int32):
+    status 0 normal, 1 the mean fallback, 2 the reference's ZeroDivisionError (sum != 0 over a zero denominator)."""
+    torch = _torch()
+    i32, i64, f64 = torch.int32, torch.int64, torch.float64
+    n = rowptr.shape[0] - 1
+    cols = sorted_cols
+    n_cols = int(cols.max()) + 1 if cols.numel() else 0
+    _knn_csr('knn_predict', rowptr, cols, n_cols)
+    _f64_vec('knn_predict: sorted_vals', sorted_vals, cols.shape[0])
+    _f64_vec('knn_predict: means', means, n)
+    if cols.numel() > 1:
+        row = torch.repeat_interleave(torch.arange(n, device=cols.device), rowptr[1:] - rowptr[:-1])
+        if bool(((cols[1:] <= cols[:-1]) & (row[1:] == row[:-1])).any()):
+            raise QRecError('knn_predict: sorted_cols must rise strictly within each row (knn_sorted_view)')
+    _knn_queries('knn_predict', queries, n)
+    Q = queries.shape[0]
+    if ids.dim() != 2 or ids.shape[0] != Q or sims.shape != ids.shape or counts.shape != (Q,):
+        raise QRecError('knn_predict: ids / sims must be [%d, K] and counts [%d]' % (Q, Q))
+    K = ids.shape[1]
+    if Q and (int(counts.min()) < 0 or int(counts.max()) > K):
+        raise QRecError('knn_predict: a count is outside [0, %d]' % K)
+    if K and Q and int(ids.max()) >= n:
+        raise QRecError('knn_predict: a neighbour id is outside [0, %d)' % n)
+    L = line_qpos.shape[0]
+    if line_qpos.dtype != i32 or line_probe.dtype != i32 or line_probe.shape != (L,):
+        raise QRecError('knn_predict: line_qpos and line_probe must be int32 of one length')
+    if L and (int(line_qpos.min()) < 0 or int(line_qpos.max()) >= Q):
+        raise QRecError('knn_predict: a line query position is outside [0, %d)' % Q)
+    if L and int(line_probe.min()) < -1:
+        raise QRecError('knn_predict: a probe id is below -1')
+    pred = torch.empty(L, dtype=f64, device=cols.device)
+    status = torch.empty(L, dtype=i32, device=cols.device)
+    check(lib.qrec_knn_predict_f64(_dev(rowptr, i64, 'rowptr'), _dev(cols, i32, 'sorted_cols'),
+                                   _dev(sorted_vals, f64, 'sorted_vals'),
+                                   _dev(means, f64, 'means'), float(global_mean), _dev(queries, i32, 'queries'), K,
+                                   _dev(ids, i32, 'ids'), _dev(sims, f64, 'sims'), _dev(counts, i32, 'counts'), L,
+                                   _dev(line_qpos, i32, 'line_qpos'), _dev(line_probe, i32, 'line_probe'),
+                                   int(bool(minus_one_unrated)), pred.data_ptr(), status.data_ptr(), _stream()),
+          'qrec_knn_predict_f64')
+    return pred, status
+
+
+def slopeone_predict(item_rowptr, item_users, item_vals, item_means, user_rowptr, user_items, user_vals, user_means,
+                     global_mean, test_items, line_qpos, line_user, max_ctas=0):
+    """SlopeOne initModel + predictForRating for every test line in one launch.  item_* / user_*: the training set by
+    item (Rating.rating_csr('item')) and by user (rating_csr('user')) with itemMeans / userMeans; test_items (int32):
+    the test item list (testSet_i order), an item id or -1 when cold; line_qpos (int32): each line's position in
+    test_items; line_user (int32): its user id or -1 when cold.  Returns (pred float64, status int32); status 1 marks
+    the mean fallbacks.  max_ctas > 0 caps the grid (the result does not depend on it)."""
+    torch = _torch()
+    i32, i64, f64 = torch.int32, torch.int64, torch.float64
+    n_items, n_users = item_rowptr.shape[0] - 1, user_rowptr.shape[0] - 1
+    _knn_csr('slopeone_predict: item rows', item_rowptr, item_users, n_users)
+    _knn_csr('slopeone_predict: user rows', user_rowptr, user_items, n_items)
+    if item_users.shape[0] != user_items.shape[0]:
+        raise QRecError('slopeone_predict: the item and user rows hold different numbers of ratings')
+    _f64_vec('slopeone_predict: item_vals', item_vals, item_users.shape[0])
+    _f64_vec('slopeone_predict: user_vals', user_vals, user_items.shape[0])
+    _f64_vec('slopeone_predict: item_means', item_means, n_items)
+    _f64_vec('slopeone_predict: user_means', user_means, n_users)
+    _knn_queries('slopeone_predict', test_items, n_items)
+    _knn_sorted(item_rowptr, item_users, max(n_users, 1))
+    Q, L = test_items.shape[0], line_qpos.shape[0]
+    if line_qpos.dtype != i32 or line_user.dtype != i32 or line_user.shape != (L,):
+        raise QRecError('slopeone_predict: line_qpos and line_user must be int32 of one length')
+    if L and (int(line_qpos.min()) < 0 or int(line_qpos.max()) >= Q):
+        raise QRecError('slopeone_predict: a line position is outside [0, %d)' % Q)
+    if L and (int(line_user.min()) < -1 or int(line_user.max()) >= n_users):
+        raise QRecError('slopeone_predict: a user is outside [0, %d) and not -1 (cold)' % n_users)
+    dev = item_users.device
+    line_out = torch.argsort(line_qpos.to(i64), stable=True)
+    line_rowptr = torch.zeros(Q + 1, dtype=i64, device=dev)
+    line_rowptr[1:] = torch.cumsum(torch.bincount(line_qpos.to(i64), minlength=Q), 0)
+    by_item_user = line_user[line_out].contiguous()
+    pred = torch.empty(L, dtype=f64, device=dev)
+    status = torch.empty(L, dtype=i32, device=dev)
+    check(lib.qrec_slopeone_predict_f64(_dev(item_rowptr, i64, 'item_rowptr'), _dev(item_users, i32, 'item_users'),
+                                        _dev(item_vals, f64, 'item_vals'), _dev(item_means, f64, 'item_means'),
+                                        _dev(user_rowptr, i64, 'user_rowptr'), _dev(user_items, i32, 'user_items'),
+                                        _dev(user_vals, f64, 'user_vals'), _dev(user_means, f64, 'user_means'),
+                                        float(global_mean), n_items, _dev(test_items, i32, 'test_items'), Q,
+                                        line_rowptr.data_ptr(), by_item_user.data_ptr(), line_out.data_ptr(),
+                                        pred.data_ptr(), status.data_ptr(), int(max_ctas), _stream()),
+          'qrec_slopeone_predict_f64')
+    return pred, status

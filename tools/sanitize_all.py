@@ -204,6 +204,29 @@ def main():
                            dev(E.als_row_order(sq_rp.cpu().numpy())), asum_out=torch.empty_like(A_sq))
         torch.cuda.synchronize()
         print('sanitize_all: + K14, launched', E.launch_count(), 'kernels')
+        # K15 (UserKNN / ItemKNN / SlopeOne): neighbour lists of every metric over the user rows (cold queries
+        # included), K past the candidate lists, the predictions, and SlopeOne's fused launch on one CTA and on many
+        up = np.unique(np.stack([u, i]), axis=1)                                 # distinct (user, item), user-major
+        rp_h = np.concatenate([[0], np.bincount(up[0], minlength=nu).cumsum()]).astype(np.int64)
+        krp, kcol = dev(rp_h), dev(up[1].astype(np.int32))
+        kv = dev((np.arange(up.shape[1]) % 9 + 1).astype(np.float64) / 2)
+        km = dev(np.bincount(up[0], weights=kv.cpu().numpy(), minlength=nu) / np.maximum(np.diff(rp_h), 1))
+        kq = dev(np.concatenate([np.arange(0, nu, 7), [-1, -1]]).astype(np.int32))
+        for metric in (0, 1, 2):
+            ksq = dev(E.knn_squares(rp_h, kv.cpu().numpy(), km.cpu().numpy(), metric))
+            for K in (20, nu + 5):
+                out = E.knn_neighbours(krp, kcol, kv, ksq, km, ni, kq, metric, K)
+            lq = dev(np.arange(kq.shape[0], dtype=np.int32))
+            E.knn_predict(krp, *E.knn_sorted_view(krp, kcol, kv), km, 3.0, kq, *out, lq, dev(np.full(kq.shape[0], 1, np.int32)), True)
+        ikv = torch.full((icol.shape[0],), 3.5, dtype=torch.float64, device='cuda')
+        ikm = torch.full((ni,), 3.5, dtype=torch.float64, device='cuda')
+        titems = dev(np.concatenate([np.arange(0, ni, 5), [-1]]).astype(np.int32))
+        for c in (1, 0):
+            E.slopeone_predict(irp, icol, ikv, ikm, krp, kcol, kv, km, 3.0, titems,
+                               dev((np.arange(300) % titems.shape[0]).astype(np.int32)),
+                               dev((np.arange(300) % nu).astype(np.int32)), max_ctas=c)
+        torch.cuda.synchronize()
+        print('sanitize_all: + K15, launched', E.launch_count(), 'kernels')
 
 
 if __name__ == '__main__':
