@@ -601,7 +601,12 @@ int qrec_mf_order_prepare(int64_t n, const int32_t* u, const int32_t* i, int32_t
 int64_t qrec_mf_order_depth(int64_t n, const int32_t* u, const int32_t* i, int32_t num_users,
                             int32_t num_items);
 /* Parity mode: sequential-equivalent epoch (dataflow over row versions, see qrec_bpr_sgd_ordered_*).
- * ver_p[num_users], ver_q[num_items], ticket[1] must be zero on entry. */
+ * ver_p[num_users], ver_q[num_items], ticket[1] must be zero on entry.
+ * kind 3 is SoRec's trust-edge pass (model/rating/SoRec.py:42-60) on the tables (P, Z): entries are the
+ * edges (u, v) in relation-list order, r = weight*tuv, and reg_u / reg_i carry regS / regZ:
+ *   e = r - P[u].Z[v];  P[u] += lr*((regS*e)*Z[v]);  Z[v] += lr*((regS*e)*P[u](new) - regZ*Z[v](old));
+ *   loss += regS*e^2.
+ * Its wait arrays are qrec_mf_order_prepare(n, u, v, num_users, num_users, ...); it takes no bias vectors. */
 int qrec_mf_sgd_ordered_f64(int32_t kind, double* dev_P, double* dev_Q, int32_t d, int64_t n,
                             const int32_t* dev_u, const int32_t* dev_i, const double* dev_r,
                             const int32_t* dev_wait_u, const int32_t* dev_wait_i, int32_t* dev_ver_p,
@@ -633,6 +638,52 @@ int qrec_mf_predict_pairs_f32(const float* dev_P, const float* dev_Q, int32_t d,
 int qrec_mf_predict_pairs_f64(const double* dev_P, const double* dev_Q, int32_t d, int64_t n,
                               const int32_t* dev_u, const int32_t* dev_i, const double* dev_Bu,
                               const double* dev_Bi, double global_mean, double* dev_out, void* stream);
+
+/* =====================================================================================
+ * K16 -- RSTE's rating pass (model/rating/RSTE.py:20-64).  Entry (u, i) predicts
+ *   alpha*(P[u].Q[i]) + ((1-alpha) * sum_f w_f (P[f].Q[i])) / denom[u]    (P[u].Q[i] alone when denom[u] == 0)
+ * over u's followees f (f_rowptr[num_users+1] / f_cols / f_w, in the cleaned followee dict's order; a self-follow
+ * is allowed) and updates P[u], Q[i] with K9 kind 1's step on the error alpha*e; loss += e^2.
+ * denom[u] is the reference's np.array(weights).sum(), computed by the caller.  d: 1..256.
+ * ===================================================================================== */
+/* Wait numbers of an entry stream (host, one O(n + sum of the entries' out-degrees) pass):
+ *   wait_u[k] / wait_i[k]: earlier entries writing P[u[k]] / Q[i[k]];
+ *   wait_reads_u[k]: earlier entries reading P[u[k]] as a followee row (a self-follow is no such read);
+ *   pos_rowptr[num_users+1] / pos[n]: the entry positions of each user, ascending;
+ *   *depth: the longest dependency chain of the stream (n / depth = average parallel width).
+ * Rejects ids outside [0, num_users) x [0, num_items), a rowptr that does not start at 0 or falls, and a followee
+ * outside [0, num_users). */
+int qrec_rste_order_prepare(int64_t n, const int32_t* u, const int32_t* i, int32_t num_users, int32_t num_items,
+                            const int64_t* f_rowptr, const int32_t* f_cols, int32_t* wait_u, int32_t* wait_i,
+                            int32_t* wait_reads_u, int64_t* pos_rowptr, int32_t* pos, int64_t* depth);
+/* Sequential-equivalent epoch over the entries in array order (dataflow over row versions and read counts, see
+ * rste_kernels.cu).  ver_p[num_users], ver_q[num_items], reads_p[num_users], ticket[1] must be zero on entry.
+ * The result does not depend on n_warps (0 = fill the GPU). */
+int qrec_rste_sgd_ordered_f64(double* dev_P, double* dev_Q, int32_t d, int64_t n, const int32_t* dev_u,
+                              const int32_t* dev_i, const double* dev_r, const int32_t* dev_wait_u,
+                              const int32_t* dev_wait_i, const int32_t* dev_wait_reads_u,
+                              const int64_t* dev_pos_rowptr, const int32_t* dev_pos, const int64_t* dev_f_rowptr,
+                              const int32_t* dev_f_cols, const double* dev_f_w, const double* dev_denom,
+                              int32_t* dev_ver_p, int32_t* dev_ver_q, int32_t* dev_reads_p,
+                              unsigned long long* dev_ticket, double lr, double reg_u, double reg_i, double alpha,
+                              double* dev_loss, int32_t n_warps, void* stream);
+int qrec_rste_sgd_ordered_f32(float* dev_P, float* dev_Q, int32_t d, int64_t n, const int32_t* dev_u,
+                              const int32_t* dev_i, const float* dev_r, const int32_t* dev_wait_u,
+                              const int32_t* dev_wait_i, const int32_t* dev_wait_reads_u,
+                              const int64_t* dev_pos_rowptr, const int32_t* dev_pos, const int64_t* dev_f_rowptr,
+                              const int32_t* dev_f_cols, const float* dev_f_w, const float* dev_denom,
+                              int32_t* dev_ver_p, int32_t* dev_ver_q, int32_t* dev_reads_p,
+                              unsigned long long* dev_ticket, float lr, float reg_u, float reg_i, float alpha,
+                              double* dev_loss, int32_t n_warps, void* stream);
+/* out[k] = the blend above for the known pair (u[k], i[k]) (RSTE's predictForRating), one warp per pair. */
+int qrec_rste_predict_pairs_f64(const double* dev_P, const double* dev_Q, int32_t d, int64_t n, const int32_t* dev_u,
+                                const int32_t* dev_i, const int64_t* dev_f_rowptr, const int32_t* dev_f_cols,
+                                const double* dev_f_w, const double* dev_denom, double alpha, double* dev_out,
+                                void* stream);
+int qrec_rste_predict_pairs_f32(const float* dev_P, const float* dev_Q, int32_t d, int64_t n, const int32_t* dev_u,
+                                const int32_t* dev_i, const int64_t* dev_f_rowptr, const int32_t* dev_f_cols,
+                                const float* dev_f_w, const float* dev_denom, float alpha, float* dev_out,
+                                void* stream);
 
 /* =====================================================================================
  * K10 -- WRMF (implicit-feedback ALS, model/ranking/WRMF.py:19-61).  A half-epoch solves every row of one

@@ -80,6 +80,14 @@ SIGNATURES = {
                                         C.c_float, vp, vp, C.c_float, C.c_float, vp, C.c_int64, vp]),
     'qrec_mf_predict_pairs_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_float, vp, vp]),
     'qrec_mf_predict_pairs_f64': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_double, vp, vp]),
+    'qrec_rste_order_prepare': (C.c_int, [C.c_int64, c_i32p, c_i32p, C.c_int32, C.c_int32, c_i64p, c_i32p, c_i32p,
+                                          c_i32p, c_i32p, c_i64p, c_i32p, c_i64p]),
+    'qrec_rste_sgd_ordered_f64': (C.c_int, [vp, vp, C.c_int32, C.c_int64] + [vp] * 16 +
+                                  [C.c_double] * 4 + [vp, C.c_int32, vp]),
+    'qrec_rste_sgd_ordered_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64] + [vp] * 16 +
+                                  [C.c_float] * 4 + [vp, C.c_int32, vp]),
+    'qrec_rste_predict_pairs_f64': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_double, vp, vp]),
+    'qrec_rste_predict_pairs_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp]),
     'qrec_als_gram_workspace_bytes': (C.c_int64, [C.c_int64, C.c_int32]),
     'qrec_als_gram_f32': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),
     'qrec_als_gram_f64': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),

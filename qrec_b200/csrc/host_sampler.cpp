@@ -356,4 +356,56 @@ int qrec_mf_order_prepare(int64_t n, const int32_t* u, const int32_t* i, int32_t
   return QREC_OK;
 }
 
+// RSTE's rating pass (model/rating/RSTE.py:20-64): entry (u, i) reads P[u], Q[i] and the followee rows P[f]
+// (f_rowptr / f_cols, a CSR over users) and writes P[u], Q[i].  One pass, O(n + sum of the entries' out-degrees).
+int qrec_rste_order_prepare(int64_t n, const int32_t* u, const int32_t* i, int32_t num_users, int32_t num_items,
+                            const int64_t* f_rowptr, const int32_t* f_cols, int32_t* wait_u, int32_t* wait_i,
+                            int32_t* wait_reads_u, int64_t* pos_rowptr, int32_t* pos, int64_t* depth) {
+  QREC_REQUIRE(num_users >= 0 && num_items >= 0, "qrec_rste_order_prepare: bad sizes");
+  QREC_REQUIRE(n >= 0 && n < (int64_t(1) << 31), "qrec_rste_order_prepare: n=%lld outside [0, 2^31)", (long long)n);
+  QREC_REQUIRE(f_rowptr && pos_rowptr && depth, "qrec_rste_order_prepare: null pointer");
+  QREC_REQUIRE(n == 0 || (u && i && wait_u && wait_i && wait_reads_u && pos), "qrec_rste_order_prepare: null pointer");
+  QREC_REQUIRE(f_rowptr[0] == 0, "qrec_rste_order_prepare: followee rowptr must start at 0");
+  for (int32_t r = 0; r < num_users; ++r)
+    QREC_REQUIRE(f_rowptr[r + 1] >= f_rowptr[r], "qrec_rste_order_prepare: followee rowptr falls at user %d", r);
+  const int64_t nnz = f_rowptr[num_users];
+  QREC_REQUIRE(nnz == 0 || f_cols, "qrec_rste_order_prepare: null followee list");
+  for (int64_t j = 0; j < nnz; ++j)
+    QREC_REQUIRE(f_cols[j] >= 0 && f_cols[j] < num_users, "qrec_rste_order_prepare: followee %lld out of range",
+                 (long long)j);
+  for (int64_t k = 0; k < n; ++k)
+    QREC_REQUIRE(u[k] >= 0 && u[k] < num_users && i[k] >= 0 && i[k] < num_items,
+                 "qrec_rste_order_prepare: id out of range at entry %lld", (long long)k);
+  // writes / foreign reads counted so far, and the dependency level of the last write / latest read of each row
+  std::vector<int32_t> cu((size_t)num_users, 0), cq((size_t)num_items, 0), cr((size_t)num_users, 0);
+  std::vector<int64_t> lw((size_t)num_users, 0), lr((size_t)num_users, 0), lq((size_t)num_items, 0);
+  int64_t deep = 0;
+  for (int64_t k = 0; k < n; ++k) {
+    const int32_t uu = u[k], ii = i[k];
+    wait_u[k] = cu[uu]++;
+    wait_i[k] = cq[ii]++;
+    wait_reads_u[k] = cr[uu];
+    int64_t lv = lw[uu] > lr[uu] ? lw[uu] : lr[uu];
+    if (lq[ii] > lv) lv = lq[ii];
+    for (int64_t j = f_rowptr[uu]; j < f_rowptr[uu + 1]; ++j)
+      if (f_cols[j] != uu && lw[f_cols[j]] > lv) lv = lw[f_cols[j]];
+    ++lv;
+    for (int64_t j = f_rowptr[uu]; j < f_rowptr[uu + 1]; ++j) {
+      const int32_t f = f_cols[j];
+      if (f == uu) continue;
+      ++cr[f];
+      if (lv > lr[f]) lr[f] = lv;
+    }
+    lw[uu] = lq[ii] = lv;
+    if (lv > deep) deep = lv;
+  }
+  *depth = deep;
+  // entry positions by user, ascending: rows of the CSR are the users' write counts (cu)
+  pos_rowptr[0] = 0;
+  for (int32_t r = 0; r < num_users; ++r) pos_rowptr[r + 1] = pos_rowptr[r] + cu[r];
+  std::vector<int64_t> fill(pos_rowptr, pos_rowptr + num_users);
+  for (int64_t k = 0; k < n; ++k) pos[fill[u[k]]++] = (int32_t)k;
+  return QREC_OK;
+}
+
 }  // extern "C"

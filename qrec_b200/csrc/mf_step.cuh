@@ -4,6 +4,9 @@
 //   kind 0  BasicMF.py:22-23   P[u] += (lr*e)*q ;           Q[i] += (lr*e)*P[u]
 //   kind 1  PMF.py:21-22       P[u] += lr*(e*q - regU*p) ;  Q[i] += lr*(e*P[u] - regI*q)
 //   kind 2  SVD.py:27-30,88    kind 1 + biases; prediction = ((dot + mean) + Bi[i]) + Bu[u]
+//   kind 3  SoRec.py:42-60     one trust edge (u, v) on the tables (P, Z); the "rating" is weight*tuv, regS and
+//                              regZ travel in the reg_u / reg_i slots and g = regS*e:
+//                              P[u] += lr*(g*z) ;  Z[v] += lr*(g*P[u] - regZ*z) ;  loss += regS*e^2
 #pragma once
 
 namespace qrec {
@@ -20,16 +23,32 @@ __device__ __forceinline__ T mf_prediction(T dot, T global_mean, T bi, T bu) {
   return KIND == 2 ? mf_add(mf_add(mf_add(dot, global_mean), bi), bu) : dot;
 }
 
-// one component of both rows; g = lr*err (kind 0 only)
+// the scalar the kernels hand to mf_update_parity as g: lr*err for kind 0, regS*err for kind 3 (unused otherwise)
+template <typename T, int KIND>
+__device__ __forceinline__ T mf_step_scale(T err, T lr, T reg_u) {
+  return KIND == 3 ? mf_mul(reg_u, err) : mf_mul(lr, err);
+}
+
+// one component of both rows; g = mf_step_scale(err, lr, reg_u) (kinds 0 and 3)
 template <typename T, int KIND>
 __device__ __forceinline__ void mf_update_parity(T p, T q, T err, T g, T lr, T reg_u, T reg_i, T& pn, T& qn) {
   if (KIND == 0) {
     pn = mf_add(p, mf_mul(g, q));
     qn = mf_add(q, mf_mul(g, pn));
+  } else if (KIND == 3) {
+    pn = mf_add(p, mf_mul(lr, mf_mul(g, q)));
+    qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(g, pn), mf_mul(reg_i, q))));
   } else {
     pn = mf_add(p, mf_mul(lr, mf_sub(mf_mul(err, q), mf_mul(reg_u, p))));
     qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(err, pn), mf_mul(reg_i, q))));
   }
+}
+
+// the entry's term of the epoch loss: e^2, regS*e^2 for a trust edge (kind 3)
+template <typename T, int KIND>
+__device__ __forceinline__ double mf_loss_term(T err, T reg_u) {
+  const double sq = (double)err * (double)err;
+  return KIND == 3 ? (double)reg_u * sq : sq;
 }
 
 template <typename T>

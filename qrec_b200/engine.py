@@ -917,6 +917,7 @@ def mask_rated(scores, users, rowptr, cols, value=0.0):
 # K9: rating-prediction MF family (kind 0 BasicMF, 1 PMF, 2 SVD)
 # ---------------------------------------------------------------------------------------------
 MF_KINDS = {'BasicMF': 0, 'PMF': 1, 'SVD': 2}
+SOREC_EDGES = 3    # kind 3: SoRec's trust-edge pass on (P, Z), regS / regZ in the reg_u / reg_i slots
 
 
 def _opt(t, dtype, name):
@@ -927,6 +928,8 @@ def mf_sgd_ordered(kind, P, Q, u, i, r, wu, wi, lr, reg_u, reg_i, loss, Bu=None,
                    global_mean=0.0, n_warps=0):
     """Parity mode: sequential-equivalent pass over the entries (u, i, r) in array order."""
     torch = _torch()
+    if kind == SOREC_EDGES:
+        _sorec_edge_checks(P, Q, u, i, r, wu, wi, Bu, Bi)
     f64 = P.dtype == torch.float64
     dt = torch.float64 if f64 else torch.float32
     d = P.shape[1]
@@ -960,6 +963,31 @@ def mf_sgd_batch(kind, P, Q, u, i, r, lr, reg_u, reg_i, loss, Bu=None, Bi=None, 
     return loss
 
 
+def _sorec_edge_checks(P, Z, u, v, r, wu, wv, Bu, Bi):
+    """QRecError on what kind 3 (SoRec's edge pass on the tables (P, Z)) cannot take."""
+    torch = _torch()
+    if Bu is not None or Bi is not None:
+        raise QRecError('mf_sgd_ordered: kind 3 (SoRec edges) takes no bias vectors')
+    if P.dtype not in (torch.float32, torch.float64) or Z.dtype != P.dtype:
+        raise QRecError('mf_sgd_ordered: P and Z must be float32 or float64 tables of one dtype')
+    if P.dim() != 2 or Z.dim() != 2 or Z.shape[1] != P.shape[1]:
+        raise QRecError('mf_sgd_ordered: P and Z must be 2-D tables of one width')
+    if not 1 <= P.shape[1] <= 256:
+        raise QRecError('mf_sgd_ordered: d=%d unsupported (1..256)' % P.shape[1])
+    n = u.shape[0]
+    if any(t.dim() != 1 or t.shape[0] != n for t in (v, r, wu, wv)):
+        raise QRecError('mf_sgd_ordered: u, v, r and the wait arrays must all hold %d entries' % n)
+    if r.dtype != P.dtype:
+        raise QRecError('mf_sgd_ordered: r must be %s, got %s' % (P.dtype, r.dtype))
+    _ids_below(u, P.shape[0], 'mf_sgd_ordered: an edge source is outside [0, %d)')
+    _ids_below(v, Z.shape[0], 'mf_sgd_ordered: an edge target is outside [0, %d)')
+
+
+def _ids_below(ids, bound, message):
+    if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= bound):
+        raise QRecError(message % bound)
+
+
 def mf_predict_pairs(P, Q, u, i, Bu=None, Bi=None, global_mean=0.0, out=None):
     """out[k] = P[u[k]].Q[i[k]] (+ global_mean + Bi + Bu): predictForRating for known pairs."""
     torch = _torch()
@@ -971,6 +999,121 @@ def mf_predict_pairs(P, Q, u, i, Bu=None, Bi=None, global_mean=0.0, out=None):
     check(fn(_dev(P, dt, 'P'), _dev(Q, dt, 'Q'), P.shape[1], u.shape[0], _dev(u, torch.int32, 'u'),
              _dev(i, torch.int32, 'i'), _opt(Bu, dt, 'Bu'), _opt(Bi, dt, 'Bi'), float(global_mean),
              _dev(out, dt, 'out'), _stream()), 'qrec_mf_predict_pairs')
+    return out
+
+
+# ---------------------------------------------------------------------------------------------
+# K16: RSTE's rating pass -- the ordered epoch and test-pair prediction over the followee CSR
+# ---------------------------------------------------------------------------------------------
+def rste_order_prepare(u, i, num_users, num_items, f_rowptr, f_cols):
+    """Wait numbers of an RSTE entry stream (host, one pass): (wait_u, wait_i, wait_reads_u, pos_rowptr, pos, depth).
+    pos_rowptr / pos: each user's entry positions, ascending; depth: the stream's longest dependency chain."""
+    u = np.ascontiguousarray(u, dtype=np.int32)
+    i = np.ascontiguousarray(i, dtype=np.int32)
+    f_rowptr = np.ascontiguousarray(f_rowptr, dtype=np.int64)
+    f_cols = np.ascontiguousarray(f_cols, dtype=np.int32)
+    n = u.shape[0]
+    if i.shape[0] != n:
+        raise QRecError('rste_order_prepare: u and i differ in length')
+    if f_rowptr.shape != (int(num_users) + 1,):
+        raise QRecError('rste_order_prepare: the followee rowptr needs %d entries' % (int(num_users) + 1))
+    if f_rowptr[-1] != f_cols.shape[0]:
+        raise QRecError('rste_order_prepare: the followee rowptr ends at %d, not at len(f_cols) = %d'
+                        % (f_rowptr[-1], f_cols.shape[0]))
+    wu, wi, wr = (np.empty(n, np.int32) for _ in range(3))
+    pos_rowptr, pos = np.empty(int(num_users) + 1, np.int64), np.empty(n, np.int32)
+    depth = np.zeros(1, np.int64)
+    check(lib.qrec_rste_order_prepare(n, _i32p(u), _i32p(i), int(num_users), int(num_items), _i64p(f_rowptr),
+                                      _i32p(f_cols), _i32p(wu), _i32p(wi), _i32p(wr), _i64p(pos_rowptr), _i32p(pos),
+                                      _i64p(depth)), 'qrec_rste_order_prepare')
+    return wu, wi, wr, pos_rowptr, pos, int(depth[0])
+
+
+def _rste_checks(name, P, Q, f_rowptr, f_cols, f_w, denom, typed):
+    """QRecError unless (P, Q) are tables of one float dtype and width 1..256, the followee CSR and denom describe P's
+    users, and every tensor of `typed` ((tensor, dtype, name) triples, the entry arrays) has its dtype.  Shapes and
+    dtypes are checked first, then that every tensor is a contiguous CUDA tensor, then the contents: the CSR's rowptr
+    rises from 0 to len(f_cols) and every followee id names a user.  Returns the CUDA tensors' pointers."""
+    torch = _torch()
+    if P.dtype not in (torch.float32, torch.float64) or Q.dtype != P.dtype:
+        raise QRecError('%s: P and Q must be float32 or float64 tables of one dtype' % name)
+    if P.dim() != 2 or Q.dim() != 2 or Q.shape[1] != P.shape[1]:
+        raise QRecError('%s: P and Q must be 2-D tables of one width' % name)
+    if not 1 <= P.shape[1] <= 256:
+        raise QRecError('%s: d=%d unsupported (1..256)' % (name, P.shape[1]))
+    U = P.shape[0]
+    if denom.dim() != 1 or denom.shape[0] != U:
+        raise QRecError('%s: denom needs one entry per user (%d), got %d' % (name, U, denom.numel()))
+    if f_rowptr.dim() != 1 or f_rowptr.shape[0] != U + 1:
+        raise QRecError('%s: the followee rowptr needs %d entries' % (name, U + 1))
+    if f_cols.dim() != 1 or f_w.dim() != 1 or f_w.shape[0] != f_cols.shape[0]:
+        raise QRecError('%s: followee ids and weights differ in length' % name)
+    tensors = [(P, P.dtype, 'P'), (Q, P.dtype, 'Q'), (f_rowptr, torch.int64, 'f_rowptr'), (f_cols, torch.int32, 'f_cols'),
+               (f_w, P.dtype, 'f_w'), (denom, P.dtype, 'denom')] + list(typed)
+    for t, dt, tname in tensors:
+        if t.dtype != dt:
+            raise QRecError('%s: %s must be %s, got %s' % (name, tname, dt, t.dtype))
+    ptrs = {tname: _dev(t, dt, '%s: %s' % (name, tname)) for t, dt, tname in tensors}
+    if int(f_rowptr[0]) != 0 or int(f_rowptr[-1]) != f_cols.shape[0] or bool((f_rowptr[1:] < f_rowptr[:-1]).any()):
+        raise QRecError('%s: the followee rowptr must rise from 0 to len(f_cols) = %d' % (name, f_cols.shape[0]))
+    _ids_below(f_cols, U, name + ': a followee is outside [0, %d)')
+    return ptrs
+
+
+def rste_sgd_ordered(P, Q, u, i, r, wu, wi, wr, pos_rowptr, pos, f_rowptr, f_cols, f_w, denom, lr, reg_u, reg_i,
+                     alpha, loss, n_warps=0):
+    """RSTE's rating pass over the entries (u, i, r) in array order, sequential-equivalent, in place on P and Q
+    (float64 or float32).  wu / wi / wr / pos_rowptr / pos: rste_order_prepare of the same stream and followee CSR
+    (f_rowptr int64, f_cols int32, f_w the weights); denom[u]: the sum of u's weights.  loss (float64) += sum e^2."""
+    torch = _torch()
+    name = 'rste_sgd_ordered'
+    n = u.shape[0]
+    if any(t.dim() != 1 or t.shape[0] != n for t in (u, i, r, wu, wi, wr, pos)):
+        raise QRecError('%s: u, i, r, the wait arrays and pos must all hold %d entries' % (name, n))
+    if pos_rowptr.dim() != 1 or pos_rowptr.shape[0] != P.shape[0] + 1:
+        raise QRecError('%s: pos_rowptr needs %d entries' % (name, P.shape[0] + 1))
+    if loss.numel() < 1:
+        raise QRecError('%s: loss needs one entry' % name)
+    i32 = torch.int32
+    ptr = _rste_checks(name, P, Q, f_rowptr, f_cols, f_w, denom,
+                       [(u, i32, 'u'), (i, i32, 'i'), (r, P.dtype, 'r'), (wu, i32, 'wu'), (wi, i32, 'wi'),
+                        (wr, i32, 'wr'), (pos_rowptr, torch.int64, 'pos_rowptr'), (pos, i32, 'pos'),
+                        (loss, torch.float64, 'loss')])
+    _ids_below(u, P.shape[0], name + ': a user id is outside [0, %d)')
+    _ids_below(i, Q.shape[0], name + ': an item id is outside [0, %d)')
+    # the kernel bisects pos[pos_rowptr[f] .. pos_rowptr[f+1]): the rows must tile pos
+    if int(pos_rowptr[0]) != 0 or int(pos_rowptr[-1]) != n or bool((pos_rowptr[1:] < pos_rowptr[:-1]).any()):
+        raise QRecError('%s: pos_rowptr must rise from 0 to len(pos) = %d' % (name, n))
+    ver_p = torch.zeros(P.shape[0], dtype=i32, device=P.device)
+    reads_p = torch.zeros(P.shape[0], dtype=i32, device=P.device)
+    ver_q = torch.zeros(Q.shape[0], dtype=i32, device=P.device)
+    ticket = torch.zeros(1, dtype=torch.int64, device=P.device)
+    fn = lib.qrec_rste_sgd_ordered_f64 if P.dtype == torch.float64 else lib.qrec_rste_sgd_ordered_f32
+    check(fn(ptr['P'], ptr['Q'], P.shape[1], n, ptr['u'], ptr['i'], ptr['r'], ptr['wu'], ptr['wi'], ptr['wr'],
+             ptr['pos_rowptr'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'], ptr['f_w'], ptr['denom'], ver_p.data_ptr(),
+             ver_q.data_ptr(), reads_p.data_ptr(), ticket.data_ptr(), float(lr), float(reg_u), float(reg_i),
+             float(alpha), ptr['loss'], int(n_warps), _stream()), 'qrec_rste_sgd_ordered')
+    return loss
+
+
+def rste_predict_pairs(P, Q, u, i, f_rowptr, f_cols, f_w, denom, alpha, out=None):
+    """RSTE's predictForRating for the known pairs (u[k], i[k]): alpha*P[u].Q[i] + ((1-alpha)*sum_f w_f P[f].Q[i]) /
+    denom[u], or P[u].Q[i] when denom[u] == 0."""
+    torch = _torch()
+    name = 'rste_predict_pairs'
+    if u.dim() != 1 or i.dim() != 1 or i.shape[0] != u.shape[0]:
+        raise QRecError('%s: u and i differ in length' % name)
+    if out is not None and out.shape != u.shape:
+        raise QRecError('%s: out needs %d entries' % (name, u.shape[0]))
+    typed = [(u, torch.int32, 'u'), (i, torch.int32, 'i')] + ([(out, P.dtype, 'out')] if out is not None else [])
+    ptr = _rste_checks(name, P, Q, f_rowptr, f_cols, f_w, denom, typed)
+    _ids_below(u, P.shape[0], name + ': a user id is outside [0, %d)')
+    _ids_below(i, Q.shape[0], name + ': an item id is outside [0, %d)')
+    if out is None:
+        out = torch.empty(u.shape[0], dtype=P.dtype, device=P.device)
+    fn = lib.qrec_rste_predict_pairs_f64 if P.dtype == torch.float64 else lib.qrec_rste_predict_pairs_f32
+    check(fn(ptr['P'], ptr['Q'], P.shape[1], u.shape[0], ptr['u'], ptr['i'], ptr['f_rowptr'], ptr['f_cols'],
+             ptr['f_w'], ptr['denom'], float(alpha), out.data_ptr(), _stream()), 'qrec_rste_predict_pairs')
     return out
 
 

@@ -1,0 +1,126 @@
+#!/usr/bin/env python
+"""SoRec's trust-edge pass (K9 kind 3) and RSTE's rating pass (K16), in float64 as the parity path runs them, on the
+two synthetic shapes of bench_serec.py (qrec_b200.synthetic, Zipf-skewed item popularity):
+  * lastfm-like: 1,892 users x 17,632 items, 40 entries per user, d = 20;
+  * yelp2018-like: 31,668 users x 38,048 items, 36 entries per user, d = 64.
+Followee counts are bench_serec.py's draw (a fifth of the users follow nobody, the rest a log-normal count); the
+followees are drawn uniformly among the other users, weight 1.  The entry stream and the edge list are shuffled.
+
+Timed with CUDA events, one launch per pass: SoRec's edge pass, RSTE's rating pass, and K9 PMF (kind 1) on the same
+entry stream, so that the cost of the followee reads shows.  The host wait numbers are prepared beforehand.  The passes
+are launched through the C entry points: the engine wrappers' input checks read device values back (ids, CSR bounds),
+which would put host round trips inside the timed window of some passes and not others.  Each pass zeroes its row
+counters and ticket inside the window (two memsets), as every ordered launch needs.  One JSON line per shape with the
+milliseconds per pass, each pass's dependency-chain depth, entries per second, and the card's name and power limit."""
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from bench_expomf import card, timed   # noqa: E402
+from bench_serec import degrees        # noqa: E402
+
+SHAPES = (('lastfm', 1892, 17632, 40, 20, 3), ('yelp2018', 31668, 38048, 36, 64, 2))   # name, U, I, per user, d, reps
+
+
+def followees(U, seed=3):
+    rng = np.random.default_rng(seed)
+    deg = degrees(U)
+    rowptr = np.zeros(U + 1, np.int64)
+    rowptr[1:] = np.cumsum(deg)
+    cols = np.empty(rowptr[-1], np.int32)
+    for a in range(U):
+        pick = rng.choice(U - 1, size=int(deg[a]), replace=False)
+        cols[rowptr[a]:rowptr[a + 1]] = pick + (pick >= a)             # anyone but a
+    return rowptr, cols
+
+
+def main():
+    import torch
+    from qrec_b200 import engine as E, synthetic
+    assert torch.cuda.is_available(), 'bench_social_rating needs a GPU'
+    torch.cuda.set_device(0)
+    name, limit = card(torch)
+    f64, dev = torch.float64, torch.device('cuda')
+    for label, U, I, per_user, D, reps in SHAPES:
+        data = synthetic.make_interactions(U, I, per_user, zipf=True)
+        rng = np.random.default_rng(1)
+        perm = rng.permutation(data['u'].shape[0])
+        u = data['u'].cpu().numpy().astype(np.int32)[perm]
+        i = data['i'].cpu().numpy().astype(np.int32)[perm]
+        n = u.shape[0]
+        r = torch.from_numpy(rng.integers(1, 9, n) * 0.5).to(dev, f64)
+        rowptr, cols = followees(U)
+        w = np.ones(cols.shape[0])
+        denom = np.diff(rowptr).astype(np.float64)
+        social = (torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev), torch.from_numpy(w).to(dev),
+                  torch.from_numpy(denom).to(dev))
+        eu = np.repeat(np.arange(U, dtype=np.int32), np.diff(rowptr))
+        eperm = rng.permutation(eu.shape[0])
+        eu, ev = eu[eperm], cols[eperm]
+        g = torch.Generator(device='cuda').manual_seed(1)
+        P = torch.rand(U, D, device=dev, dtype=f64, generator=g) / 3
+        Q = torch.rand(I, D, device=dev, dtype=f64, generator=g) / 3
+        Z = torch.rand(U, D, device=dev, dtype=f64, generator=g) / 10
+        loss = torch.zeros(1, dtype=f64, device=dev)
+        du, di = torch.from_numpy(u).to(dev), torch.from_numpy(i).to(dev)
+
+        wu, wi, wr, pr, pos, rste_depth = E.rste_order_prepare(u, i, U, I, rowptr, cols)
+        rste_dev = [torch.from_numpy(a).to(dev) for a in (wu, wi, wr, pr, pos)]
+        mwu, mwi = (torch.from_numpy(a).to(dev) for a in E.mf_order_prepare(u, i, U, I))
+        pmf_depth = E.mf_order_depth(u, i, U, I)
+        ewu, ewv = (torch.from_numpy(a).to(dev) for a in E.mf_order_prepare(eu, ev, U, U))
+        edge_depth = E.mf_order_depth(eu, ev, U, U)
+        due, dve = torch.from_numpy(eu).to(dev), torch.from_numpy(ev).to(dev)
+        te = torch.rand(eu.shape[0], device=dev, dtype=f64, generator=g)
+
+        def width(m, depth):
+            return int(min(2368, max(64, 16 * m / max(1, depth))))
+
+        # raw launches (see the docstring); counters: ver_p | ver_q (or ver_z) | reads_p, and one ticket per pass
+        ptr = lambda t: t.data_ptr()                                    # noqa: E731
+        st = torch.cuda.current_stream().cuda_stream
+        rste_n, pmf_n, edge_n = width(n, rste_depth), width(n, pmf_depth), width(eu.shape[0], edge_depth)
+        rste_cnt, pmf_cnt, edge_cnt = (torch.zeros(c, dtype=torch.int32, device=dev) for c in (2 * U + I, U + I, 2 * U))
+        tickets = torch.zeros(3, dtype=torch.int64, device=dev)
+
+        def rste():
+            rste_cnt.zero_(); tickets[0:1].zero_()
+            E.check(E.lib.qrec_rste_sgd_ordered_f64(
+                ptr(P), ptr(Q), D, n, ptr(du), ptr(di), ptr(r), *(ptr(a) for a in rste_dev), *(ptr(a) for a in social),
+                ptr(rste_cnt), ptr(rste_cnt) + 4 * U, ptr(rste_cnt) + 4 * (U + I), ptr(tickets), 1e-3, 1e-3, 1e-3, 0.6,
+                ptr(loss), rste_n, st), 'qrec_rste_sgd_ordered_f64')
+
+        def pmf():
+            pmf_cnt.zero_(); tickets[1:2].zero_()
+            E.check(E.lib.qrec_mf_sgd_ordered_f64(
+                1, ptr(P), ptr(Q), D, n, ptr(du), ptr(di), ptr(r), ptr(mwu), ptr(mwi), ptr(pmf_cnt),
+                ptr(pmf_cnt) + 4 * U, ptr(tickets) + 8, 1e-3, 1e-3, 1e-3, None, None, 0.0, 0.0, ptr(loss), pmf_n, st),
+                'qrec_mf_sgd_ordered_f64')
+
+        def edges():
+            edge_cnt.zero_(); tickets[2:3].zero_()
+            E.check(E.lib.qrec_mf_sgd_ordered_f64(
+                E.SOREC_EDGES, ptr(P), ptr(Z), D, eu.shape[0], ptr(due), ptr(dve), ptr(te), ptr(ewu), ptr(ewv),
+                ptr(edge_cnt), ptr(edge_cnt) + 4 * U, ptr(tickets) + 16, 1e-3, 0.1, 0.1, None, None, 0.0, 0.0,
+                ptr(loss), edge_n, st), 'qrec_mf_sgd_ordered_f64')
+
+        for fn in (rste, pmf, edges):                                   # warm-up
+            fn()
+        t_rste, t_pmf, t_edges = timed(torch, rste, reps), timed(torch, pmf, reps), timed(torch, edges, reps)
+        print(json.dumps(dict(
+            shape=label, users=U, items=I, entries=n, d=D, dtype='float64', edges=int(eu.shape[0]),
+            followee_reads=int(np.diff(rowptr)[u].sum()), deg_mean=round(float(np.diff(rowptr).mean()), 2),
+            deg_max=int(np.diff(rowptr).max()),
+            ms_sorec_edge_pass=round(t_edges, 3), ms_rste_pass=round(t_rste, 3), ms_pmf_pass=round(t_pmf, 3),
+            depth_sorec_edges=edge_depth, depth_rste=rste_depth, depth_pmf=pmf_depth,
+            entries_per_s_sorec_edges=round(eu.shape[0] / (t_edges / 1e3)), entries_per_s_rste=round(n / (t_rste / 1e3)),
+            entries_per_s_pmf=round(n / (t_pmf / 1e3)), gpu=name, power_limit=limit)), flush=True)
+
+
+if __name__ == '__main__':
+    main()
