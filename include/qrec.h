@@ -606,7 +606,10 @@ int64_t qrec_mf_order_depth(int64_t n, const int32_t* u, const int32_t* i, int32
  * edges (u, v) in relation-list order, r = weight*tuv, and reg_u / reg_i carry regS / regZ:
  *   e = r - P[u].Z[v];  P[u] += lr*((regS*e)*Z[v]);  Z[v] += lr*((regS*e)*P[u](new) - regZ*Z[v](old));
  *   loss += regS*e^2.
- * Its wait arrays are qrec_mf_order_prepare(n, u, v, num_users, num_users, ...); it takes no bias vectors. */
+ * Its wait arrays are qrec_mf_order_prepare(n, u, v, num_users, num_users, ...); it takes no bias vectors.
+ * kind 4 is SocialMF's rating pass (model/rating/SocialMF.py:15-24): kind 1 on copies of both rows,
+ *   P[u] += lr*(e*Q[i] - regU*P[u]);  Q[i] += lr*(e*P[u](old) - regI*Q[i]);  loss += e^2.
+ * It takes no bias vectors either.  qrec_mf_sgd_batch_f32 takes kinds 0..2 only. */
 int qrec_mf_sgd_ordered_f64(int32_t kind, double* dev_P, double* dev_Q, int32_t d, int64_t n,
                             const int32_t* dev_u, const int32_t* dev_i, const double* dev_r,
                             const int32_t* dev_wait_u, const int32_t* dev_wait_i, int32_t* dev_ver_p,
@@ -684,6 +687,39 @@ int qrec_rste_predict_pairs_f32(const float* dev_P, const float* dev_Q, int32_t 
                                 const int32_t* dev_i, const int64_t* dev_f_rowptr, const int32_t* dev_f_cols,
                                 const float* dev_f_w, const float* dev_denom, float alpha, float* dev_out,
                                 void* stream);
+
+/* =====================================================================================
+ * K17 -- the trust-neighbourhood user pass of SocialMF (kind 0, model/rating/SocialMF.py:26-43) and SoReg (kind 1,
+ * model/rating/SoReg.py:54-72).  The users visit[0..n) in order (the reference's social.user restricted to training
+ * users, each at most once), each updating its own row of P from its followees f (f_rowptr[num_users+1] / f_cols /
+ * f_val, in the cleaned followee dict's order) and, for SoReg, its followers g (g_rowptr / g_cols / g_val, in the
+ * cleaned follower dict's order); a self-follow reads the row before the update:
+ *   kind 0 (f_val = weights, coef = regS):  fPred = sum_f w_f*P[f], denom = sum_f w_f (both from 0, in order);
+ *     when denom != 0:  rl = P[u] - fPred/denom;  P[u] -= (lr*regS)*rl;  loss += regS*(rl.rl).
+ *   kind 1 (f_val / g_val = Sim[u][.], coef = alpha):  f1 = sum_f Sim*(P[u]-P[f]), f2 = sum_g Sim*(P[u]-P[g]);
+ *     P[u] += lr*((-alpha)*(f1+f2));  loss += simSum after every followee, simSum += Sim*|P[u]-P[f]|^2.
+ * d: 1..256.
+ * ===================================================================================== */
+/* Schedule of a visiting order (host, one pass): pos[num_users] = each user's visit position, -1 when not visited;
+ * *depth = the longest chain of users each waiting for an earlier followee or follower (n / depth = average parallel
+ * width).  Rejects a visit outside [0, num_users) or repeated, a rowptr that does not start at 0, falls or does not
+ * end at its column count (f_nnz / g_nnz), and a column outside [0, num_users).  Built once per model. */
+int qrec_social_order_prepare(int64_t n, const int32_t* visit, int32_t num_users, const int64_t* f_rowptr,
+                              const int32_t* f_cols, int64_t f_nnz, const int64_t* g_rowptr, const int32_t* g_cols,
+                              int64_t g_nnz, int32_t* pos, int64_t* depth);
+/* Sequential-equivalent pass (one done flag per user, see social_pass_kernels.cu): user visit[k] waits for every
+ * followee and follower visited before k.  pos from qrec_social_order_prepare; done[num_users] and ticket[1] must be
+ * zero on entry.  g_val may be null for kind 0.  The result does not depend on n_warps (0 = fill the GPU). */
+int qrec_social_user_pass_f64(int32_t kind, double* dev_P, int32_t d, int64_t n, const int32_t* dev_visit,
+                              const int32_t* dev_pos, const int64_t* dev_f_rowptr, const int32_t* dev_f_cols,
+                              const double* dev_f_val, const int64_t* dev_g_rowptr, const int32_t* dev_g_cols,
+                              const double* dev_g_val, int32_t* dev_done, unsigned long long* dev_ticket, double lr,
+                              double coef, double* dev_loss, int32_t n_warps, void* stream);
+int qrec_social_user_pass_f32(int32_t kind, float* dev_P, int32_t d, int64_t n, const int32_t* dev_visit,
+                              const int32_t* dev_pos, const int64_t* dev_f_rowptr, const int32_t* dev_f_cols,
+                              const float* dev_f_val, const int64_t* dev_g_rowptr, const int32_t* dev_g_cols,
+                              const float* dev_g_val, int32_t* dev_done, unsigned long long* dev_ticket, float lr,
+                              float coef, double* dev_loss, int32_t n_warps, void* stream);
 
 /* =====================================================================================
  * K10 -- WRMF (implicit-feedback ALS, model/ranking/WRMF.py:19-61).  A half-epoch solves every row of one
@@ -880,6 +916,16 @@ int qrec_slopeone_predict_f64(const int64_t* dev_item_rowptr, const int32_t* dev
                               const int64_t* dev_line_rowptr, const int32_t* dev_line_user,
                               const int64_t* dev_line_out, double* dev_pred, int32_t* dev_status, int32_t max_ctas,
                               void* stream);
+/* SoReg's similarities of listed pairs (model/rating/SoReg.py:35-36): out[p] = (pcc(a[p], b[p]) + w[p]) / 2.0 with
+ * util/qmath.py's pearson_sp over the rows rowptr / cols / vals (insertion order), their squares sq ((x - mean)**2,
+ * as for qrec_knn_neighbours_f64) and means.  Row a's entries are walked in insertion order and each key is looked up
+ * by bisection in row b of the sorted view (sorted_cols ascending per row, sorted_vals / sorted_sq permuted alike).
+ * One thread per pair; bitwise reproducible. */
+int qrec_knn_pair_similarity_f64(const int64_t* dev_rowptr, const int32_t* dev_cols, const double* dev_vals,
+                                  const double* dev_sq, const double* dev_means, const int32_t* dev_sorted_cols,
+                                  const double* dev_sorted_vals, const double* dev_sorted_sq, int64_t n_pairs,
+                                  const int32_t* dev_a, const int32_t* dev_b, const double* dev_w, double* dev_out,
+                                  void* stream);
 
 #ifdef __cplusplus
 }

@@ -88,6 +88,12 @@ SIGNATURES = {
                                   [C.c_float] * 4 + [vp, C.c_int32, vp]),
     'qrec_rste_predict_pairs_f64': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_double, vp, vp]),
     'qrec_rste_predict_pairs_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp]),
+    'qrec_social_order_prepare': (C.c_int, [C.c_int64, c_i32p, C.c_int32, c_i64p, c_i32p, C.c_int64, c_i64p, c_i32p,
+                                            C.c_int64, c_i32p, c_i64p]),
+    'qrec_social_user_pass_f64': (C.c_int, [C.c_int32, vp, C.c_int32, C.c_int64] + [vp] * 10 +
+                                  [C.c_double] * 2 + [vp, C.c_int32, vp]),
+    'qrec_social_user_pass_f32': (C.c_int, [C.c_int32, vp, C.c_int32, C.c_int64] + [vp] * 10 +
+                                  [C.c_float] * 2 + [vp, C.c_int32, vp]),
     'qrec_als_gram_workspace_bytes': (C.c_int64, [C.c_int64, C.c_int32]),
     'qrec_als_gram_f32': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),
     'qrec_als_gram_f64': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),
@@ -109,6 +115,7 @@ SIGNATURES = {
                                           C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, vp]),
     'qrec_knn_predict_f64': (C.c_int, [vp, vp, vp, vp, C.c_double, vp, C.c_int32, vp, vp, vp, C.c_int64, vp, vp,
                                        C.c_int32, vp, vp, vp]),
+    'qrec_knn_pair_similarity_f64': (C.c_int, [vp] * 8 + [C.c_int64] + [vp] * 5),
     'qrec_slopeone_predict_f64': (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, C.c_double, C.c_int32, vp, C.c_int32, vp,
                                             vp, vp, vp, vp, C.c_int32, vp]),
     'qrec_svdpp_sgd_ordered_f64': (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, C.c_double,

@@ -408,4 +408,54 @@ int qrec_rste_order_prepare(int64_t n, const int32_t* u, const int32_t* i, int32
   return QREC_OK;
 }
 
+// The trust-neighbourhood user pass (K17, social_pass_kernels.cu) over the visiting order visit[0..n): pos[u] = the
+// position of user u in it, -1 when u is not visited; *depth = the longest chain of users each waiting for an earlier
+// followee or follower (f_* / g_*: the followee and follower CSRs over users, with f_nnz / g_nnz columns).
+int qrec_social_order_prepare(int64_t n, const int32_t* visit, int32_t num_users, const int64_t* f_rowptr,
+                              const int32_t* f_cols, int64_t f_nnz, const int64_t* g_rowptr, const int32_t* g_cols,
+                              int64_t g_nnz, int32_t* pos, int64_t* depth) {
+  QREC_REQUIRE(num_users >= 0 && n >= 0 && n <= num_users, "qrec_social_order_prepare: n=%lld, num_users=%d",
+               (long long)n, num_users);
+  QREC_REQUIRE(f_rowptr && g_rowptr && depth && (num_users == 0 || pos) && (n == 0 || visit),
+               "qrec_social_order_prepare: null pointer");
+  const int64_t* rowptrs[2] = {f_rowptr, g_rowptr};
+  const int32_t* colss[2] = {f_cols, g_cols};
+  const int64_t nnzs[2] = {f_nnz, g_nnz};
+  for (int t = 0; t < 2; ++t) {
+    const int64_t* rp = rowptrs[t];
+    QREC_REQUIRE(rp[0] == 0 && rp[num_users] == nnzs[t],
+                 "qrec_social_order_prepare: %s rowptr must run from 0 to %lld", t ? "follower" : "followee",
+                 (long long)nnzs[t]);
+    for (int32_t r = 0; r < num_users; ++r)
+      QREC_REQUIRE(rp[r + 1] >= rp[r], "qrec_social_order_prepare: %s rowptr falls at user %d",
+                   t ? "follower" : "followee", r);
+    QREC_REQUIRE(nnzs[t] == 0 || colss[t], "qrec_social_order_prepare: null column list");
+    for (int64_t j = 0; j < nnzs[t]; ++j)
+      QREC_REQUIRE(colss[t][j] >= 0 && colss[t][j] < num_users, "qrec_social_order_prepare: %s %lld out of range",
+                   t ? "follower" : "followee", (long long)j);
+  }
+  for (int32_t r = 0; r < num_users; ++r) pos[r] = -1;
+  for (int64_t k = 0; k < n; ++k) {
+    const int32_t uu = visit[k];
+    QREC_REQUIRE(uu >= 0 && uu < num_users, "qrec_social_order_prepare: visit %lld out of range", (long long)k);
+    QREC_REQUIRE(pos[uu] < 0, "qrec_social_order_prepare: user %d visited twice", uu);
+    pos[uu] = (int32_t)k;
+  }
+  std::vector<int64_t> level((size_t)num_users, 0);
+  int64_t deep = 0;
+  for (int64_t k = 0; k < n; ++k) {
+    const int32_t uu = visit[k];
+    int64_t lv = 0;
+    for (int t = 0; t < 2; ++t)
+      for (int64_t j = rowptrs[t][uu]; j < rowptrs[t][uu + 1]; ++j) {
+        const int32_t v = colss[t][j];
+        if (v != uu && pos[v] >= 0 && pos[v] < k && level[v] > lv) lv = level[v];
+      }
+    level[uu] = ++lv;
+    if (lv > deep) deep = lv;
+  }
+  *depth = deep;
+  return QREC_OK;
+}
+
 }  // extern "C"

@@ -22,6 +22,8 @@
 //     bisection in the neighbour's sorted row.
 //   * slopeone_predict_kernel -- one persistent CTA per test item: the item's diff / count row against every item is
 //     scattered into per-CTA scratch, then every test line of the item is served from it.
+//   * knn_pair_similarity_kernel -- one thread per listed pair (a, b): pcc(a, b) with a's row walked in insertion
+//     order and each key looked up by bisection in b's sorted row, then (pcc + w) / 2.0 (SoReg's similarity).
 //   Scratch is per CTA and O(rows + columns): no queries x rows table is ever formed.
 #include "common.h"
 #include "knn_step.cuh"
@@ -316,6 +318,36 @@ knn_predict_kernel(const long long* __restrict__ rowptr, const int* __restrict__
   }
 }
 
+// One thread per pair p: out[p] = (pcc(a[p], b[p]) + w[p]) / 2.0 (SoReg.py:35-36, util/qmath.py: pearson_sp).  Row a
+// is walked in insertion order (cols / vals / sq); each of its keys is looked up by bisection in row b of the sorted
+// view (scols / svals / ssq: the same rows with their columns ascending, values and squares in the same permutation).
+__global__ void __launch_bounds__(kThreads)
+knn_pair_similarity_kernel(const long long* __restrict__ rowptr, const int* __restrict__ cols,
+                           const double* __restrict__ vals, const double* __restrict__ sq,
+                           const double* __restrict__ means, const int* __restrict__ scols,
+                           const double* __restrict__ svals, const double* __restrict__ ssq, long long n_pairs,
+                           const int* __restrict__ pa, const int* __restrict__ pb, const double* __restrict__ w,
+                           double* __restrict__ out) {
+  for (long long p = blockIdx.x * (long long)kThreads + threadIdx.x; p < n_pairs;
+       p += (long long)gridDim.x * kThreads) {
+    const int a = pa[p], b = pb[p];
+    const double ma = means[a], mb = means[b];
+    const long long bb = rowptr[b], be = rowptr[b + 1];
+    KnnAcc acc{0.0, 0.0, 0.0, 0};
+    for (long long e = rowptr[a]; e < rowptr[a + 1]; ++e) {
+      const int x = cols[e];
+      long long lo = bb, hi = be;
+      while (lo < hi) {
+        const long long mid = (lo + hi) >> 1;
+        if (scols[mid] < x) lo = mid + 1; else hi = mid;
+      }
+      if (lo == be || scols[lo] != x) continue;
+      knn_add<kPearson>(acc, vals[e], sq[e], ma, svals[lo], ssq[lo], mb);
+    }
+    out[p] = __ddiv_rn(__dadd_rn(knn_similarity<kPearson>(acc), w[p]), 2.0);
+  }
+}
+
 __host__ __device__ inline size_t slopeone_scratch_stride(int n_items) {
   return (sizeof(KnnAcc) * (size_t)n_items + sizeof(int) * (size_t)n_items + 255) & ~(size_t)255;
 }
@@ -438,6 +470,20 @@ int qrec_knn_predict_f64(const int64_t* rowptr, const int32_t* sorted_cols, cons
   knn_predict_kernel<<<capped_grid((n_lines + kThreads - 1) / kThreads, 8), kThreads, 0, (cudaStream_t)stream>>>(
       (const long long*)rowptr, sorted_cols, sorted_vals, means, global_mean, queries, K, nbr_ids, nbr_sims, nbr_cnt,
       n_lines, line_qpos, line_probe, minus_one_unrated, pred, status);
+  QREC_LAUNCH_CHECK();
+  return QREC_OK;
+}
+
+int qrec_knn_pair_similarity_f64(const int64_t* rowptr, const int32_t* cols, const double* vals, const double* sq,
+                                  const double* means, const int32_t* sorted_cols, const double* sorted_vals,
+                                  const double* sorted_sq, int64_t n_pairs, const int32_t* a, const int32_t* b,
+                                  const double* w, double* out, void* stream) {
+  QREC_REQUIRE(n_pairs >= 0, "knn_pair_similarity: n_pairs=%lld < 0", (long long)n_pairs);
+  if (n_pairs == 0) return QREC_OK;
+  QREC_REQUIRE(rowptr && means && a && b && w && out, "knn_pair_similarity: null pointer");
+  knn_pair_similarity_kernel<<<capped_grid((n_pairs + kThreads - 1) / kThreads, 8), kThreads, 0,
+                               (cudaStream_t)stream>>>((const long long*)rowptr, cols, vals, sq, means, sorted_cols,
+                                                       sorted_vals, sorted_sq, n_pairs, a, b, w, out);
   QREC_LAUNCH_CHECK();
   return QREC_OK;
 }

@@ -2,7 +2,8 @@
 //
 //   reference: model/rating/BasicMF.py:13-23 (kind 0), model/rating/PMF.py:13-22 (kind 1),
 //              model/rating/SVD.py:17-32 + predictForRating SVD.py:84-90 (kind 2),
-//              model/rating/SoRec.py:42-60 (kind 3: the trust-edge pass, on the tables (P, Z))
+//              model/rating/SoRec.py:42-60 (kind 3: the trust-edge pass, on the tables (P, Z)),
+//              model/rating/SocialMF.py:15-24 (kind 4: kind 1 on copies of the rows)
 //
 //   e = r - P[u].Q[i]                (SVD: - globalMean - Bi[i] - Bu[u], added in that order)
 //   kind 0:  P[u] += (lr*e)*Q[i];                  Q[i] += (lr*e)*P[u](new)
@@ -10,10 +11,12 @@
 //   kind 2:  kind 1 + Bu[u] += lr*(e - regB*Bu[u]);  Bi[i] += lr*(e - regB*Bi[i])
 //   kind 3:  P[u] += lr*((regS*e)*Z[v]);  Z[v] += lr*((regS*e)*P[u](new) - regZ*Z[v](old))
 //            (regS / regZ in the reg_u / reg_i slots, no bias vectors; the parity kernel only)
+//   kind 4:  P[u] += lr*(e*Q[i] - regU*P[u]);      Q[i] += lr*(e*P[u](old) - regI*Q[i](old))
+//            (no bias vectors; the parity kernel only)
 //   loss += e^2  (kind 3: regS*e^2)
 //
 // `p = self.P[u]` is a numpy view in the reference, so the item row is updated from the already
-// updated user row -- both kernels keep that.
+// updated user row -- both kernels keep that.  SocialMF copies both rows first (kind 4).
 //
 //   * mf_sgd_ordered_kernel -- parity mode, the same dataflow scheme as bpr_sgd_ordered_kernel:
 //     warps take entries in array order from a ticket counter and wait until their two rows have
@@ -220,10 +223,11 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
                    const int* wu, const int* wi, int* ver_p, int* ver_q, unsigned long long* ticket, T lr,
                    T reg_u, T reg_i, T* Bu, T* Bi, T reg_b, T global_mean, double* loss, int n_warps,
                    cudaStream_t st) {
-  QREC_REQUIRE(kind >= 0 && kind <= 3, "mf_sgd_ordered: kind=%d (0 BasicMF, 1 PMF, 2 SVD, 3 SoRec edges)", kind);
+  QREC_REQUIRE(kind >= 0 && kind <= 4, "mf_sgd_ordered: kind=%d (0 BasicMF, 1 PMF, 2 SVD, 3 SoRec edges, 4 SocialMF)",
+               kind);
   QREC_REQUIRE(P && Q && loss && ticket && ver_p && ver_q, "mf_sgd_ordered: null pointer");
   QREC_REQUIRE(kind != 2 || (Bu && Bi), "mf_sgd_ordered: kind 2 needs the bias vectors");
-  QREC_REQUIRE(kind != 3 || (!Bu && !Bi), "mf_sgd_ordered: kind 3 takes no bias vectors");
+  QREC_REQUIRE(kind < 3 || (!Bu && !Bi), "mf_sgd_ordered: kind %d takes no bias vectors", kind);
   QREC_REQUIRE(d >= 1 && d <= 256, "mf_sgd_ordered: d=%d unsupported (1..256)", d);
   QREC_REQUIRE(n >= 0, "mf_sgd_ordered: n < 0");
   if (n == 0) return QREC_OK;
@@ -234,7 +238,8 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
     const auto kernel = kind == 0   ? mf_sgd_ordered_kernel<T, E, 0>
                         : kind == 1 ? mf_sgd_ordered_kernel<T, E, 1>
                         : kind == 2 ? mf_sgd_ordered_kernel<T, E, 2>
-                                    : mf_sgd_ordered_kernel<T, E, 3>;
+                        : kind == 3 ? mf_sgd_ordered_kernel<T, E, 3>
+                                    : mf_sgd_ordered_kernel<T, E, 4>;
     kernel<<<grid, 256, 0, st>>>(P, Q, d, n, u, i, r, wu, wi, ver_p, ver_q, ticket, lr, reg_u, reg_i, Bu, Bi, reg_b,
                                  global_mean, loss);
   });

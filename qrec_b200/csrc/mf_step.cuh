@@ -7,6 +7,8 @@
 //   kind 3  SoRec.py:42-60     one trust edge (u, v) on the tables (P, Z); the "rating" is weight*tuv, regS and
 //                              regZ travel in the reg_u / reg_i slots and g = regS*e:
 //                              P[u] += lr*(g*z) ;  Z[v] += lr*(g*P[u] - regZ*z) ;  loss += regS*e^2
+//   kind 4  SocialMF.py:15-24  kind 1 on copies of both rows: the item step reads the user row as it was before
+//                              P[u] += lr*(e*q - regU*p) ;  Q[i] += lr*(e*p - regI*q)
 #pragma once
 
 namespace qrec {
@@ -38,6 +40,9 @@ __device__ __forceinline__ void mf_update_parity(T p, T q, T err, T g, T lr, T r
   } else if (KIND == 3) {
     pn = mf_add(p, mf_mul(lr, mf_mul(g, q)));
     qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(g, pn), mf_mul(reg_i, q))));
+  } else if (KIND == 4) {
+    pn = mf_add(p, mf_mul(lr, mf_sub(mf_mul(err, q), mf_mul(reg_u, p))));
+    qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(err, p), mf_mul(reg_i, q))));
   } else {
     pn = mf_add(p, mf_mul(lr, mf_sub(mf_mul(err, q), mf_mul(reg_u, p))));
     qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(err, pn), mf_mul(reg_i, q))));

@@ -918,6 +918,7 @@ def mask_rated(scores, users, rowptr, cols, value=0.0):
 # ---------------------------------------------------------------------------------------------
 MF_KINDS = {'BasicMF': 0, 'PMF': 1, 'SVD': 2}
 SOREC_EDGES = 3    # kind 3: SoRec's trust-edge pass on (P, Z), regS / regZ in the reg_u / reg_i slots
+SOCIALMF_RATINGS = 4    # kind 4: SocialMF's rating pass, kind 1 on copies of both rows
 
 
 def _opt(t, dtype, name):
@@ -930,6 +931,8 @@ def mf_sgd_ordered(kind, P, Q, u, i, r, wu, wi, lr, reg_u, reg_i, loss, Bu=None,
     torch = _torch()
     if kind == SOREC_EDGES:
         _sorec_edge_checks(P, Q, u, i, r, wu, wi, Bu, Bi)
+    if kind == SOCIALMF_RATINGS and (Bu is not None or Bi is not None):
+        raise QRecError('mf_sgd_ordered: kind 4 (SocialMF ratings) takes no bias vectors')
     f64 = P.dtype == torch.float64
     dt = torch.float64 if f64 else torch.float32
     d = P.shape[1]
@@ -1115,6 +1118,87 @@ def rste_predict_pairs(P, Q, u, i, f_rowptr, f_cols, f_w, denom, alpha, out=None
     check(fn(ptr['P'], ptr['Q'], P.shape[1], u.shape[0], ptr['u'], ptr['i'], ptr['f_rowptr'], ptr['f_cols'],
              ptr['f_w'], ptr['denom'], float(alpha), out.data_ptr(), _stream()), 'qrec_rste_predict_pairs')
     return out
+
+
+# ---------------------------------------------------------------------------------------------
+# K17: the trust-neighbourhood user pass of SocialMF and SoReg
+# ---------------------------------------------------------------------------------------------
+SOCIAL_PASS_KINDS = {'SocialMF': 0, 'SoReg': 1}
+
+
+def social_order_prepare(visit, num_users, f_rowptr, f_cols, g_rowptr, g_cols):
+    """Schedule of a visiting order (host, one pass): (pos, depth).  pos[u] is user u's position in `visit`, -1 when u
+    is not visited; depth is the longest chain of users each waiting for an earlier followee (f_*) or follower (g_*).
+    The order is fixed per model, so this runs once."""
+    visit = np.ascontiguousarray(visit, dtype=np.int32)
+    f_rowptr, g_rowptr = (np.ascontiguousarray(a, dtype=np.int64) for a in (f_rowptr, g_rowptr))
+    f_cols, g_cols = (np.ascontiguousarray(a, dtype=np.int32) for a in (f_cols, g_cols))
+    U = int(num_users)
+    for rp, side in ((f_rowptr, 'followee'), (g_rowptr, 'follower')):
+        if rp.shape != (U + 1,):
+            raise QRecError('social_order_prepare: the %s rowptr needs %d entries' % (side, U + 1))
+    if visit.ndim != 1 or visit.shape[0] > U:
+        raise QRecError('social_order_prepare: the visiting order lists %d users, more than %d' % (visit.size, U))
+    pos, depth = np.empty(U, np.int32), np.zeros(1, np.int64)
+    check(lib.qrec_social_order_prepare(visit.shape[0], _i32p(visit), U, _i64p(f_rowptr), _i32p(f_cols),
+                                        f_cols.shape[0], _i64p(g_rowptr), _i32p(g_cols), g_cols.shape[0], _i32p(pos),
+                                        _i64p(depth)), 'qrec_social_order_prepare')
+    return pos, int(depth[0])
+
+
+def social_user_pass(kind, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_cols, g_val, lr, coef, loss,
+                     n_warps=0):
+    """The trust-neighbourhood user pass, sequential-equivalent, in place on P (float32 or float64): kind 0 SocialMF
+    (f_val: the followee weights, coef: regS), kind 1 SoReg (f_val / g_val: the similarities Sim[u][.] of the
+    followees / followers, coef: alpha).  visit (int32): the visiting order; pos: social_order_prepare's; f_* / g_*:
+    the followee / follower CSRs (rowptr int64, cols int32); g_val may be None for kind 0.  loss (float64) += the
+    pass's loss terms."""
+    torch = _torch()
+    name = 'social_user_pass'
+    if kind not in (0, 1):
+        raise QRecError('%s: kind must be 0 (SocialMF) or 1 (SoReg), got %r' % (name, kind))
+    if kind == 1 and g_val is None:
+        raise QRecError('%s: SoReg needs the followers\' similarities (g_val)' % name)
+    if P.dtype not in (torch.float32, torch.float64) or P.dim() != 2:
+        raise QRecError('%s: P must be a 2-D float32 or float64 table' % name)
+    if not 1 <= P.shape[1] <= 256:
+        raise QRecError('%s: d=%d unsupported (1..256)' % (name, P.shape[1]))
+    U = P.shape[0]
+    if visit.dim() != 1 or visit.shape[0] > U:
+        raise QRecError('%s: the visiting order must be 1-D and list at most %d users' % (name, U))
+    if pos.shape != (U,):
+        raise QRecError('%s: pos needs one entry per user (%d)' % (name, U))
+    for rp, cols, val, side in ((f_rowptr, f_cols, f_val, 'followee'), (g_rowptr, g_cols, g_val, 'follower')):
+        if rp.dim() != 1 or rp.shape[0] != U + 1:
+            raise QRecError('%s: the %s rowptr needs %d entries' % (name, side, U + 1))
+        if cols.dim() != 1 or (val is not None and val.shape != cols.shape):
+            raise QRecError('%s: %s ids and values differ in length' % (name, side))
+    if loss.numel() < 1:
+        raise QRecError('%s: loss needs one entry' % name)
+    i32, i64 = torch.int32, torch.int64
+    tensors = [(P, P.dtype, 'P'), (visit, i32, 'visit'), (pos, i32, 'pos'), (f_rowptr, i64, 'f_rowptr'),
+               (f_cols, i32, 'f_cols'), (f_val, P.dtype, 'f_val'), (g_rowptr, i64, 'g_rowptr'), (g_cols, i32, 'g_cols'),
+               (loss, torch.float64, 'loss')] + ([(g_val, P.dtype, 'g_val')] if g_val is not None else [])
+    for t, dt, tname in tensors:
+        if t.dtype != dt:
+            raise QRecError('%s: %s must be %s, got %s' % (name, tname, dt, t.dtype))
+    ptr = {tname: _dev(t, dt, '%s: %s' % (name, tname)) for t, dt, tname in tensors}
+    n = visit.shape[0]
+    _ids_below(visit, U, name + ': a visited user is outside [0, %d)')
+    for rp, cols, side in ((f_rowptr, f_cols, 'followee'), (g_rowptr, g_cols, 'follower')):
+        if int(rp[0]) != 0 or int(rp[-1]) != cols.shape[0] or bool((rp[1:] < rp[:-1]).any()):
+            raise QRecError('%s: the %s rowptr must rise from 0 to len = %d' % (name, side, cols.shape[0]))
+        _ids_below(cols, U, name + ': a ' + side + ' is outside [0, %d)')
+    # every wait reads pos: it must name exactly the visit positions
+    if int((pos >= 0).sum()) != n or (n and not bool((pos[visit.long()] == torch.arange(n, device=pos.device)).all())):
+        raise QRecError('%s: pos does not match the visiting order' % name)
+    done = torch.zeros(U, dtype=i32, device=P.device)
+    ticket = torch.zeros(1, dtype=torch.int64, device=P.device)
+    fn = lib.qrec_social_user_pass_f64 if P.dtype == torch.float64 else lib.qrec_social_user_pass_f32
+    check(fn(int(kind), ptr['P'], P.shape[1], n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'],
+             ptr['f_val'], ptr['g_rowptr'], ptr['g_cols'], ptr.get('g_val'), done.data_ptr(), ticket.data_ptr(),
+             float(lr), float(coef), ptr['loss'], int(n_warps), _stream()), 'qrec_social_user_pass')
+    return loss
 
 
 # =============================================================================================
@@ -1649,6 +1733,44 @@ def knn_predict(rowptr, sorted_cols, sorted_vals, means, global_mean, queries, i
                                    int(bool(minus_one_unrated)), pred.data_ptr(), status.data_ptr(), _stream()),
           'qrec_knn_predict_f64')
     return pred, status
+
+
+def knn_pair_similarity(rowptr, cols, vals, sq, means, sorted_cols, sorted_vals, sorted_sq, a, b, w):
+    """SoReg's similarities of listed pairs: (pcc(a[k], b[k]) + w[k]) / 2.0 with pearson_sp over the rows rowptr /
+    cols / vals (insertion order, Rating.rating_csr), sq = knn_squares(.., metric 0) and the row means; sorted_cols /
+    sorted_vals and sorted_sq: knn_sorted_view of (cols, vals) and of (cols, sq).  a / b int32 row ids, w float64.
+    Returns float64 [len(a)].  Shapes and dtypes are checked first, then that every tensor is a contiguous CUDA tensor,
+    then the contents."""
+    torch = _torch()
+    i32, i64, f64 = torch.int32, torch.int64, torch.float64
+    name = 'knn_pair_similarity'
+    if rowptr.dtype != i64 or rowptr.dim() != 1 or rowptr.shape[0] < 1:
+        raise QRecError('%s: rowptr must be a 1-D int64 tensor of n_rows + 1 entries' % name)
+    if cols.dtype != i32 or cols.dim() != 1 or sorted_cols.dtype != i32 or sorted_cols.shape != cols.shape:
+        raise QRecError('%s: cols and sorted_cols must be 1-D int32 tensors of one length' % name)
+    n, nnz = rowptr.shape[0] - 1, cols.shape[0]
+    for t, tname in ((vals, 'vals'), (sq, 'sq'), (sorted_vals, 'sorted_vals'), (sorted_sq, 'sorted_sq')):
+        _f64_vec('%s: %s' % (name, tname), t, nnz)
+    _f64_vec(name + ': means', means, n)
+    if a.dtype != i32 or b.dtype != i32 or a.dim() != 1 or b.shape != a.shape:
+        raise QRecError('%s: a and b must be int32 of one length' % name)
+    _f64_vec(name + ': w', w, a.shape[0])
+    tensors = ((rowptr, i64, 'rowptr'), (cols, i32, 'cols'), (vals, f64, 'vals'), (sq, f64, 'sq'),
+               (means, f64, 'means'), (sorted_cols, i32, 'sorted_cols'), (sorted_vals, f64, 'sorted_vals'),
+               (sorted_sq, f64, 'sorted_sq'), (a, i32, 'a'), (b, i32, 'b'), (w, f64, 'w'))
+    ptr = [_dev(t, dt, '%s: %s' % (name, tname)) for t, dt, tname in tensors]
+    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
+        raise QRecError('%s: rowptr must rise from 0 to len(cols) = %d' % (name, nnz))
+    if nnz > 1:   # the bisection needs every row of the sorted view ascending
+        row = torch.repeat_interleave(torch.arange(n, device=cols.device), rowptr[1:] - rowptr[:-1])
+        if bool(((sorted_cols[1:] <= sorted_cols[:-1]) & (row[1:] == row[:-1])).any()):
+            raise QRecError('%s: sorted_cols must rise strictly within each row (knn_sorted_view)' % name)
+    _ids_below(a, n, name + ': a row id is outside [0, %d)')
+    _ids_below(b, n, name + ': a row id is outside [0, %d)')
+    out = torch.empty(a.shape[0], dtype=f64, device=cols.device)
+    check(lib.qrec_knn_pair_similarity_f64(*ptr[:8], a.shape[0], *ptr[8:], out.data_ptr(), _stream()),
+          'qrec_knn_pair_similarity_f64')
+    return out
 
 
 def slopeone_predict(item_rowptr, item_users, item_vals, item_means, user_rowptr, user_items, user_vals, user_means,

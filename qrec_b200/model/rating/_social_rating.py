@@ -1,4 +1,4 @@
-"""Shared pieces of the social rating models SoRec and RSTE on the H100 engine.
+"""Shared pieces of the social rating models SoRec, RSTE, SocialMF and SoReg on the H100 engine.
 
 Both train in the reference's order with the in-order kernels, in float64 (`engine=-precision f64`, the default) or
 float32 (`-precision f32`; `-mode fast` runs the same kernels in float32, as WRMF and CoFactor do).  There is no
@@ -29,6 +29,29 @@ def followee_csr(data, social):
         denom[k] = np.array(w).sum()
         rowptr[k + 1] = len(cols)
     return rowptr, np.array(cols, np.int32), np.array(weights, np.float64), denom
+
+
+def follower_csr(data, social, values=None):
+    """The cleaned follower dicts as a CSR over the training users' ids, each row in the dict's insertion order:
+    (rowptr int64 [U+1], cols int32, vals float64).  vals are the relation weights, or values[u][g] (names) when
+    `values` is given (SoReg's Sim)."""
+    U = len(data.user)
+    rowptr = np.zeros(U + 1, np.int64)
+    cols, vals = [], []
+    for k in range(U):
+        name = data.id2user[k]
+        for g, wg in social.getFollowers(name).items():
+            if data.containsUser(g):
+                cols.append(data.user[g])
+                vals.append(wg if values is None else values[name][g])
+        rowptr[k + 1] = len(cols)
+    return rowptr, np.array(cols, np.int32), np.array(vals, np.float64)
+
+
+def visit_order(data, social):
+    """The user pass's visiting order: `social.user` (the first-appearance order of the relation list as read, before
+    the cleaning) restricted to training users, as ids (SocialMF.py:26-27, SoReg.py:54-58)."""
+    return np.array([data.user[name] for name in social.user if data.containsUser(name)], np.int32)
 
 
 class SocialRatingMF(SocialRecommender):

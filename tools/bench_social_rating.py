@@ -1,13 +1,15 @@
 #!/usr/bin/env python
-"""SoRec's trust-edge pass (K9 kind 3) and RSTE's rating pass (K16), in float64 as the parity path runs them, on the
-two synthetic shapes of bench_serec.py (qrec_b200.synthetic, Zipf-skewed item popularity):
+"""SoRec's trust-edge pass (K9 kind 3), RSTE's rating pass (K16), the user passes of SocialMF and SoReg (K17) and SoReg's
+pair similarities (qrec_knn_pair_similarity_f64), in float64 as the parity path runs them, on the two synthetic shapes of bench_serec.py (qrec_b200.synthetic, Zipf-skewed item popularity):
   * lastfm-like: 1,892 users x 17,632 items, 40 entries per user, d = 20;
   * yelp2018-like: 31,668 users x 38,048 items, 36 entries per user, d = 64.
 Followee counts are bench_serec.py's draw (a fifth of the users follow nobody, the rest a log-normal count); the
 followees are drawn uniformly among the other users, weight 1.  The entry stream and the edge list are shuffled.
 
 Timed with CUDA events, one launch per pass: SoRec's edge pass, RSTE's rating pass, and K9 PMF (kind 1) on the same
-entry stream, so that the cost of the followee reads shows.  The host wait numbers are prepared beforehand.  The passes
+entry stream, so that the cost of the followee reads shows; SocialMF's and SoReg's user passes over a shuffled visiting
+order of all users (followers are the transpose of the followees; SoReg's similarities are drawn uniformly); and the
+Pearson similarity of every trust edge over the users' rated rows (half-step ratings), built once per model.  The host wait numbers are prepared beforehand.  The passes
 are launched through the C entry points: the engine wrappers' input checks read device values back (ids, CSR bounds),
 which would put host round trips inside the timed window of some passes and not others.  Each pass zeroes its row
 counters and ticket inside the window (two memsets), as every ordered launch needs.  One JSON line per shape with the
@@ -109,15 +111,58 @@ def main():
                 ptr(edge_cnt), ptr(edge_cnt) + 4 * U, ptr(tickets) + 16, 1e-3, 0.1, 0.1, None, None, 0.0, 0.0,
                 ptr(loss), edge_n, st), 'qrec_mf_sgd_ordered_f64')
 
-        for fn in (rste, pmf, edges):                                   # warm-up
+        # K17: the user passes over a shuffled visiting order; followers = the followees' transpose
+        gorder = np.argsort(cols, kind='stable')
+        grp = np.zeros(U + 1, np.int64)
+        grp[1:] = np.cumsum(np.bincount(cols, minlength=U))
+        gcols = np.repeat(np.arange(U, dtype=np.int32), np.diff(rowptr))[gorder]
+        visit = rng.permutation(U).astype(np.int32)
+        spos, social_depth = E.social_order_prepare(visit, U, rowptr, cols, grp, gcols)
+        sdev = [torch.from_numpy(a).to(dev) for a in (visit, spos, grp, gcols)]
+        sim_f = torch.rand(cols.shape[0], device=dev, dtype=f64, generator=g)
+        sim_g = torch.rand(cols.shape[0], device=dev, dtype=f64, generator=g)
+        social_n = width(U, social_depth)
+        done = torch.zeros(U, dtype=torch.int32, device=dev)
+        stickets = torch.zeros(2, dtype=torch.int64, device=dev)
+
+        def user_pass(kind):
+            def run():
+                done.zero_(); stickets[kind:kind + 1].zero_()
+                E.check(E.lib.qrec_social_user_pass_f64(
+                    kind, ptr(P), D, U, ptr(sdev[0]), ptr(sdev[1]), ptr(social[0]), ptr(social[1]),
+                    ptr(social[2]) if kind == 0 else ptr(sim_f), ptr(sdev[2]), ptr(sdev[3]), ptr(sim_g), ptr(done),
+                    ptr(stickets) + 8 * kind, 1e-3, 0.1, ptr(loss), social_n, st), 'qrec_social_user_pass_f64')
+            return run
+
+        # SoReg's similarities: one per trust edge, over each user's distinct rated items
+        up = np.unique(np.stack([u, i]), axis=1)
+        krp = np.concatenate([[0], np.bincount(up[0], minlength=U).cumsum()]).astype(np.int64)
+        kv = rng.integers(1, 9, up.shape[1]) * 0.5
+        km = np.bincount(up[0], weights=kv, minlength=U) / np.maximum(np.diff(krp), 1)
+        kdev = [torch.from_numpy(a).to(dev) for a in (krp, up[1].astype(np.int32), kv, E.knn_squares(krp, kv, km, 0), km)]
+        ksorted = E.knn_sorted_view(kdev[0], kdev[1], kdev[2]) + E.knn_sorted_view(kdev[0], kdev[1], kdev[3])[1:]
+        pa, pb = (torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in (eu, ev))
+        pw = torch.ones(eu.shape[0], dtype=f64, device=dev)
+        sims = torch.empty(eu.shape[0], dtype=f64, device=dev)
+
+        def pair_sims():
+            E.check(E.lib.qrec_knn_pair_similarity_f64(*(ptr(a) for a in kdev), *(ptr(a) for a in ksorted),
+                                                       eu.shape[0], ptr(pa), ptr(pb), ptr(pw), ptr(sims), st),
+                    'qrec_knn_pair_similarity_f64')
+
+        socialmf, soreg = user_pass(0), user_pass(1)
+        for fn in (rste, pmf, edges, socialmf, soreg, pair_sims):      # warm-up
             fn()
         t_rste, t_pmf, t_edges = timed(torch, rste, reps), timed(torch, pmf, reps), timed(torch, edges, reps)
+        t_socialmf, t_soreg, t_sims = timed(torch, socialmf, reps), timed(torch, soreg, reps), timed(torch, pair_sims, reps)
         print(json.dumps(dict(
             shape=label, users=U, items=I, entries=n, d=D, dtype='float64', edges=int(eu.shape[0]),
             followee_reads=int(np.diff(rowptr)[u].sum()), deg_mean=round(float(np.diff(rowptr).mean()), 2),
             deg_max=int(np.diff(rowptr).max()),
             ms_sorec_edge_pass=round(t_edges, 3), ms_rste_pass=round(t_rste, 3), ms_pmf_pass=round(t_pmf, 3),
-            depth_sorec_edges=edge_depth, depth_rste=rste_depth, depth_pmf=pmf_depth,
+            ms_socialmf_user_pass=round(t_socialmf, 3), ms_soreg_user_pass=round(t_soreg, 3),
+            ms_soreg_pair_similarity=round(t_sims, 3),
+            depth_sorec_edges=edge_depth, depth_rste=rste_depth, depth_pmf=pmf_depth, depth_social_users=social_depth,
             entries_per_s_sorec_edges=round(eu.shape[0] / (t_edges / 1e3)), entries_per_s_rste=round(n / (t_rste / 1e3)),
             entries_per_s_pmf=round(n / (t_pmf / 1e3)), gpu=name, power_limit=limit)), flush=True)
 

@@ -227,6 +227,30 @@ def main():
                                dev((np.arange(300) % nu).astype(np.int32)), max_ctas=c)
         torch.cuda.synchronize()
         print('sanitize_all: + K15, launched', E.launch_count(), 'kernels')
+        # K17 (SocialMF / SoReg user pass) on a ring-with-chords trust graph with self-follows, both kinds and dtypes,
+        # one CTA and a full grid; SoReg's pair similarities over the K15 user rows
+        fol = [sorted({(a + 1) % nu, (7 * a + 3) % nu, a}) for a in range(nu)]
+        frp = np.concatenate([[0], np.cumsum([len(x) for x in fol])]).astype(np.int64)
+        fcol = np.array([v for x in fol for v in x], np.int32)
+        back = np.argsort(fcol, kind='stable')
+        grp = np.concatenate([[0], np.cumsum(np.bincount(fcol, minlength=nu))]).astype(np.int64)
+        gcol = np.repeat(np.arange(nu, dtype=np.int32), np.diff(frp))[back]
+        visit = np.random.default_rng(4).permutation(nu)[: nu - 3].astype(np.int32)
+        spos, _ = E.social_order_prepare(visit, nu, frp, fcol, grp, gcol)
+        for dt in (torch.float64, torch.float32):
+            vals = torch.rand(fcol.shape[0], device='cuda').to(dt)
+            for kind in (0, 1):
+                for nw in (1, 0):
+                    E.social_user_pass(kind, torch.rand(nu, 33, device='cuda').to(dt), dev(visit), dev(spos), dev(frp),
+                                       dev(fcol), vals, dev(grp), dev(gcol), vals[torch.from_numpy(back).cuda()], 0.05,
+                                       0.1, torch.zeros(1, dtype=torch.float64, device='cuda'), n_warps=nw)
+        ksq = dev(E.knn_squares(rp_h, kv.cpu().numpy(), km.cpu().numpy(), 0))
+        pa = dev(np.arange(0, nu, 3).astype(np.int32))
+        E.knn_pair_similarity(krp, kcol, kv, ksq, km, *E.knn_sorted_view(krp, kcol, kv),
+                              E.knn_sorted_view(krp, kcol, ksq)[1], pa, (pa * 5 + 1) % nu,
+                              torch.ones(pa.shape[0], dtype=torch.float64, device='cuda'))
+        torch.cuda.synchronize()
+        print('sanitize_all: + K17 and the pair similarities, launched', E.launch_count(), 'kernels')
 
 
 if __name__ == '__main__':
