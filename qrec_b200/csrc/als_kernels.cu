@@ -386,27 +386,17 @@ inline size_t cof_smem_bytes(int d) {
   return sizeof(double) * ((size_t)a_words(d) + (size_t)(kStage + 4) * pad4(d) + 3 * kStage);
 }
 
-__device__ __forceinline__ void wait_stamp(const int* p, int sweep) {
-  unsigned backoff = 32, polls = 0;
-  while (ld_acquire_gpu(p) != sweep) {
-    __nanosleep(backoff);
-    if (backoff < 256) backoff <<= 1;
-    // as in the ordered SGD kernels: ~10 s of polling means the stamps do not belong to this sweep -- abort the
-    // launch instead of hanging the GPU
-    if (++polls > (1u << 25)) __trap();
-  }
-}
-
 // One in-order item sweep (CoFactor.py, trainModel, item loop; arithmetic in cofactor_step.cuh).  For item i:
 //   A_Y = XtX + sum_u alpha*r x x^T + lambda*I + sum_c G_c G_c^T  -> Y_i      (X rows weight alpha*r, G rows weight 1)
 //   A_G = sum_c Y_c Y_c^T + gamma*I                               -> G_i, then w_i, c_i   (items with contexts only)
 // A and b are float64; a system that is not positive definite leaves its row unchanged and is counted in n_failed.
 //
 // Order.  The reference updates in place in item-id order, so a context c < i is read after its own update in this
-// sweep and c > i before it.  CTAs take items from `ticket` in id order.  Before reading its contexts a CTA waits
-// (acquire) until the stamp of every context c < i equals `sweep`; after writing Y_i, G_i, w_i, c_i it publishes its
-// own stamp (release add).  The SPPMI is symmetric, so a context c > i has i among its own contexts and waits for
-// i's stamp before it reads anything of i or writes its own rows: i reads c's values from before the sweep.
+// sweep and c > i before it.  The sweep runs on the in-order protocol of device.cuh with one CTA per item: CTAs take
+// items from `ticket` in id order.  Before reading its contexts a CTA waits (acquire) until the stamp of every
+// context c < i equals `sweep`; after writing Y_i, G_i, w_i, c_i it publishes its own stamp (release add).  The SPPMI
+// is symmetric, so a context c > i has i among its own contexts and waits for i's stamp before it reads anything of
+// i or writes its own rows: i reads c's values from before the sweep.
 // No deadlock: a CTA takes a ticket only while it runs and holds one at a time, and it waits only on smaller tickets,
 // which running CTAs hold; the CTA with the smallest unfinished ticket waits on nobody, so it always finishes.  Every
 // CTA of the persistent grid is resident at once (persistent_grid sizes it by occupancy), so no waiting CTA keeps
@@ -465,7 +455,7 @@ cofactor_item_sweep_kernel(T* Y, T* G, T* wb, T* cb, const T* __restrict__ X, co
     }
     for (long long k = cbeg + t; k < cend; k += kThreads) {
       const int c = __ldg(scol + k);
-      if (c < i) wait_stamp(stamps + c, sweep);
+      if (c < i) spin_until<32, 256>([=] { return ld_acquire_gpu(stamps + c) == sweep; });
     }
     __syncthreads();
     // contexts, first pass: G rows with weight 1 into A_Y and b_Y, and w_i's sum

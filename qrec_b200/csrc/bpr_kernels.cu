@@ -7,11 +7,9 @@
 // Two kernels:
 //   * bpr_sgd_ordered_kernel  -- parity mode.  The reference loop is Gauss-Seidel: triple k
 //     must see every earlier update of its three rows.  Instead of level-by-level launches
-//     the kernel runs the epoch as a dataflow: warps claim triples in array order from a
-//     ticket counter and spin until each of their three rows has reached the version
-//     (= number of earlier touches) computed by qrec_bpr_order_prepare.  Because tickets are
-//     handed out in order to running warps, the oldest unfinished triple always has its
-//     dependencies satisfied, so the scheme cannot deadlock whatever the grid size.
+//     the kernel runs the epoch as a dataflow on the in-order protocol of device.cuh: warps
+//     take triples in array order and wait until each of their three rows has reached the
+//     version (= number of earlier touches) computed by qrec_bpr_order_prepare.
 //   * bpr_sgd_batch_kernel    -- throughput mode.  LPR lanes own one triple (d=64: a half
 //     warp, one float4 per lane = one 128-bit LDG per row), the dot products are reduced with
 //     xor-shuffles inside the lane group and the three row deltas go back with
@@ -46,25 +44,13 @@ bpr_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
   double local_loss = 0.0;
   const T a_u = mul_rn(lr, reg_u), a_i = mul_rn(lr, reg_i);
   while (true) {
-    unsigned long long k = 0;
-    if (lane == 0) k = atomicAdd(ticket, 1ULL);
-    k = __shfl_sync(0xffffffffu, k, 0);
+    const unsigned long long k = warp_next_ticket(ticket);
     if (k >= (unsigned long long)n) break;
     const int uu = u[k], ii = i[k], jj = j[k];
     // lanes 0..2 each watch one row version
     const int* vp = lane == 0 ? ver_p + uu : (lane == 1 ? ver_q + ii : ver_q + jj);
     const int need = lane == 0 ? wu[k] : (lane == 1 ? wi[k] : wj[k]);
-    unsigned backoff = 8, polls = 0;
-    while (true) {
-      const int have = lane < 3 ? ld_acquire_gpu(vp) : need;
-      if (__all_sync(0xffffffffu, have == need)) break;
-      __nanosleep(backoff);
-      if (backoff < 64) backoff <<= 1;
-      // a ticket waits for at most (#resident warps) predecessors, i.e. milliseconds; ~10 s of polling
-      // means the wait_* arrays do not describe this triple stream -- abort the launch instead of
-      // hanging the GPU (the host sees a launch failure)
-      if (++polls > (1u << 27)) __trap();
-    }
+    spin_until<8, 64>([=] { return __all_sync(0xffffffffu, (lane < 3 ? ld_acquire_gpu(vp) : need) == need); });
     T* pr = P + (size_t)uu * d;
     T* qir = Q + (size_t)ii * d;
     T* qjr = Q + (size_t)jj * d;
@@ -98,8 +84,7 @@ bpr_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
         __stcg(qjr + c, qjn);
       }
     }
-    __threadfence();
-    __syncwarp();
+    warp_fence();
     if (lane < 3) red_release_gpu_add(const_cast<int*>(vp), 1);
     if (lane == 0) local_loss += neg_log(s);
   }
@@ -568,13 +553,7 @@ int launch_ordered(T* P, T* Q, int d, long long n, const int* u, const int* i, c
   QREC_REQUIRE(n >= 0, "bpr_sgd_ordered: n < 0");
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && j && wu && wi && wj, "bpr_sgd_ordered: null index pointer");
-  // 2 CTAs of 8 warps per SM: enough warps to cover the dependency DAG's width at the
-  // synthetic scale (~25 independent triples per level in user-major order) without
-  // drowning the LSU in pollers.
-  // n_warps > 0: the caller knows the width of the dependency DAG (qrec_bpr_order_depth) and asks
-  // for about that many pollers -- thousands of idle warps hammering the version counters slow the
-  // few that can make progress (1.4 independent triples per level on FilmTrust, ~25 at SYN scale)
-  const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
+  const int grid = ordered_grid(n_warps);
   with_lane_elems(d, [&](auto e) {
     bpr_sgd_ordered_kernel<T, decltype(e)::E><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, j, wu, wi, wj, ver_p, ver_q,
                                                                     ticket, lr, reg_u, reg_i, loss);

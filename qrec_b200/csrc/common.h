@@ -14,9 +14,11 @@ void count_launch(int n = 1);
 
 // Launch sizing (core.cpp).  sm_count(): SMs of the current device, queried once per device (132, an H100 SXM's,
 // if the query fails).  capped_grid(): `blocks` CTAs, but at most ctas_per_sm per SM and at least one (the
-// kernels are grid-stride loops).
+// kernels are grid-stride loops).  ordered_grid(): the grid of 8-warp CTAs for a warp-per-position in-order kernel
+// (device.cuh) asked for about n_warps pollers, 0 for the default.
 int sm_count();
 int capped_grid(long long blocks, int ctas_per_sm);
+int ordered_grid(int n_warps);
 // Raises `kernel`'s dynamic shared-memory limit to at least `bytes` on the current device.  The limit belongs to
 // the kernel as loaded on each device, so it is set once per (kernel, device); safe to call from several threads.
 cudaError_t allow_dynamic_smem(const void* kernel, int bytes);

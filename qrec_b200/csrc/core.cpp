@@ -39,6 +39,13 @@ int capped_grid(long long blocks, int ctas_per_sm) {
   return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
 }
 
+// 2 CTAs of 8 warps per SM: enough warps to cover the dependency DAG's width at the synthetic scale (~25 independent
+// triples per level of K1 in user-major order) without drowning the LSU in pollers.
+// n_warps > 0: the caller knows the width of the dependency DAG (e.g. qrec_bpr_order_depth) and asks for about that
+// many pollers -- thousands of idle warps hammering the version counters slow the few that can make progress
+// (1.4 independent triples per level on FilmTrust, ~25 at SYN scale)
+int ordered_grid(int n_warps) { return n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2; }
+
 cudaError_t allow_dynamic_smem(const void* kernel, int bytes) {
   static std::mutex mu;
   static std::map<std::pair<const void*, int>, int> granted;   // (kernel, device) -> limit set

@@ -1,6 +1,6 @@
 // Device building blocks shared by the kernels of libqrec.so: the vector scatter-add every hot kernel ends in,
-// lane-group reductions, the SFU sigmoid / -ln of the throughput kernels, the row-version protocol of the parity
-// kernels, the per-block loss reduction and the mbarrier helpers of the bulk-copy (TMA) pipelines.
+// lane-group reductions, the SFU sigmoid / -ln of the throughput kernels, the ticket / wait / publish protocol of the
+// in-order kernels, the per-block loss reduction and the mbarrier helpers of the bulk-copy (TMA) pipelines.
 #pragma once
 #include <cstdint>
 
@@ -81,6 +81,44 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
 }
 __device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
   asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// ---- In-order kernels.  K1's, K9's and K16's ordered SGD kernels and K17's user pass replay a sequential loop with
+// one warp per position; K12's item sweep does so with one CTA per item.  They share one protocol:
+//   * positions are drawn from a global ticket in order (warp_next_ticket; K12 draws per CTA), so they go to running
+//     warps in order;
+//   * before it reads, a position polls the counters that earlier positions publish until they reach the values it
+//     needs (spin_until with acquire loads);
+//   * after it writes, every lane's stores are made visible (warp_fence) before the release adds that publish them.
+// A position waits only on smaller ones, which running warps hold, and the smallest unfinished position waits on
+// nobody, so the scheme cannot deadlock whatever the grid size.  A position waits for at most (#resident warps)
+// predecessors, i.e. milliseconds; about 8.6 s (2^33 ns) of polling means its wait numbers do not describe the
+// stream, and it traps (the host sees a launch failure) instead of hanging the GPU.
+
+// the warp's next position: lane 0 draws it, every lane gets it
+__device__ __forceinline__ unsigned long long warp_next_ticket(unsigned long long* ticket) {
+  unsigned long long k = 0;
+  if ((threadIdx.x & 31) == 0) k = atomicAdd(ticket, 1ULL);
+  return __shfl_sync(0xffffffffu, k, 0);
+}
+
+// Polls until ready() is true, sleeping FIRST_NS after the first miss and doubling up to MAX_NS; traps after
+// 2^33 / MAX_NS polls.  Warp kernels pass a ready() that votes with __all_sync, so the warp leaves together.
+template <unsigned FIRST_NS, unsigned MAX_NS, typename F>
+__device__ __forceinline__ void spin_until(F ready) {
+  constexpr unsigned kMaxPolls = (unsigned)((1ULL << 33) / MAX_NS);
+  unsigned backoff = FIRST_NS, polls = 0;
+  while (!ready()) {
+    __nanosleep(backoff);
+    if (backoff < MAX_NS) backoff <<= 1;
+    if (++polls > kMaxPolls) __trap();
+  }
+}
+
+// every lane's row writes visible before any lane's release add
+__device__ __forceinline__ void warp_fence() {
+  __threadfence();
+  __syncwarp();
 }
 
 // The block's per-thread fp32 loss terms summed into *loss with one double atomic (none when the sum is 0).

@@ -18,11 +18,10 @@
 // `p = self.P[u]` is a numpy view in the reference, so the item row is updated from the already
 // updated user row -- both kernels keep that.  SocialMF copies both rows first (kind 4).
 //
-//   * mf_sgd_ordered_kernel -- parity mode, the same dataflow scheme as bpr_sgd_ordered_kernel:
-//     warps take entries in array order from a ticket counter and wait until their two rows have
-//     reached the version (= number of earlier touches) computed by qrec_mf_order_prepare; mul/add
-//     are kept apart (no FMA) in numpy's evaluation order.  Bu[u] / Bi[i] ride on the version
-//     counters of P[u] / Q[i].
+//   * mf_sgd_ordered_kernel -- parity mode, on the in-order protocol of device.cuh: warps take
+//     entries in array order and wait until their two rows have reached the version (= number
+//     of earlier touches) computed by qrec_mf_order_prepare; mul/add are kept apart (no FMA) in
+//     numpy's evaluation order.  Bu[u] / Bi[i] ride on the version counters of P[u] / Q[i].
 //   * mf_sgd_batch_kernel   -- throughput mode: LPR lanes own one entry (one float4 per lane and
 //     row), xor-shuffle dot, both row deltas go back with red.global.add.v4.f32; rows shared by
 //     in-flight entries receive the sum of their deltas.
@@ -50,24 +49,13 @@ mf_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
   const int lane = threadIdx.x & 31;
   double local_loss = 0.0;
   while (true) {
-    unsigned long long k = 0;
-    if (lane == 0) k = atomicAdd(ticket, 1ULL);
-    k = __shfl_sync(0xffffffffu, k, 0);
+    const unsigned long long k = warp_next_ticket(ticket);
     if (k >= (unsigned long long)n) break;
     const int uu = u[k], ii = i[k];
     const T rating = r[k];
     const int* vp = lane == 0 ? ver_p + uu : ver_q + ii;   // lanes 0 and 1 each watch one row version
     const int need = lane == 0 ? wu[k] : wi[k];
-    unsigned backoff = 8, polls = 0;
-    while (true) {
-      const int have = lane < 2 ? ld_acquire_gpu(vp) : need;
-      if (__all_sync(0xffffffffu, have == need)) break;
-      __nanosleep(backoff);
-      if (backoff < 64) backoff <<= 1;
-      // as in bpr_sgd_ordered_kernel: ~10 s of polling means the wait arrays do not describe this
-      // entry stream -- abort the launch instead of hanging the GPU
-      if (++polls > (1u << 27)) __trap();
-    }
+    spin_until<8, 64>([=] { return __all_sync(0xffffffffu, (lane < 2 ? ld_acquire_gpu(vp) : need) == need); });
     T* pr = P + (size_t)uu * d;
     T* qr = Q + (size_t)ii * d;
     T p[E], q[E];
@@ -105,8 +93,7 @@ mf_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
       if (lane == 0) __stcg(Bu + uu, qrec::mf_bias_parity<T>(bu, err, lr, reg_b));
       if (lane == 1) __stcg(Bi + ii, qrec::mf_bias_parity<T>(bi, err, lr, reg_b));
     }
-    __threadfence();
-    __syncwarp();
+    warp_fence();
     if (lane < 2) red_release_gpu_add(const_cast<int*>(vp), 1);
     if (lane == 0) local_loss += qrec::mf_loss_term<T, KIND>(err, reg_u);
   }
@@ -232,7 +219,7 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
   QREC_REQUIRE(n >= 0, "mf_sgd_ordered: n < 0");
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && r && wu && wi, "mf_sgd_ordered: null entry pointer");
-  const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
+  const int grid = ordered_grid(n_warps);
   with_lane_elems(d, [&](auto e) {
     constexpr int E = decltype(e)::E;
     const auto kernel = kind == 0   ? mf_sgd_ordered_kernel<T, E, 0>

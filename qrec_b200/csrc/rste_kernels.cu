@@ -1,7 +1,7 @@
 // K16: RSTE's rating pass (model/rating/RSTE.py:20-64) on the GPU.
 //
-//   rste_sgd_ordered_kernel -- the epoch in list order, sequential-equivalent.  Warps take entries from a ticket
-//     counter (one warp per entry, lanes across d).  An entry (u, i) reads its own rows P[u], Q[i] and the rows
+//   rste_sgd_ordered_kernel -- the epoch in list order, sequential-equivalent, on the in-order protocol of
+//     device.cuh (one warp per entry, lanes across d).  An entry (u, i) reads its own rows P[u], Q[i] and the rows
 //     P[f] of all u's followees, and writes P[u] and Q[i] only (rste_step.cuh has the formulas).  Before it reads,
 //     entry k waits until
 //       ver_p[u]   == wait_u[k]        writes to P[u] by earlier entries        (read/write after write)
@@ -35,18 +35,6 @@ __device__ __forceinline__ int count_below(const int* __restrict__ a, int n, lon
   return lo;
 }
 
-// poll until every lane's `have()` equals its `need`; ~10 s of polling means the wait arrays do not describe
-// this entry stream -- abort the launch instead of hanging the GPU (as mf_sgd_ordered_kernel does)
-template <typename F>
-__device__ __forceinline__ void wait_all(int need, F have) {
-  unsigned backoff = 8, polls = 0;
-  while (!__all_sync(0xffffffffu, have() == need)) {
-    __nanosleep(backoff);
-    if (backoff < 64) backoff <<= 1;
-    if (++polls > (1u << 27)) __trap();
-  }
-}
-
 // warp-wide P[row].q over the lane's E elements (element e*32+lane)
 template <typename T, int E>
 __device__ __forceinline__ T row_dot(const T* __restrict__ row, const T (&q)[E], int d, int lane) {
@@ -71,9 +59,7 @@ rste_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n
   const int lane = threadIdx.x & 31;
   double local_loss = 0.0;
   while (true) {
-    unsigned long long k = 0;
-    if (lane == 0) k = atomicAdd(ticket, 1ULL);
-    k = __shfl_sync(0xffffffffu, k, 0);
+    const unsigned long long k = warp_next_ticket(ticket);
     if (k >= (unsigned long long)n) break;
     const int uu = u[k], ii = i[k];
     const T rating = r[k];
@@ -83,7 +69,7 @@ rste_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n
     {
       const int* vp = lane == 0 ? ver_p + uu : lane == 1 ? ver_q + ii : reads_p + uu;
       const int need = lane == 0 ? wu[k] : lane == 1 ? wi[k] : lane == 2 ? wr[k] : 0;
-      wait_all(need, [&] { return lane < 3 ? ld_acquire_gpu(vp) : 0; });
+      spin_until<8, 64>([=] { return __all_sync(0xffffffffu, (lane < 3 ? ld_acquire_gpu(vp) : 0) == need); });
     }
     // followee rows, 32 at a time: each lane finds its followee's write count before position k
     for (long long base = fb; base < fe; base += 32) {
@@ -94,7 +80,7 @@ rste_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n
         const long long pb = pos_rowptr[f];
         need = count_below(pos + pb, (int)(pos_rowptr[f + 1] - pb), (long long)k);
       }
-      wait_all(need, [&] { return f != uu ? ld_acquire_gpu(ver_p + f) : 0; });
+      spin_until<8, 64>([=] { return __all_sync(0xffffffffu, (f != uu ? ld_acquire_gpu(ver_p + f) : 0) == need); });
     }
 
     T* pr = P + (size_t)uu * d;
@@ -121,8 +107,7 @@ rste_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n
       social = qrec::rste_social_add(social, __ldg(f_w + j), fdot);
     }
     // the followee rows are read: let their owners' later entries write them
-    __threadfence();
-    __syncwarp();
+    warp_fence();
     for (long long j = fb + lane; j < fe; j += 32) {
       const int f = __ldg(f_cols + j);
       if (f != uu) red_release_gpu_add(reads_p + f, 1);
@@ -141,8 +126,7 @@ rste_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n
         __stcg(qr + c, qn);
       }
     }
-    __threadfence();
-    __syncwarp();
+    warp_fence();
     if (lane == 0) red_release_gpu_add(ver_p + uu, 1);
     if (lane == 1) red_release_gpu_add(ver_q + ii, 1);
     if (lane == 0) local_loss += (double)err * (double)err;
@@ -191,7 +175,7 @@ int launch_ordered(T* P, T* Q, int d, long long n, const int* u, const int* i, c
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(u && i && r && wu && wi && wr && pos_rowptr && pos && f_rowptr && denom,
                "rste_sgd_ordered: null entry pointer");
-  const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
+  const int grid = ordered_grid(n_warps);
   with_lane_elems(d, [&](auto e) {
     constexpr int E = decltype(e)::E;
     rste_sgd_ordered_kernel<T, E><<<grid, 256, 0, st>>>(P, Q, d, n, u, i, r, wu, wi, wr, pos_rowptr, pos, f_rowptr,

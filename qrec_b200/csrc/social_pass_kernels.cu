@@ -2,7 +2,7 @@
 // (model/rating/SoReg.py:54-72) on the GPU.
 //
 //   social_user_pass_kernel -- the pass over the visiting order (the reference's `self.social.user` restricted to
-//     training users), sequential-equivalent.  Warps take visit positions from a ticket counter (one warp per user,
+//     training users), sequential-equivalent, on the in-order protocol of device.cuh (one warp per visit position,
 //     lanes across d).  User u reads its own row and the rows of its followees (SoReg: and of its followers), and
 //     writes its own row only; social_pass_step.cuh has the formulas.  Each user is visited at most once, so one
 //     done flag per user records every dependency: before it reads, the warp at position k waits until done[v] is
@@ -23,9 +23,7 @@ using namespace qrec;
 constexpr int kSocialMF = 0;
 constexpr int kSoReg = 1;
 
-// waits until done[v] is set for every neighbour v = cols[j] (j in [b, e)) visited before position k; as
-// mf_sgd_ordered_kernel: ~10 s of polling means the schedule does not describe this graph -- abort the launch
-// instead of hanging the GPU
+// waits until done[v] is set for every neighbour v = cols[j] (j in [b, e)) visited before position k
 __device__ __forceinline__ void wait_neighbours(const int* __restrict__ cols, long long b, long long e, int uu,
                                                 const int* __restrict__ pos, long long k, const int* done, int lane) {
   for (long long base = b; base < e; base += 32) {
@@ -36,12 +34,7 @@ __device__ __forceinline__ void wait_neighbours(const int* __restrict__ cols, lo
       const int pv = v != uu ? __ldg(pos + v) : -1;
       if (pv >= 0 && pv < k) flag = done + v;
     }
-    unsigned backoff = 8, polls = 0;
-    while (!__all_sync(0xffffffffu, flag == nullptr || ld_acquire_gpu(flag) != 0)) {
-      __nanosleep(backoff);
-      if (backoff < 64) backoff <<= 1;
-      if (++polls > (1u << 27)) __trap();
-    }
+    spin_until<8, 64>([=] { return __all_sync(0xffffffffu, flag == nullptr || ld_acquire_gpu(flag) != 0); });
   }
 }
 
@@ -56,9 +49,7 @@ social_user_pass_kernel(T* __restrict__ P, int d, long long n, const int* __rest
   const int lane = threadIdx.x & 31;
   double local_loss = 0.0;
   while (true) {
-    unsigned long long k = 0;
-    if (lane == 0) k = atomicAdd(ticket, 1ULL);
-    k = __shfl_sync(0xffffffffu, k, 0);
+    const unsigned long long k = warp_next_ticket(ticket);
     if (k >= (unsigned long long)n) break;
     const int uu = __ldg(visit + k);
     const long long fb = __ldg(f_rowptr + uu), fe = __ldg(f_rowptr + uu + 1);
@@ -139,8 +130,7 @@ social_user_pass_kernel(T* __restrict__ P, int d, long long n, const int* __rest
         if (c < d) __stcg(pr + c, soreg_step(p[e], lr, coef, a1[e], a2[e]));
       }
     }
-    __threadfence();
-    __syncwarp();
+    warp_fence();
     if (lane == 0) red_release_gpu_add(done + uu, 1);
   }
   if (lane == 0 && local_loss != 0.0) atomicAdd(loss, local_loss);
@@ -156,7 +146,7 @@ int launch_pass(int kind, T* P, int d, long long n, const int* visit, const int*
   if (n == 0) return QREC_OK;
   QREC_REQUIRE(P && visit && pos && f_rowptr && g_rowptr && done && ticket && loss, "social_user_pass: null pointer");
   QREC_REQUIRE(kind != kSoReg || g_val, "social_user_pass: SoReg needs the followers' similarities");
-  const int grid = n_warps > 0 ? capped_grid((n_warps + 7) / 8, 2) : sm_count() * 2;
+  const int grid = ordered_grid(n_warps);
   with_lane_elems(d, [&](auto e) {
     constexpr int E = decltype(e)::E;
     const auto kernel = kind == kSocialMF ? social_user_pass_kernel<T, E, kSocialMF>

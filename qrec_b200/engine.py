@@ -268,6 +268,14 @@ def _stream():
     return _torch().cuda.current_stream().cuda_stream
 
 
+def _order_counters(device, *lengths):
+    """The state one launch of an in-order kernel starts from: zeroed int32 counters of the given lengths, then a
+    zeroed int64 ticket, on `device`."""
+    torch = _torch()
+    return ([torch.zeros(n, dtype=torch.int32, device=device) for n in lengths]
+            + [torch.zeros(1, dtype=torch.int64, device=device)])
+
+
 def sample_neg_philox(u, sorted_rowptr, sorted_cols, num_items, seed, epoch, out=None):
     torch = _torch()
     n = u.shape[0]
@@ -290,9 +298,7 @@ def bpr_sgd_ordered(P, Q, u, i, j, wu, wi, wj, lr, reg_u, reg_i, loss, n_warps=0
     n = u.shape[0]
     d = P.shape[1]
     assert Q.shape[1] == d
-    ver_p = torch.zeros(P.shape[0], dtype=torch.int32, device=P.device)
-    ver_q = torch.zeros(Q.shape[0], dtype=torch.int32, device=P.device)
-    ticket = torch.zeros(1, dtype=torch.int64, device=P.device)
+    ver_p, ver_q, ticket = _order_counters(P.device, P.shape[0], Q.shape[0])
     fn = lib.qrec_bpr_sgd_ordered_f64 if f64 else lib.qrec_bpr_sgd_ordered_f32
     check(fn(_dev(P, dt, 'P'), _dev(Q, dt, 'Q'), d, n, _dev(u, torch.int32, 'u'),
              _dev(i, torch.int32, 'i'), _dev(j, torch.int32, 'j'), _dev(wu, torch.int32, 'wu'),
@@ -937,9 +943,7 @@ def mf_sgd_ordered(kind, P, Q, u, i, r, wu, wi, lr, reg_u, reg_i, loss, Bu=None,
     dt = torch.float64 if f64 else torch.float32
     d = P.shape[1]
     assert Q.shape[1] == d and u.shape[0] == i.shape[0] == r.shape[0]
-    ver_p = torch.zeros(P.shape[0], dtype=torch.int32, device=P.device)
-    ver_q = torch.zeros(Q.shape[0], dtype=torch.int32, device=P.device)
-    ticket = torch.zeros(1, dtype=torch.int64, device=P.device)
+    ver_p, ver_q, ticket = _order_counters(P.device, P.shape[0], Q.shape[0])
     fn = lib.qrec_mf_sgd_ordered_f64 if f64 else lib.qrec_mf_sgd_ordered_f32
     check(fn(int(kind), _dev(P, dt, 'P'), _dev(Q, dt, 'Q'), d, u.shape[0], _dev(u, torch.int32, 'u'),
              _dev(i, torch.int32, 'i'), _dev(r, dt, 'r'), _dev(wu, torch.int32, 'wu'), _dev(wi, torch.int32, 'wi'),
@@ -1087,10 +1091,7 @@ def rste_sgd_ordered(P, Q, u, i, r, wu, wi, wr, pos_rowptr, pos, f_rowptr, f_col
     # the kernel bisects pos[pos_rowptr[f] .. pos_rowptr[f+1]): the rows must tile pos
     if int(pos_rowptr[0]) != 0 or int(pos_rowptr[-1]) != n or bool((pos_rowptr[1:] < pos_rowptr[:-1]).any()):
         raise QRecError('%s: pos_rowptr must rise from 0 to len(pos) = %d' % (name, n))
-    ver_p = torch.zeros(P.shape[0], dtype=i32, device=P.device)
-    reads_p = torch.zeros(P.shape[0], dtype=i32, device=P.device)
-    ver_q = torch.zeros(Q.shape[0], dtype=i32, device=P.device)
-    ticket = torch.zeros(1, dtype=torch.int64, device=P.device)
+    ver_p, reads_p, ver_q, ticket = _order_counters(P.device, P.shape[0], P.shape[0], Q.shape[0])
     fn = lib.qrec_rste_sgd_ordered_f64 if P.dtype == torch.float64 else lib.qrec_rste_sgd_ordered_f32
     check(fn(ptr['P'], ptr['Q'], P.shape[1], n, ptr['u'], ptr['i'], ptr['r'], ptr['wu'], ptr['wi'], ptr['wr'],
              ptr['pos_rowptr'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'], ptr['f_w'], ptr['denom'], ver_p.data_ptr(),
@@ -1192,8 +1193,7 @@ def social_user_pass(kind, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_c
     # every wait reads pos: it must name exactly the visit positions
     if int((pos >= 0).sum()) != n or (n and not bool((pos[visit.long()] == torch.arange(n, device=pos.device)).all())):
         raise QRecError('%s: pos does not match the visiting order' % name)
-    done = torch.zeros(U, dtype=i32, device=P.device)
-    ticket = torch.zeros(1, dtype=torch.int64, device=P.device)
+    done, ticket = _order_counters(P.device, U)
     fn = lib.qrec_social_user_pass_f64 if P.dtype == torch.float64 else lib.qrec_social_user_pass_f32
     check(fn(int(kind), ptr['P'], P.shape[1], n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'],
              ptr['f_val'], ptr['g_rowptr'], ptr['g_cols'], ptr.get('g_val'), done.data_ptr(), ticket.data_ptr(),
@@ -1372,7 +1372,7 @@ def cofactor_item_sweep(Y, G, w, c, X, XtX, item_csr, sppmi, lam, gamma, alpha, 
         stamps, sweep = torch.zeros(n_items, dtype=torch.int32, device=Y.device), 1
     elif stamps.shape != (n_items,) or (n_items and not bool((stamps == sweep - 1).all())):
         raise QRecError('cofactor_item_sweep: stamps must hold %d (sweep - 1) for every item' % (sweep - 1))
-    ticket = torch.zeros(1, dtype=torch.int64, device=Y.device)
+    (ticket,) = _order_counters(Y.device)
     fn = lib.qrec_cofactor_item_sweep_f64 if dt == torch.float64 else lib.qrec_cofactor_item_sweep_f32
     with _failures(n_failed, Y.device, 'cofactor_item_sweep: %d system(s) that are not positive definite left their '
                    'rows unchanged') as n_failed:
