@@ -60,7 +60,7 @@ class RatedCSR(object):
         self.sorted_rowptr = np.zeros(self.num_users + 1, dtype=np.int64)
         self.pos_rowptr = np.zeros(self.num_users + 1, dtype=np.int64)
         sorted_cols, pos_cols, possorted_cols = (np.empty(n, dtype=np.int32) for _ in range(3))
-        check(lib.qrec_build_rated_csr(n, _i64p(u_ids), _i64p(i_ids), r.ctypes.data_as(C.POINTER(C.c_double)) if r is not None else None,
+        check(lib.qrec_build_rated_csr(n, _i64p(u_ids), _i64p(i_ids), None if r is None else r.ctypes.data_as(C.POINTER(C.c_double)),
                                        self.num_users, self.num_items, float(positive_threshold), _i64p(self.sorted_rowptr),
                                        _i32p(sorted_cols), _i64p(self.pos_rowptr), _i32p(pos_cols), _i32p(possorted_cols)),
               'qrec_build_rated_csr')
@@ -264,6 +264,87 @@ def _dev(t, dtype, name):
     return t.data_ptr()
 
 
+def _opt(t, dtype, name):
+    return None if t is None else _dev(t, dtype, name)
+
+
+# ---------------------------------------------------------------------------------------------
+# argument checks.  A checking wrapper raises QRecError in three steps: shapes, lengths and dtypes; then that every
+# tensor is a contiguous CUDA tensor (_ptrs); then the contents, which need reductions on the device.  `name` is the
+# wrapper's name and `label` the argument's, as the message shows them.
+# ---------------------------------------------------------------------------------------------
+def _entry(base, dtype):
+    """libqrec's entry point `base` for tables of `dtype`, and the dtype it takes: base_f64 for float64, else base_f32."""
+    torch = _torch()
+    if dtype == torch.float64:
+        return getattr(lib, base + '_f64'), torch.float64
+    return getattr(lib, base + '_f32'), torch.float32
+
+
+def _tables(name, tables, d_max=None, f32=False):
+    """Width d of the 2-D tables `tables` ((tensor, label) pairs): they share one width, 1..d_max when d_max is given,
+    and one dtype, float32 when `f32`, else float32 or float64."""
+    torch = _torch()
+    t0 = tables[0][0]
+    group = ' and '.join(label for _, label in tables)
+    if f32:
+        for t, label in tables:
+            if t.dtype != torch.float32:
+                raise QRecError('%s: %s must be float32, got %s' % (name, label, t.dtype))
+    elif len(tables) == 1:
+        if t0.dtype not in (torch.float32, torch.float64) or t0.dim() != 2:
+            raise QRecError('%s: %s must be a 2-D float32 or float64 table' % (name, group))
+    elif t0.dtype not in (torch.float32, torch.float64) or any(t.dtype != t0.dtype for t, _ in tables):
+        raise QRecError('%s: %s must be float32 or float64 tables of one dtype' % (name, group))
+    if any(t.dim() != 2 for t, _ in tables) or any(t.shape[1] != t0.shape[1] for t, _ in tables):
+        raise QRecError('%s: %s must be 2-D tables of one width' % (name, group))
+    d = t0.shape[1]
+    if d_max is not None and not 1 <= d <= d_max:
+        raise QRecError('%s: d=%d unsupported (1..%d)' % (name, d, d_max))
+    return d
+
+
+def _lengths(name, label, n, *ts):
+    """The arrays `ts` (tensors or numpy arrays) are 1-D with n entries each."""
+    if any(tuple(t.shape) != (n,) for t in ts):
+        raise QRecError('%s: %s %s %d entries' % (name, label, 'needs' if len(ts) == 1 else 'must all hold', n))
+
+
+def _vector(name, label, t, dtype, n=None):
+    """t is a 1-D tensor of `dtype`, with n entries when n is given."""
+    if n is None:
+        if t.dtype != dtype or t.dim() != 1:
+            raise QRecError('%s: %s must be a 1-D %s tensor' % (name, label, str(dtype)[6:]))
+    elif t.dtype != dtype or tuple(t.shape) != (n,):
+        raise QRecError('%s: %s must be %s [%d], got %s %s' % (name, label, str(dtype)[6:], n, t.dtype, tuple(t.shape)))
+
+
+def _ptrs(name, typed):
+    """Device pointers of `typed` ((tensor, dtype, label) triples) by label, after checking every dtype and then that
+    every tensor is a contiguous CUDA tensor.  A None tensor passes as a None pointer."""
+    for t, dt, label in typed:
+        if t is not None and t.dtype != dt:
+            raise QRecError('%s: %s must be %s, got %s' % (name, label, dt, t.dtype))
+    return {label: _opt(t, dt, '%s: %s' % (name, label)) for t, dt, label in typed}
+
+
+def _rowptr(name, label, rowptr, nnz, nnz_label='len(cols)'):
+    """The CSR rowptr rises from 0 to nnz, the length of its column array."""
+    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (rowptr.shape[0] > 1 and bool((rowptr[1:] < rowptr[:-1]).any())):
+        raise QRecError('%s: %s must rise from 0 to %s = %d' % (name, label, nnz_label, nnz))
+
+
+def _bounded(name, message, t, lo=None, hi=None):
+    """Every entry of t lies in [lo, hi), a bound that is None not being checked; else QRecError('name: message')."""
+    if t.numel() and ((lo is not None and int(t.min()) < lo) or (hi is not None and int(t.max()) >= hi)):
+        raise QRecError('%s: %s' % (name, message))
+
+
+def _ids(name, label, ids, hi, lo=0):
+    """Every id lies in [lo, hi): lo = -1 admits the cold marker -1, lo = None sets no lower bound."""
+    _bounded(name, '%s is outside [0, %d)%s' % (label, hi, ' and not -1 (cold)' if lo == -1 else ''), ids, lo, hi)
+
+
 def _stream():
     return _torch().cuda.current_stream().cuda_stream
 
@@ -293,13 +374,11 @@ def bpr_sgd_ordered(P, Q, u, i, j, wu, wi, wj, lr, reg_u, reg_i, loss, n_warps=0
     """Parity mode: sequential-equivalent BPR.optimization over the triples in array order.
     n_warps: pollers to launch (0 = fill the GPU); ~4x the DAG width (n / bpr_order_depth) is best."""
     torch = _torch()
-    f64 = P.dtype == torch.float64
-    dt = torch.float64 if f64 else torch.float32
+    fn, dt = _entry('qrec_bpr_sgd_ordered', P.dtype)
     n = u.shape[0]
     d = P.shape[1]
     assert Q.shape[1] == d
     ver_p, ver_q, ticket = _order_counters(P.device, P.shape[0], Q.shape[0])
-    fn = lib.qrec_bpr_sgd_ordered_f64 if f64 else lib.qrec_bpr_sgd_ordered_f32
     check(fn(_dev(P, dt, 'P'), _dev(Q, dt, 'Q'), d, n, _dev(u, torch.int32, 'u'),
              _dev(i, torch.int32, 'i'), _dev(j, torch.int32, 'j'), _dev(wu, torch.int32, 'wu'),
              _dev(wi, torch.int32, 'wi'), _dev(wj, torch.int32, 'wj'), ver_p.data_ptr(),
@@ -345,7 +424,7 @@ def bpr_epoch_usermajor(P, Q, rowptr, i, rated_rowptr, rated_cols, num_items, se
                                            rowptr.shape[0] - 1, int(i.shape[0]), _dev(rowptr, torch.int64, 'rowptr'),
                                            _dev(i, torch.int32, 'i'), _dev(rated_rowptr, torch.int64, 'rated_rowptr'),
                                            _dev(rated_cols, torch.int32, 'rated_cols'), int(num_items), int(seed),
-                                           int(epoch), _dev(j_out, torch.int32, 'j_out') if j_out is not None else None,
+                                           int(epoch), _opt(j_out, torch.int32, 'j_out'),
                                            float(lr), float(reg_u), float(reg_i), _dev(loss, torch.float64, 'loss'),
                                            _stream()), 'qrec_bpr_epoch_usermajor_f32')
     return loss
@@ -374,7 +453,7 @@ def bpr_epoch_usermajor_sig(P, Q, rowptr, i, rated_rowptr, rated_cols, rated_sig
                                                _dev(i, torch.int32, 'i'), _dev(rated_rowptr, torch.int64, 'rated_rowptr'),
                                                _dev(rated_cols, torch.int32, 'rated_cols'),
                                                _dev(rated_sig, torch.int32, 'rated_sig'), int(num_items), int(seed),
-                                               int(epoch), _dev(j_out, torch.int32, 'j_out') if j_out is not None else None,
+                                               int(epoch), _opt(j_out, torch.int32, 'j_out'),
                                                float(lr), float(reg_u), float(reg_i), _dev(loss, torch.float64, 'loss'),
                                                _stream()), 'qrec_bpr_epoch_usermajor_sig_f32')
     return loss
@@ -406,7 +485,7 @@ def table_delta(Q, B, D, S=None):
     """D = Q - B (and S = D): this rank's not-yet-exchanged item-row updates (csrc/table_sync.cu)."""
     torch = _torch()
     check(lib.qrec_table_delta_f32(_dev(Q, torch.float32, 'Q'), _dev(B, torch.float32, 'B'), _dev(D, torch.float32, 'D'),
-                                   _dev(S, torch.float32, 'S') if S is not None else None, Q.numel(), _stream()),
+                                   _opt(S, torch.float32, 'S'), Q.numel(), _stream()),
           'qrec_table_delta_f32')
 
 
@@ -465,8 +544,8 @@ def adj_normalize(rowptr, cols, pair, pair_w, deg, vals):
     """deg = weighted row sums, vals = D^-1/2 A D^-1/2 entries (fp32, the reference's operand order)."""
     torch = _torch()
     check(lib.qrec_adj_normalize_f32(rowptr.shape[0] - 1, _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'),
-                                     _dev(pair, torch.int32, 'pair') if pair is not None else None,
-                                     _dev(pair_w, torch.float32, 'pair_w') if pair_w is not None else None,
+                                     _opt(pair, torch.int32, 'pair'),
+                                     _opt(pair_w, torch.float32, 'pair_w'),
                                      _dev(deg, torch.float32, 'deg'), _dev(vals, torch.float32, 'vals'), _stream()),
           'qrec_adj_normalize_f32')
     return vals
@@ -484,7 +563,7 @@ def edge_keep_philox(n_lines, drop_rate, seed, tag, epoch, device, out=None):
 def adj_line_weights(line_pair, keep, pair_w):
     torch = _torch()
     check(lib.qrec_adj_line_weights_f32(line_pair.shape[0], _dev(line_pair, torch.int32, 'line_pair'),
-                                        _dev(keep, torch.uint8, 'keep') if keep is not None else None, pair_w.shape[0],
+                                        _opt(keep, torch.uint8, 'keep'), pair_w.shape[0],
                                         _dev(pair_w, torch.float32, 'pair_w'), _stream()), 'qrec_adj_line_weights_f32')
     return pair_w
 
@@ -522,14 +601,14 @@ def gemv_t(A, v, out, alpha=1.0, beta=0.0):
     row slice of a workspace is fine), out [cols]."""
     torch = _torch()
     ptr, ld = _strided_rows(A, 'A')
-    check(lib.qrec_gemv_t_f32(ptr, max(ld, A.shape[1]), A.shape[0], A.shape[1], _dev(v, torch.float32, 'v') if v is not None else None,
+    check(lib.qrec_gemv_t_f32(ptr, max(ld, A.shape[1]), A.shape[0], A.shape[1], _opt(v, torch.float32, 'v'),
                               float(alpha), float(beta), _dev(out, torch.float32, 'out'), _stream()), 'qrec_gemv_t_f32')
     return out
 
 
 def sumsq(x, out):
     torch = _torch()
-    fn = lib.qrec_sumsq_f64 if x.dtype == torch.float64 else lib.qrec_sumsq_f32
+    fn, _ = _entry('qrec_sumsq', x.dtype)
     check(fn(_dev(x, x.dtype, 'x'), x.numel(), _dev(out, torch.float64, 'out'), _stream()), 'qrec_sumsq')
     return out
 
@@ -545,6 +624,15 @@ def table_snapshot(src, dst):
     return dst
 
 
+def _host_ptr(a, dtype_np, dtype_t, name):
+    torch = _torch()
+    if isinstance(a, np.ndarray):
+        assert a.dtype == dtype_np and a.flags.c_contiguous, name
+        return a.ctypes.data, a.shape[0]
+    assert (not a.is_cuda) and a.dtype == dtype_t and a.is_contiguous(), name
+    return a.data_ptr(), a.shape[0]
+
+
 class HostPipeline(object):
     """qrec_ctx: copy/compute pipeline for epochs whose triples live in host memory."""
 
@@ -556,7 +644,7 @@ class HostPipeline(object):
         """sig: rated_signature(...) of ALL users ([n_users, 16] int32 CUDA) or None; kept alive by the pipeline."""
         torch = _torch()
         self._sig = sig
-        check(lib.qrec_ctx_set_rated_signature(self._ctx, _dev(sig, torch.int32, 'rated_sig') if sig is not None else None),
+        check(lib.qrec_ctx_set_rated_signature(self._ctx, _opt(sig, torch.int32, 'rated_sig')),
               'qrec_ctx_set_rated_signature')
 
     def close(self):
@@ -573,17 +661,9 @@ class HostPipeline(object):
     def bpr_epoch(self, P, Q, u, i, j, lr, reg_u, reg_i):
         """u,i,j: host int32 (numpy arrays or CPU torch tensors; pinned gives overlap)."""
         torch = _torch()
-
-        def hp(a, name):
-            if isinstance(a, np.ndarray):
-                assert a.dtype == np.int32 and a.flags.c_contiguous, name
-                return a.ctypes.data, a.shape[0]
-            assert (not a.is_cuda) and a.dtype == torch.int32 and a.is_contiguous(), name
-            return a.data_ptr(), a.shape[0]
-
-        pu, n = hp(u, 'u')
-        pi, ni = hp(i, 'i')
-        pj, nj = hp(j, 'j')
+        pu, n = _host_ptr(u, np.int32, torch.int32, 'u')
+        pi, ni = _host_ptr(i, np.int32, torch.int32, 'i')
+        pj, nj = _host_ptr(j, np.int32, torch.int32, 'j')
         assert n == ni == nj
         torch.cuda.current_stream().synchronize()   # tables may have pending work on torch's stream
         loss = C.c_double(0.0)
@@ -592,33 +672,20 @@ class HostPipeline(object):
                                       C.byref(loss)), 'qrec_bpr_epoch_host')
         return loss.value
 
-
-def _host_ptr(a, dtype_np, dtype_t, name):
-    torch = _torch()
-    if isinstance(a, np.ndarray):
-        assert a.dtype == dtype_np and a.flags.c_contiguous, name
-        return a.ctypes.data, a.shape[0]
-    assert (not a.is_cuda) and a.dtype == dtype_t and a.is_contiguous(), name
-    return a.data_ptr(), a.shape[0]
-
-
-def _bpr_epoch_usermajor_host(self, P, Q, rowptr, i, rated_rowptr, rated_cols, num_items, seed, epoch, lr, reg_u, reg_i):
-    """HostPipeline method: user-major epoch with the positives (CSR: rowptr int64, i int32) in HOST
-    memory (pinned gives overlap) and fused device-side negative sampling; returns sum(-ln s)."""
-    torch = _torch()
-    prp, nr = _host_ptr(rowptr, np.int64, torch.int64, 'rowptr')
-    pi, _ = _host_ptr(i, np.int32, torch.int32, 'i')
-    torch.cuda.current_stream().synchronize()
-    loss = C.c_double(0.0)
-    check(lib.qrec_bpr_epoch_usermajor_host(self._ctx, _dev(P, torch.float32, 'P'), _dev(Q, torch.float32, 'Q'), P.shape[1],
-                                            nr - 1, prp, pi, _dev(rated_rowptr, torch.int64, 'rated_rowptr'),
-                                            _dev(rated_cols, torch.int32, 'rated_cols'), int(num_items), int(seed),
-                                            int(epoch), float(lr), float(reg_u), float(reg_i), C.byref(loss)),
-          'qrec_bpr_epoch_usermajor_host')
-    return loss.value
-
-
-HostPipeline.bpr_epoch_usermajor = _bpr_epoch_usermajor_host
+    def bpr_epoch_usermajor(self, P, Q, rowptr, i, rated_rowptr, rated_cols, num_items, seed, epoch, lr, reg_u, reg_i):
+        """User-major epoch with the positives (CSR: rowptr int64, i int32) in HOST memory (pinned gives overlap) and
+        fused device-side negative sampling; returns sum(-ln s)."""
+        torch = _torch()
+        prp, nr = _host_ptr(rowptr, np.int64, torch.int64, 'rowptr')
+        pi, _ = _host_ptr(i, np.int32, torch.int32, 'i')
+        torch.cuda.current_stream().synchronize()
+        loss = C.c_double(0.0)
+        check(lib.qrec_bpr_epoch_usermajor_host(self._ctx, _dev(P, torch.float32, 'P'), _dev(Q, torch.float32, 'Q'),
+                                                P.shape[1], nr - 1, prp, pi, _dev(rated_rowptr, torch.int64, 'rated_rowptr'),
+                                                _dev(rated_cols, torch.int32, 'rated_cols'), int(num_items), int(seed),
+                                                int(epoch), float(lr), float(reg_u), float(reg_i), C.byref(loss)),
+              'qrec_bpr_epoch_usermajor_host')
+        return loss.value
 
 
 def spmm_csr(rowptr, cols, vals, X, Y, acc=None, acc_scale=0.0, rowsplit=False):
@@ -631,7 +698,7 @@ def spmm_csr(rowptr, cols, vals, X, Y, acc=None, acc_scale=0.0, rowsplit=False):
     check(fn(n_rows, int(cols.shape[0]), _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'),
                                 _dev(vals, torch.float32, 'vals'), _dev(X, torch.float32, 'X'),
                                 _dev(Y, torch.float32, 'Y'), d,
-                                _dev(acc, torch.float32, 'acc') if acc is not None else None,
+                                _opt(acc, torch.float32, 'acc'),
                                 float(acc_scale), _stream()), 'qrec_spmm_csr_f32')
     return Y
 
@@ -646,7 +713,7 @@ def spmm_csr_scatter_rows(rowptr, cols, vals, src_rows, X, Y, acc=None, acc_scal
                                              _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'),
                                              _dev(vals, torch.float32, 'vals'), _dev(X, torch.float32, 'X'),
                                              _dev(Y, torch.float32, 'Y'), X.shape[1],
-                                             _dev(acc, torch.float32, 'acc') if acc is not None else None,
+                                             _opt(acc, torch.float32, 'acc'),
                                              float(acc_scale), _stream()), 'qrec_spmm_csr_scatter_rows_f32')
     return Y
 
@@ -679,9 +746,9 @@ def spmm_csr_rows(rowptr, cols, vals, rows, X, Y=None, compact=False, acc=None, 
     assert Y is not None or acc is not None
     check(lib.qrec_spmm_csr_rows_f32(rows.shape[0], _dev(rows, torch.int32, 'rows'), _dev(rowptr, torch.int64, 'rowptr'),
                                      _dev(cols, torch.int32, 'cols'), _dev(vals, torch.float32, 'vals'),
-                                     _dev(X, torch.float32, 'X'), _dev(Y, torch.float32, 'Y') if Y is not None else None,
+                                     _dev(X, torch.float32, 'X'), _opt(Y, torch.float32, 'Y'),
                                      1 if compact else 0, X.shape[1],
-                                     _dev(acc, torch.float32, 'acc') if acc is not None else None, float(acc_scale),
+                                     _opt(acc, torch.float32, 'acc'), float(acc_scale),
                                      _stream()), 'qrec_spmm_csr_rows_f32')
     return Y
 
@@ -756,7 +823,7 @@ def simgcl_perturb(Emb, eps, seed, tag, step, acc=None, acc_scale=0.0, d_valid=0
     torch = _torch()
     check(lib.qrec_simgcl_perturb_rows_f32(_dev(Emb, torch.float32, 'E'), Emb.shape[0], int(row_offset), Emb.shape[1],
                                            int(d_valid), float(eps), int(seed), int(tag), int(step),
-                                           _dev(acc, torch.float32, 'acc') if acc is not None else None,
+                                           _opt(acc, torch.float32, 'acc'),
                                            float(acc_scale), _stream()), 'qrec_simgcl_perturb_rows_f32')
     return Emb
 
@@ -767,7 +834,7 @@ def simgcl_perturb_listed(Ec, rows, eps, seed, tag, step, acc=None, acc_scale=0.
     torch = _torch()
     check(lib.qrec_simgcl_perturb_listed_f32(_dev(Ec, torch.float32, 'Ec'), _dev(rows, torch.int32, 'rows'), rows.shape[0],
                                              int(row_offset), Ec.shape[1], int(d_valid), float(eps), int(seed), int(tag),
-                                             int(step), _dev(acc, torch.float32, 'acc') if acc is not None else None,
+                                             int(step), _opt(acc, torch.float32, 'acc'),
                                              float(acc_scale), _stream()), 'qrec_simgcl_perturb_listed_f32')
     return Ec
 
@@ -830,7 +897,7 @@ def ngcf_act_bwd(dOut, dH_extra, H, Z, norms, keep, training, seed, tag, step, d
     torch = _torch()
     pd, ldd = _strided_rows(dOut, 'dOut')
     check(lib.qrec_ngcf_act_bwd_f32(pd, ldd,
-                                    _dev(dH_extra, torch.float32, 'dH_extra') if dH_extra is not None else None,
+                                    _opt(dH_extra, torch.float32, 'dH_extra'),
                                     _dev(H, torch.float32, 'H'), _dev(Z, torch.float32, 'Z'),
                                     _dev(norms, torch.float32, 'norms'), Z.shape[0], Z.shape[1], float(keep),
                                     int(training), int(seed), int(tag), int(step), _dev(dZ, torch.float32, 'dZ'),
@@ -861,8 +928,8 @@ def tc_gemm(A, B, C, b_is_nk=False, epilogue=EPI_NONE, bias=None, mask=None):
     assert (B.shape[1] if b_is_nk else B.shape[0]) == K and tuple(C.shape) == (M, N)
     check(lib.qrec_tc_gemm_tf32(int(b_is_nk), M, N, K, _dev(A, torch.float32, 'A'), _ld(A),
                                 _dev(B, torch.float32, 'B'), _ld(B), _dev(C, torch.float32, 'C'), _ld(C),
-                                int(epilogue), _dev(bias, torch.float32, 'bias') if bias is not None else None,
-                                _dev(mask, torch.float32, 'mask') if mask is not None else None,
+                                int(epilogue), _opt(bias, torch.float32, 'bias'),
+                                _opt(mask, torch.float32, 'mask'),
                                 _ld(mask) if mask is not None else 0, _stream()), 'qrec_tc_gemm_tf32')
     return C
 
@@ -876,8 +943,8 @@ def tc_gemm_v2(A, B, C, b_is_nk=False, epilogue=EPI_NONE, bias=None, mask=None):
     assert (B.shape[1] if b_is_nk else B.shape[0]) == K and tuple(C.shape) == (M, N)
     check(lib.qrec_tc_gemm_tf32_v2(int(b_is_nk), M, N, K, _dev(A, torch.float32, 'A'), _ld(A),
                                    _dev(B, torch.float32, 'B'), _ld(B), _dev(C, torch.float32, 'C'), _ld(C),
-                                   int(epilogue), _dev(bias, torch.float32, 'bias') if bias is not None else None,
-                                   _dev(mask, torch.float32, 'mask') if mask is not None else None,
+                                   int(epilogue), _opt(bias, torch.float32, 'bias'),
+                                   _opt(mask, torch.float32, 'mask'),
                                    _ld(mask) if mask is not None else 0, _stream()), 'qrec_tc_gemm_tf32_v2')
     return C
 
@@ -901,12 +968,12 @@ def scatter_add_rows(G, idx, src, scale=1.0):
 
 def neumf_head(mode, training, UG, IG, H3, h_mf, h_mlp, r, reg, loss, y, dz, GMF, dUG, dIG, dH3):
     torch = _torch()
-    f = lambda t, n: _dev(t, torch.float32, n) if t is not None else None      # noqa: E731
+    f = lambda t, n: _opt(t, torch.float32, n)      # noqa: E731
     n = (UG if UG is not None else H3).shape[0]
     d = (UG if UG is not None else H3).shape[1]
     check(lib.qrec_neumf_head_f32(int(mode), int(training), f(UG, 'UG'), f(IG, 'IG'), f(H3, 'H3'), f(h_mf, 'h_mf'),
                                   f(h_mlp, 'h_mlp'), f(r, 'r'), n, d, float(reg),
-                                  _dev(loss, torch.float64, 'loss') if loss is not None else None,
+                                  _opt(loss, torch.float64, 'loss'),
                                   f(y, 'y'), f(dz, 'dz'), f(GMF, 'GMF'), f(dUG, 'dUG'), f(dIG, 'dIG'), f(dH3, 'dH3'),
                                   _stream()), 'qrec_neumf_head_f32')
 
@@ -927,24 +994,27 @@ SOREC_EDGES = 3    # kind 3: SoRec's trust-edge pass on (P, Z), regS / regZ in t
 SOCIALMF_RATINGS = 4    # kind 4: SocialMF's rating pass, kind 1 on copies of both rows
 
 
-def _opt(t, dtype, name):
-    return _dev(t, dtype, name) if t is not None else None
-
-
 def mf_sgd_ordered(kind, P, Q, u, i, r, wu, wi, lr, reg_u, reg_i, loss, Bu=None, Bi=None, reg_b=0.0,
                    global_mean=0.0, n_warps=0):
     """Parity mode: sequential-equivalent pass over the entries (u, i, r) in array order."""
     torch = _torch()
-    if kind == SOREC_EDGES:
-        _sorec_edge_checks(P, Q, u, i, r, wu, wi, Bu, Bi)
+    name = 'mf_sgd_ordered'
+    if kind == SOREC_EDGES:     # kind 3 runs SoRec's edge pass on the tables (P, Z)
+        if Bu is not None or Bi is not None:
+            raise QRecError('%s: kind 3 (SoRec edges) takes no bias vectors' % name)
+        _tables(name, ((P, 'P'), (Q, 'Z')), 256)
+        _lengths(name, 'u, v, r and the wait arrays', u.shape[0], i, r, wu, wi)
+        if r.dtype != P.dtype:
+            raise QRecError('%s: r must be %s, got %s' % (name, P.dtype, r.dtype))
+        # the edge ids come before the device check, so that a bad edge list names itself whatever device it is on
+        _ids(name, 'an edge source', u, P.shape[0])
+        _ids(name, 'an edge target', i, Q.shape[0])
     if kind == SOCIALMF_RATINGS and (Bu is not None or Bi is not None):
-        raise QRecError('mf_sgd_ordered: kind 4 (SocialMF ratings) takes no bias vectors')
-    f64 = P.dtype == torch.float64
-    dt = torch.float64 if f64 else torch.float32
+        raise QRecError('%s: kind 4 (SocialMF ratings) takes no bias vectors' % name)
+    fn, dt = _entry('qrec_mf_sgd_ordered', P.dtype)
     d = P.shape[1]
     assert Q.shape[1] == d and u.shape[0] == i.shape[0] == r.shape[0]
     ver_p, ver_q, ticket = _order_counters(P.device, P.shape[0], Q.shape[0])
-    fn = lib.qrec_mf_sgd_ordered_f64 if f64 else lib.qrec_mf_sgd_ordered_f32
     check(fn(int(kind), _dev(P, dt, 'P'), _dev(Q, dt, 'Q'), d, u.shape[0], _dev(u, torch.int32, 'u'),
              _dev(i, torch.int32, 'i'), _dev(r, dt, 'r'), _dev(wu, torch.int32, 'wu'), _dev(wi, torch.int32, 'wi'),
              ver_p.data_ptr(), ver_q.data_ptr(), ticket.data_ptr(), float(lr), float(reg_u), float(reg_i),
@@ -970,39 +1040,12 @@ def mf_sgd_batch(kind, P, Q, u, i, r, lr, reg_u, reg_i, loss, Bu=None, Bi=None, 
     return loss
 
 
-def _sorec_edge_checks(P, Z, u, v, r, wu, wv, Bu, Bi):
-    """QRecError on what kind 3 (SoRec's edge pass on the tables (P, Z)) cannot take."""
-    torch = _torch()
-    if Bu is not None or Bi is not None:
-        raise QRecError('mf_sgd_ordered: kind 3 (SoRec edges) takes no bias vectors')
-    if P.dtype not in (torch.float32, torch.float64) or Z.dtype != P.dtype:
-        raise QRecError('mf_sgd_ordered: P and Z must be float32 or float64 tables of one dtype')
-    if P.dim() != 2 or Z.dim() != 2 or Z.shape[1] != P.shape[1]:
-        raise QRecError('mf_sgd_ordered: P and Z must be 2-D tables of one width')
-    if not 1 <= P.shape[1] <= 256:
-        raise QRecError('mf_sgd_ordered: d=%d unsupported (1..256)' % P.shape[1])
-    n = u.shape[0]
-    if any(t.dim() != 1 or t.shape[0] != n for t in (v, r, wu, wv)):
-        raise QRecError('mf_sgd_ordered: u, v, r and the wait arrays must all hold %d entries' % n)
-    if r.dtype != P.dtype:
-        raise QRecError('mf_sgd_ordered: r must be %s, got %s' % (P.dtype, r.dtype))
-    _ids_below(u, P.shape[0], 'mf_sgd_ordered: an edge source is outside [0, %d)')
-    _ids_below(v, Z.shape[0], 'mf_sgd_ordered: an edge target is outside [0, %d)')
-
-
-def _ids_below(ids, bound, message):
-    if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= bound):
-        raise QRecError(message % bound)
-
-
 def mf_predict_pairs(P, Q, u, i, Bu=None, Bi=None, global_mean=0.0, out=None):
     """out[k] = P[u[k]].Q[i[k]] (+ global_mean + Bi + Bu): predictForRating for known pairs."""
     torch = _torch()
-    f64 = P.dtype == torch.float64
-    dt = torch.float64 if f64 else torch.float32
+    fn, dt = _entry('qrec_mf_predict_pairs', P.dtype)
     if out is None:
         out = torch.empty(u.shape[0], dtype=dt, device=P.device)
-    fn = lib.qrec_mf_predict_pairs_f64 if f64 else lib.qrec_mf_predict_pairs_f32
     check(fn(_dev(P, dt, 'P'), _dev(Q, dt, 'Q'), P.shape[1], u.shape[0], _dev(u, torch.int32, 'u'),
              _dev(i, torch.int32, 'i'), _opt(Bu, dt, 'Bu'), _opt(Bi, dt, 'Bi'), float(global_mean),
              _dev(out, dt, 'out'), _stream()), 'qrec_mf_predict_pairs')
@@ -1022,8 +1065,7 @@ def rste_order_prepare(u, i, num_users, num_items, f_rowptr, f_cols):
     n = u.shape[0]
     if i.shape[0] != n:
         raise QRecError('rste_order_prepare: u and i differ in length')
-    if f_rowptr.shape != (int(num_users) + 1,):
-        raise QRecError('rste_order_prepare: the followee rowptr needs %d entries' % (int(num_users) + 1))
+    _lengths('rste_order_prepare', 'the followee rowptr', int(num_users) + 1, f_rowptr)
     if f_rowptr[-1] != f_cols.shape[0]:
         raise QRecError('rste_order_prepare: the followee rowptr ends at %d, not at len(f_cols) = %d'
                         % (f_rowptr[-1], f_cols.shape[0]))
@@ -1036,37 +1078,6 @@ def rste_order_prepare(u, i, num_users, num_items, f_rowptr, f_cols):
     return wu, wi, wr, pos_rowptr, pos, int(depth[0])
 
 
-def _rste_checks(name, P, Q, f_rowptr, f_cols, f_w, denom, typed):
-    """QRecError unless (P, Q) are tables of one float dtype and width 1..256, the followee CSR and denom describe P's
-    users, and every tensor of `typed` ((tensor, dtype, name) triples, the entry arrays) has its dtype.  Shapes and
-    dtypes are checked first, then that every tensor is a contiguous CUDA tensor, then the contents: the CSR's rowptr
-    rises from 0 to len(f_cols) and every followee id names a user.  Returns the CUDA tensors' pointers."""
-    torch = _torch()
-    if P.dtype not in (torch.float32, torch.float64) or Q.dtype != P.dtype:
-        raise QRecError('%s: P and Q must be float32 or float64 tables of one dtype' % name)
-    if P.dim() != 2 or Q.dim() != 2 or Q.shape[1] != P.shape[1]:
-        raise QRecError('%s: P and Q must be 2-D tables of one width' % name)
-    if not 1 <= P.shape[1] <= 256:
-        raise QRecError('%s: d=%d unsupported (1..256)' % (name, P.shape[1]))
-    U = P.shape[0]
-    if denom.dim() != 1 or denom.shape[0] != U:
-        raise QRecError('%s: denom needs one entry per user (%d), got %d' % (name, U, denom.numel()))
-    if f_rowptr.dim() != 1 or f_rowptr.shape[0] != U + 1:
-        raise QRecError('%s: the followee rowptr needs %d entries' % (name, U + 1))
-    if f_cols.dim() != 1 or f_w.dim() != 1 or f_w.shape[0] != f_cols.shape[0]:
-        raise QRecError('%s: followee ids and weights differ in length' % name)
-    tensors = [(P, P.dtype, 'P'), (Q, P.dtype, 'Q'), (f_rowptr, torch.int64, 'f_rowptr'), (f_cols, torch.int32, 'f_cols'),
-               (f_w, P.dtype, 'f_w'), (denom, P.dtype, 'denom')] + list(typed)
-    for t, dt, tname in tensors:
-        if t.dtype != dt:
-            raise QRecError('%s: %s must be %s, got %s' % (name, tname, dt, t.dtype))
-    ptrs = {tname: _dev(t, dt, '%s: %s' % (name, tname)) for t, dt, tname in tensors}
-    if int(f_rowptr[0]) != 0 or int(f_rowptr[-1]) != f_cols.shape[0] or bool((f_rowptr[1:] < f_rowptr[:-1]).any()):
-        raise QRecError('%s: the followee rowptr must rise from 0 to len(f_cols) = %d' % (name, f_cols.shape[0]))
-    _ids_below(f_cols, U, name + ': a followee is outside [0, %d)')
-    return ptrs
-
-
 def rste_sgd_ordered(P, Q, u, i, r, wu, wi, wr, pos_rowptr, pos, f_rowptr, f_cols, f_w, denom, lr, reg_u, reg_i,
                      alpha, loss, n_warps=0):
     """RSTE's rating pass over the entries (u, i, r) in array order, sequential-equivalent, in place on P and Q
@@ -1074,25 +1085,25 @@ def rste_sgd_ordered(P, Q, u, i, r, wu, wi, wr, pos_rowptr, pos, f_rowptr, f_col
     (f_rowptr int64, f_cols int32, f_w the weights); denom[u]: the sum of u's weights.  loss (float64) += sum e^2."""
     torch = _torch()
     name = 'rste_sgd_ordered'
-    n = u.shape[0]
-    if any(t.dim() != 1 or t.shape[0] != n for t in (u, i, r, wu, wi, wr, pos)):
-        raise QRecError('%s: u, i, r, the wait arrays and pos must all hold %d entries' % (name, n))
-    if pos_rowptr.dim() != 1 or pos_rowptr.shape[0] != P.shape[0] + 1:
-        raise QRecError('%s: pos_rowptr needs %d entries' % (name, P.shape[0] + 1))
+    n, U = u.shape[0], P.shape[0]
+    _lengths(name, 'u, i, r, the wait arrays and pos', n, u, i, r, wu, wi, wr, pos)
+    _lengths(name, 'pos_rowptr', U + 1, pos_rowptr)
     if loss.numel() < 1:
         raise QRecError('%s: loss needs one entry' % name)
-    i32 = torch.int32
-    ptr = _rste_checks(name, P, Q, f_rowptr, f_cols, f_w, denom,
-                       [(u, i32, 'u'), (i, i32, 'i'), (r, P.dtype, 'r'), (wu, i32, 'wu'), (wi, i32, 'wi'),
-                        (wr, i32, 'wr'), (pos_rowptr, torch.int64, 'pos_rowptr'), (pos, i32, 'pos'),
-                        (loss, torch.float64, 'loss')])
-    _ids_below(u, P.shape[0], name + ': a user id is outside [0, %d)')
-    _ids_below(i, Q.shape[0], name + ': an item id is outside [0, %d)')
+    _rste_followees(name, P, Q, f_rowptr, f_cols, f_w, denom)
+    i32, dt = torch.int32, P.dtype
+    ptr = _ptrs(name, [(P, dt, 'P'), (Q, dt, 'Q'), (f_rowptr, torch.int64, 'f_rowptr'), (f_cols, i32, 'f_cols'),
+                       (f_w, dt, 'f_w'), (denom, dt, 'denom'), (u, i32, 'u'), (i, i32, 'i'), (r, dt, 'r'),
+                       (wu, i32, 'wu'), (wi, i32, 'wi'), (wr, i32, 'wr'), (pos_rowptr, torch.int64, 'pos_rowptr'),
+                       (pos, i32, 'pos'), (loss, torch.float64, 'loss')])
+    _rowptr(name, 'the followee rowptr', f_rowptr, f_cols.shape[0], 'len(f_cols)')
+    _ids(name, 'a followee', f_cols, U)
+    _ids(name, 'a user id', u, U)
+    _ids(name, 'an item id', i, Q.shape[0])
     # the kernel bisects pos[pos_rowptr[f] .. pos_rowptr[f+1]): the rows must tile pos
-    if int(pos_rowptr[0]) != 0 or int(pos_rowptr[-1]) != n or bool((pos_rowptr[1:] < pos_rowptr[:-1]).any()):
-        raise QRecError('%s: pos_rowptr must rise from 0 to len(pos) = %d' % (name, n))
-    ver_p, reads_p, ver_q, ticket = _order_counters(P.device, P.shape[0], P.shape[0], Q.shape[0])
-    fn = lib.qrec_rste_sgd_ordered_f64 if P.dtype == torch.float64 else lib.qrec_rste_sgd_ordered_f32
+    _rowptr(name, 'pos_rowptr', pos_rowptr, n, 'len(pos)')
+    ver_p, reads_p, ver_q, ticket = _order_counters(P.device, U, U, Q.shape[0])
+    fn, _ = _entry('qrec_rste_sgd_ordered', dt)
     check(fn(ptr['P'], ptr['Q'], P.shape[1], n, ptr['u'], ptr['i'], ptr['r'], ptr['wu'], ptr['wi'], ptr['wr'],
              ptr['pos_rowptr'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'], ptr['f_w'], ptr['denom'], ver_p.data_ptr(),
              ver_q.data_ptr(), reads_p.data_ptr(), ticket.data_ptr(), float(lr), float(reg_u), float(reg_i),
@@ -1107,18 +1118,34 @@ def rste_predict_pairs(P, Q, u, i, f_rowptr, f_cols, f_w, denom, alpha, out=None
     name = 'rste_predict_pairs'
     if u.dim() != 1 or i.dim() != 1 or i.shape[0] != u.shape[0]:
         raise QRecError('%s: u and i differ in length' % name)
-    if out is not None and out.shape != u.shape:
-        raise QRecError('%s: out needs %d entries' % (name, u.shape[0]))
-    typed = [(u, torch.int32, 'u'), (i, torch.int32, 'i')] + ([(out, P.dtype, 'out')] if out is not None else [])
-    ptr = _rste_checks(name, P, Q, f_rowptr, f_cols, f_w, denom, typed)
-    _ids_below(u, P.shape[0], name + ': a user id is outside [0, %d)')
-    _ids_below(i, Q.shape[0], name + ': an item id is outside [0, %d)')
+    if out is not None:
+        _lengths(name, 'out', u.shape[0], out)
+    _rste_followees(name, P, Q, f_rowptr, f_cols, f_w, denom)
+    dt = P.dtype
+    ptr = _ptrs(name, [(P, dt, 'P'), (Q, dt, 'Q'), (f_rowptr, torch.int64, 'f_rowptr'), (f_cols, torch.int32, 'f_cols'),
+                       (f_w, dt, 'f_w'), (denom, dt, 'denom'), (u, torch.int32, 'u'), (i, torch.int32, 'i'),
+                       (out, dt, 'out')])
+    _rowptr(name, 'the followee rowptr', f_rowptr, f_cols.shape[0], 'len(f_cols)')
+    _ids(name, 'a followee', f_cols, P.shape[0])
+    _ids(name, 'a user id', u, P.shape[0])
+    _ids(name, 'an item id', i, Q.shape[0])
     if out is None:
-        out = torch.empty(u.shape[0], dtype=P.dtype, device=P.device)
-    fn = lib.qrec_rste_predict_pairs_f64 if P.dtype == torch.float64 else lib.qrec_rste_predict_pairs_f32
+        out = torch.empty(u.shape[0], dtype=dt, device=P.device)
+    fn, _ = _entry('qrec_rste_predict_pairs', dt)
     check(fn(ptr['P'], ptr['Q'], P.shape[1], u.shape[0], ptr['u'], ptr['i'], ptr['f_rowptr'], ptr['f_cols'],
              ptr['f_w'], ptr['denom'], float(alpha), out.data_ptr(), _stream()), 'qrec_rste_predict_pairs')
     return out
+
+
+def _rste_followees(name, P, Q, f_rowptr, f_cols, f_w, denom):
+    """The shapes both RSTE wrappers check: (P, Q) tables of width 1..256, and the followee CSR and denom of P's users."""
+    _tables(name, ((P, 'P'), (Q, 'Q')), 256)
+    U = P.shape[0]
+    if denom.dim() != 1 or denom.shape[0] != U:
+        raise QRecError('%s: denom needs one entry per user (%d), got %d' % (name, U, denom.numel()))
+    _lengths(name, 'the followee rowptr', U + 1, f_rowptr)
+    if f_cols.dim() != 1 or f_w.dim() != 1 or f_w.shape[0] != f_cols.shape[0]:
+        raise QRecError('%s: followee ids and weights differ in length' % name)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1136,8 +1163,7 @@ def social_order_prepare(visit, num_users, f_rowptr, f_cols, g_rowptr, g_cols):
     f_cols, g_cols = (np.ascontiguousarray(a, dtype=np.int32) for a in (f_cols, g_cols))
     U = int(num_users)
     for rp, side in ((f_rowptr, 'followee'), (g_rowptr, 'follower')):
-        if rp.shape != (U + 1,):
-            raise QRecError('social_order_prepare: the %s rowptr needs %d entries' % (side, U + 1))
+        _lengths('social_order_prepare', 'the %s rowptr' % side, U + 1, rp)
     if visit.ndim != 1 or visit.shape[0] > U:
         raise QRecError('social_order_prepare: the visiting order lists %d users, more than %d' % (visit.size, U))
     pos, depth = np.empty(U, np.int32), np.zeros(1, np.int64)
@@ -1160,43 +1186,34 @@ def social_user_pass(kind, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_c
         raise QRecError('%s: kind must be 0 (SocialMF) or 1 (SoReg), got %r' % (name, kind))
     if kind == 1 and g_val is None:
         raise QRecError('%s: SoReg needs the followers\' similarities (g_val)' % name)
-    if P.dtype not in (torch.float32, torch.float64) or P.dim() != 2:
-        raise QRecError('%s: P must be a 2-D float32 or float64 table' % name)
-    if not 1 <= P.shape[1] <= 256:
-        raise QRecError('%s: d=%d unsupported (1..256)' % (name, P.shape[1]))
+    d = _tables(name, ((P, 'P'),), 256)
     U = P.shape[0]
     if visit.dim() != 1 or visit.shape[0] > U:
         raise QRecError('%s: the visiting order must be 1-D and list at most %d users' % (name, U))
     if pos.shape != (U,):
         raise QRecError('%s: pos needs one entry per user (%d)' % (name, U))
     for rp, cols, val, side in ((f_rowptr, f_cols, f_val, 'followee'), (g_rowptr, g_cols, g_val, 'follower')):
-        if rp.dim() != 1 or rp.shape[0] != U + 1:
-            raise QRecError('%s: the %s rowptr needs %d entries' % (name, side, U + 1))
+        _lengths(name, 'the %s rowptr' % side, U + 1, rp)
         if cols.dim() != 1 or (val is not None and val.shape != cols.shape):
             raise QRecError('%s: %s ids and values differ in length' % (name, side))
     if loss.numel() < 1:
         raise QRecError('%s: loss needs one entry' % name)
-    i32, i64 = torch.int32, torch.int64
-    tensors = [(P, P.dtype, 'P'), (visit, i32, 'visit'), (pos, i32, 'pos'), (f_rowptr, i64, 'f_rowptr'),
-               (f_cols, i32, 'f_cols'), (f_val, P.dtype, 'f_val'), (g_rowptr, i64, 'g_rowptr'), (g_cols, i32, 'g_cols'),
-               (loss, torch.float64, 'loss')] + ([(g_val, P.dtype, 'g_val')] if g_val is not None else [])
-    for t, dt, tname in tensors:
-        if t.dtype != dt:
-            raise QRecError('%s: %s must be %s, got %s' % (name, tname, dt, t.dtype))
-    ptr = {tname: _dev(t, dt, '%s: %s' % (name, tname)) for t, dt, tname in tensors}
+    i32, i64, dt = torch.int32, torch.int64, P.dtype
+    ptr = _ptrs(name, [(P, dt, 'P'), (visit, i32, 'visit'), (pos, i32, 'pos'), (f_rowptr, i64, 'f_rowptr'),
+                       (f_cols, i32, 'f_cols'), (f_val, dt, 'f_val'), (g_rowptr, i64, 'g_rowptr'), (g_cols, i32, 'g_cols'),
+                       (loss, torch.float64, 'loss'), (g_val, dt, 'g_val')])
     n = visit.shape[0]
-    _ids_below(visit, U, name + ': a visited user is outside [0, %d)')
+    _ids(name, 'a visited user', visit, U)
     for rp, cols, side in ((f_rowptr, f_cols, 'followee'), (g_rowptr, g_cols, 'follower')):
-        if int(rp[0]) != 0 or int(rp[-1]) != cols.shape[0] or bool((rp[1:] < rp[:-1]).any()):
-            raise QRecError('%s: the %s rowptr must rise from 0 to len = %d' % (name, side, cols.shape[0]))
-        _ids_below(cols, U, name + ': a ' + side + ' is outside [0, %d)')
+        _rowptr(name, 'the %s rowptr' % side, rp, cols.shape[0], 'len')
+        _ids(name, 'a ' + side, cols, U)
     # every wait reads pos: it must name exactly the visit positions
     if int((pos >= 0).sum()) != n or (n and not bool((pos[visit.long()] == torch.arange(n, device=pos.device)).all())):
         raise QRecError('%s: pos does not match the visiting order' % name)
     done, ticket = _order_counters(P.device, U)
-    fn = lib.qrec_social_user_pass_f64 if P.dtype == torch.float64 else lib.qrec_social_user_pass_f32
-    check(fn(int(kind), ptr['P'], P.shape[1], n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'],
-             ptr['f_val'], ptr['g_rowptr'], ptr['g_cols'], ptr.get('g_val'), done.data_ptr(), ticket.data_ptr(),
+    fn, _ = _entry('qrec_social_user_pass', dt)
+    check(fn(int(kind), ptr['P'], d, n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'],
+             ptr['f_val'], ptr['g_rowptr'], ptr['g_cols'], ptr['g_val'], done.data_ptr(), ticket.data_ptr(),
              float(lr), float(coef), ptr['loss'], int(n_warps), _stream()), 'qrec_social_user_pass')
     return loss
 
@@ -1243,7 +1260,7 @@ def als_gram(Z, G=None, workspace=None):
         G = torch.empty(d, d, dtype=torch.float64, device=Z.device)
     if workspace is None:
         workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=Z.device)
-    fn = lib.qrec_als_gram_f64 if Z.dtype == torch.float64 else lib.qrec_als_gram_f32
+    fn, _ = _entry('qrec_als_gram', Z.dtype)
     check(fn(_dev(Z, Z.dtype, 'Z'), n, d, _dev(G, torch.float64, 'G'), _dev(workspace, torch.uint8, 'workspace'),
              workspace.numel(), _stream()), 'qrec_als_gram')
     return G
@@ -1262,7 +1279,7 @@ def als_solve_rows(X, Z, G, rowptr, cols, vals, lam, alpha, row_order, loss=None
     dt = X.dtype
     if Z.shape[1] != d:
         raise QRecError('X and Z differ in width (%d, %d)' % (d, Z.shape[1]))
-    fn = lib.qrec_als_solve_rows_f64 if dt == torch.float64 else lib.qrec_als_solve_rows_f32
+    fn, _ = _entry('qrec_als_solve_rows', dt)
     with _failures(n_failed, X.device, 'als_solve_rows: %d ' + _ROWS_FAILED) as n_failed:
         check(fn(_dev(X, dt, 'X'), _dev(Z, dt, 'Z'), _dev(G, torch.float64, 'G'), d, row_order.shape[0],
                  _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
@@ -1289,8 +1306,7 @@ def cooc_count(item_rowptr, item_users, num_users, filt):
     if nnz == 0:                                  # no ratings: no pairs
         return (torch.zeros(n_items + 1, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev),
                 torch.empty(0, dtype=torch.int32, device=dev))
-    if int(item_users.min()) < 0 or int(item_users.max()) >= num_users:
-        raise QRecError('cooc_count: a user id is outside [0, %d)' % num_users)
+    _ids('cooc_count', 'a user id', item_users, num_users)
     deg = item_rowptr[1:] - item_rowptr[:-1]
     item_of = torch.repeat_interleave(torch.arange(n_items, dtype=torch.int32, device=dev), deg, output_size=nnz)
     # user-major transpose with ascending items: the item-major entries are in item order, the sort is stable
@@ -1368,53 +1384,43 @@ def cofactor_item_sweep(Y, G, w, c, X, XtX, item_csr, sppmi, lam, gamma, alpha, 
         raise QRecError('cofactor_item_sweep: item and SPPMI rowptrs need %d entries' % (n_items + 1))
     if icol.shape[0] != ival.shape[0] or scol.shape[0] != sval.shape[0]:
         raise QRecError('cofactor_item_sweep: cols and vals differ in length')
-    if stamps is None:
+    stamps_message = 'cofactor_item_sweep: stamps must hold %d (sweep - 1) for every item' % (sweep - 1)
+    given = stamps is not None
+    if not given:
         stamps, sweep = torch.zeros(n_items, dtype=torch.int32, device=Y.device), 1
-    elif stamps.shape != (n_items,) or (n_items and not bool((stamps == sweep - 1).all())):
-        raise QRecError('cofactor_item_sweep: stamps must hold %d (sweep - 1) for every item' % (sweep - 1))
+    elif stamps.shape != (n_items,):
+        raise QRecError(stamps_message)
+    i32, i64 = torch.int32, torch.int64
+    ptr = _ptrs('cofactor_item_sweep', [
+        (Y, dt, 'Y'), (G, dt, 'G'), (w, dt, 'w'), (c, dt, 'c'), (X, dt, 'X'), (XtX, torch.float64, 'XtX'),
+        (irp, i64, 'item rowptr'), (icol, i32, 'item users'), (ival, dt, 'item ratings'), (srp, i64, 'SPPMI rowptr'),
+        (scol, i32, 'SPPMI cols'), (sval, dt, 'SPPMI vals'), (stamps, i32, 'stamps')])
+    if given and n_items and not bool((stamps == sweep - 1).all()):
+        raise QRecError(stamps_message)
     (ticket,) = _order_counters(Y.device)
-    fn = lib.qrec_cofactor_item_sweep_f64 if dt == torch.float64 else lib.qrec_cofactor_item_sweep_f32
+    fn, _ = _entry('qrec_cofactor_item_sweep', dt)
     with _failures(n_failed, Y.device, 'cofactor_item_sweep: %d system(s) that are not positive definite left their '
                    'rows unchanged') as n_failed:
-        check(fn(_dev(Y, dt, 'Y'), _dev(G, dt, 'G'), _dev(w, dt, 'w'), _dev(c, dt, 'c'), _dev(X, dt, 'X'),
-                 _dev(XtX, torch.float64, 'XtX'), d, n_items, _dev(irp, torch.int64, 'item rowptr'),
-                 _dev(icol, torch.int32, 'item users'), _dev(ival, dt, 'item ratings'),
-                 _dev(srp, torch.int64, 'SPPMI rowptr'), _dev(scol, torch.int32, 'SPPMI cols'),
-                 _dev(sval, dt, 'SPPMI vals'), float(lam), float(gamma), float(alpha),
-                 _dev(stamps, torch.int32, 'stamps'), int(sweep), ticket.data_ptr(),
-                 _dev(n_failed, torch.int32, 'n_failed'), _stream()), 'qrec_cofactor_item_sweep')
+        check(fn(ptr['Y'], ptr['G'], ptr['w'], ptr['c'], ptr['X'], ptr['XtX'], d, n_items, ptr['item rowptr'],
+                 ptr['item users'], ptr['item ratings'], ptr['SPPMI rowptr'], ptr['SPPMI cols'], ptr['SPPMI vals'],
+                 float(lam), float(gamma), float(alpha), ptr['stamps'], int(sweep), ticket.data_ptr(),
+                 _dev(n_failed, i32, 'n_failed'), _stream()), 'qrec_cofactor_item_sweep')
     return Y
 
 
 # =============================================================================================
 # K13: ExpoMF -- exposure posterior and weighted normal equations, fused per row
 # =============================================================================================
-def _exposure_checks(name, X, Z, rowptr, cols, row_order):
-    """The checks expomf_half_epoch and serec_half_epoch (`name`) share: X [n, d] and Z [m, d] float32 and not one
-    table, 1 <= d <= 128, and a CSR of n rows into [0, m) with row_order a list of its rows.  Returns (n, d, m)."""
-    f32 = _torch().float32
-    for t, tname in ((X, 'X'), (Z, 'Z')):
-        if t.dtype != f32:
-            raise QRecError('%s: %s must be float32, got %s' % (name, tname, t.dtype))
-    if X.dim() != 2 or Z.dim() != 2 or Z.shape[1] != X.shape[1]:
-        raise QRecError('%s: X and Z must be 2-D tables of one width' % name)
-    n, d = X.shape
-    m = Z.shape[0]
-    if not 1 <= d <= 128:
-        raise QRecError('%s: d=%d unsupported (1..128)' % (name, d))
+def _exposure_shapes(name, X, Z, rowptr, row_order):
+    """The shapes expomf_half_epoch and serec_half_epoch (`name`) share: X [n, d] and Z [m, d] float32 and not one
+    table, 1 <= d <= 128, a rowptr of n rows, and row_order a list of at most n rows.  Returns (n, d, m)."""
+    d = _tables(name, ((X, 'X'), (Z, 'Z')), 128, f32=True)
+    n, m = X.shape[0], Z.shape[0]
     if X.data_ptr() == Z.data_ptr():
         raise QRecError('%s: X and Z must be different tables' % name)
-    if rowptr.shape != (n + 1,):
-        raise QRecError('%s: rowptr needs %d entries' % (name, n + 1))
+    _lengths(name, 'rowptr', n + 1, rowptr)
     if row_order.dim() != 1 or row_order.shape[0] > n:
         raise QRecError('%s: row_order must be a list of at most %d rows' % (name, n))
-    if row_order.numel() and (int(row_order.min()) < 0 or int(row_order.max()) >= n):
-        raise QRecError('%s: a row of row_order is outside [0, %d)' % (name, n))
-    nnz = cols.shape[0]
-    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
-        raise QRecError('%s: rowptr must rise from 0 to len(cols) = %d' % (name, nnz))
-    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= m):
-        raise QRecError('%s: a column is outside [0, %d)' % (name, m))
     return n, d, m
 
 
@@ -1431,10 +1437,10 @@ def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, 
     optional int32 CUDA tensor counting rows whose system was not positive definite (left unchanged); when it is not
     given, the count is read back here and a failed row raises QRecError."""
     torch = _torch()
-    f32 = torch.float32
-    n, d, m = _exposure_checks('expomf_half_epoch', X, Z, rowptr, cols, row_order)
+    f32, name = torch.float32, 'expomf_half_epoch'
+    n, d, m = _exposure_shapes(name, X, Z, rowptr, row_order)
     if mu.dtype != f32:
-        raise QRecError('expomf_half_epoch: mu must be float32, got %s' % mu.dtype)
+        raise QRecError('%s: mu must be float32, got %s' % (name, mu.dtype))
     want = n if mu_by_row else m
     if mu.shape != (want,):
         raise QRecError('expomf_half_epoch: mu indexed by %s needs %d entries, got %s'
@@ -1444,12 +1450,16 @@ def expomf_half_epoch(X, Z, rowptr, cols, mu, mu_by_row, lam, lam_y, row_order, 
             raise QRecError('expomf_half_epoch: mu_out and mu need one float32 entry per row (%d)' % n)
         if mu_out.data_ptr() == mu.data_ptr():
             raise QRecError('expomf_half_epoch: mu_out must be a buffer of its own, not mu')
-    with _failures(n_failed, X.device, 'expomf_half_epoch: %d ' + _ROWS_FAILED) as n_failed:
-        check(lib.qrec_expomf_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
-                                             _dev(row_order, torch.int32, 'row_order'),
-                                             _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'),
-                                             _dev(mu, f32, 'mu'), int(bool(mu_by_row)), _opt(mu_out, f32, 'mu_out'),
-                                             float(lam), float(lam_y), float(a), float(b), int(max_ctas),
+    ptr = _ptrs(name, [(X, f32, 'X'), (Z, f32, 'Z'), (row_order, torch.int32, 'row_order'),
+                       (rowptr, torch.int64, 'rowptr'), (cols, torch.int32, 'cols'), (mu, f32, 'mu'),
+                       (mu_out, f32, 'mu_out')])
+    _ids(name, 'a row of row_order', row_order, n)
+    _rowptr(name, 'rowptr', rowptr, cols.shape[0])
+    _ids(name, 'a column', cols, m)
+    with _failures(n_failed, X.device, name + ': %d ' + _ROWS_FAILED) as n_failed:
+        check(lib.qrec_expomf_solve_rows_f32(ptr['X'], ptr['Z'], d, m, row_order.shape[0], ptr['row_order'],
+                                             ptr['rowptr'], ptr['cols'], ptr['mu'], int(bool(mu_by_row)),
+                                             ptr['mu_out'], float(lam), float(lam_y), float(a), float(b), int(max_ctas),
                                              _dev(n_failed, torch.int32, 'n_failed'), _stream()),
               'qrec_expomf_solve_rows_f32')
     return X
@@ -1471,8 +1481,8 @@ def serec_half_epoch(X, Z, rowptr, cols, asum, deg, row_is_user, lam, lam_y, row
     result does not depend on it).  n_failed: optional int32 CUDA tensor counting rows whose system was not positive
     definite (left unchanged); when it is not given, the count is read back here and a failed row raises QRecError."""
     torch = _torch()
-    f32, f64, i32 = torch.float32, torch.float64, torch.int32
-    n, d, m = _exposure_checks('serec_half_epoch', X, Z, rowptr, cols, row_order)
+    f32, f64, i32, name = torch.float32, torch.float64, torch.int32, 'serec_half_epoch'
+    n, d, m = _exposure_shapes(name, X, Z, rowptr, row_order)
     n_users, n_items = (n, m) if row_is_user else (m, n)
     if asum is not None and (asum.dtype != f64 or asum.shape != (n_items,)):
         raise QRecError('serec_half_epoch: asum needs one float64 entry per item (%d), got %s %s'
@@ -1480,20 +1490,22 @@ def serec_half_epoch(X, Z, rowptr, cols, asum, deg, row_is_user, lam, lam_y, row
     if deg.dtype != i32 or deg.shape != (n_users,):
         raise QRecError('serec_half_epoch: deg needs one int32 entry per user (%d), got %s %s'
                         % (n_users, deg.dtype, tuple(deg.shape)))
-    if n_users and int(deg.min()) < 0:
-        raise QRecError('serec_half_epoch: deg must not be negative')
     if asum_out is not None:
         if asum_out.dtype != f64 or asum_out.shape != (n,) or n != n_items:
             raise QRecError('serec_half_epoch: asum_out needs one float64 entry per row (%d), and the rows must be '
                             'the items' % n)
         if asum is not None and asum_out.data_ptr() == asum.data_ptr():
             raise QRecError('serec_half_epoch: asum_out must be a buffer of its own, not asum')
-    with _failures(n_failed, X.device, 'serec_half_epoch: %d ' + _ROWS_FAILED) as n_failed:
-        check(lib.qrec_serec_solve_rows_f32(_dev(X, f32, 'X'), _dev(Z, f32, 'Z'), d, m, row_order.shape[0],
-                                            _dev(row_order, i32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
-                                            _dev(cols, i32, 'cols'), _opt(asum, f64, 'asum'), float(mu0),
-                                            _dev(deg, i32, 'deg'), int(bool(row_is_user)),
-                                            _opt(asum_out, f64, 'asum_out'), float(lam), float(lam_y), float(a),
+    ptr = _ptrs(name, [(X, f32, 'X'), (Z, f32, 'Z'), (row_order, i32, 'row_order'), (rowptr, torch.int64, 'rowptr'),
+                       (cols, i32, 'cols'), (asum, f64, 'asum'), (deg, i32, 'deg'), (asum_out, f64, 'asum_out')])
+    _ids(name, 'a row of row_order', row_order, n)
+    _rowptr(name, 'rowptr', rowptr, cols.shape[0])
+    _ids(name, 'a column', cols, m)
+    _bounded(name, 'deg must not be negative', deg, lo=0)
+    with _failures(n_failed, X.device, name + ': %d ' + _ROWS_FAILED) as n_failed:
+        check(lib.qrec_serec_solve_rows_f32(ptr['X'], ptr['Z'], d, m, row_order.shape[0], ptr['row_order'],
+                                            ptr['rowptr'], ptr['cols'], ptr['asum'], float(mu0), ptr['deg'],
+                                            int(bool(row_is_user)), ptr['asum_out'], float(lam), float(lam_y), float(a),
                                             float(b), float(s), n_users, int(max_ctas), _dev(n_failed, i32, 'n_failed'),
                                             _stream()),
               'qrec_serec_solve_rows_f32')
@@ -1503,13 +1515,14 @@ def serec_half_epoch(X, Z, rowptr, cols, asum, deg, row_is_user, lam, lam_y, row
 # =============================================================================================
 # K11: SVD++ -- in-order parity epoch and user-major closed-form fast epoch
 # =============================================================================================
-def _svdpp_tables(P, Q, Y, Bu, Bi, dt):
-    d = P.shape[1]
-    if P.dim() != 2 or Q.dim() != 2 or Y.dim() != 2 or Q.shape[1] != d or Y.shape[1] != d:
+def _svdpp_shapes(P, Q, Y, Bu, Bi):
+    """Width d of the SVD++ tables: P, Q and Y are 2-D tables of one width, Y and Bi hold one row per item of Q, Bu one
+    per user of P.  The dtypes are _dev's to check; the library checks d."""
+    if any(t.dim() != 2 for t in (P, Q, Y)) or Q.shape[1] != P.shape[1] or Y.shape[1] != P.shape[1]:
         raise QRecError('svdpp: P, Q, Y must be 2-D tables of one width')
     if Y.shape[0] != Q.shape[0] or Bu.shape[0] != P.shape[0] or Bi.shape[0] != Q.shape[0]:
         raise QRecError('svdpp: Y / Bi need one row per item of Q, Bu one per user of P')
-    return [_dev(t, dt, name) for t, name in ((P, 'P'), (Q, 'Q'), (Y, 'Y'), (Bu, 'Bu'), (Bi, 'Bi'))], d
+    return P.shape[1]
 
 
 def svdpp_sgd_ordered(P, Q, Y, Bu, Bi, u, i, r, rowptr, cols, lr, reg_u, reg_i, reg_b, reg_y, global_mean, loss):
@@ -1517,16 +1530,16 @@ def svdpp_sgd_ordered(P, Q, Y, Bu, Bi, u, i, r, rowptr, cols, lr, reg_u, reg_i, 
     rowptr (int64 [num_users + 1]) / cols (int32): every user's distinct items in insertion order
     (Rating.rating_csr('user')).  Tables float64 or float32 (all five alike, r likewise); loss: float64 [1], += sum e^2."""
     torch = _torch()
-    dt = P.dtype
-    if dt not in (torch.float32, torch.float64):
-        raise QRecError('P must be float32 or float64, got %s' % dt)
+    if P.dtype not in (torch.float32, torch.float64):
+        raise QRecError('P must be float32 or float64, got %s' % P.dtype)
     if not (u.shape[0] == i.shape[0] == r.shape[0]):
         raise QRecError('svdpp_sgd_ordered: u, i, r differ in length')
     if rowptr.shape[0] != P.shape[0] + 1:
         raise QRecError('svdpp_sgd_ordered: rowptr has %d entries for %d users' % (rowptr.shape[0], P.shape[0]))
-    (pP, pQ, pY, pBu, pBi), d = _svdpp_tables(P, Q, Y, Bu, Bi, dt)
-    fn = lib.qrec_svdpp_sgd_ordered_f64 if dt == torch.float64 else lib.qrec_svdpp_sgd_ordered_f32
-    check(fn(pP, pQ, pY, pBu, pBi, d, u.shape[0], _dev(u, torch.int32, 'u'), _dev(i, torch.int32, 'i'), _dev(r, dt, 'r'),
+    d = _svdpp_shapes(P, Q, Y, Bu, Bi)
+    fn, dt = _entry('qrec_svdpp_sgd_ordered', P.dtype)
+    check(fn(_dev(P, dt, 'P'), _dev(Q, dt, 'Q'), _dev(Y, dt, 'Y'), _dev(Bu, dt, 'Bu'), _dev(Bi, dt, 'Bi'), d, u.shape[0],
+             _dev(u, torch.int32, 'u'), _dev(i, torch.int32, 'i'), _dev(r, dt, 'r'),
              _dev(rowptr, torch.int64, 'rowptr'), _dev(cols, torch.int32, 'cols'), float(lr), float(reg_u), float(reg_i),
              float(reg_b), float(reg_y), float(global_mean), _dev(loss, torch.float64, 'loss'), _stream()),
           'qrec_svdpp_sgd_ordered')
@@ -1544,8 +1557,9 @@ def svdpp_epoch_usermajor(P, Q, Y, Bu, Bi, rowptr, cols, vals, row_order, lr, re
         raise QRecError('svdpp_epoch_usermajor: rowptr has %d entries for %d users' % (rowptr.shape[0], P.shape[0]))
     if cols.shape[0] != vals.shape[0]:
         raise QRecError('svdpp_epoch_usermajor: cols and vals differ in length')
-    (pP, pQ, pY, pBu, pBi), d = _svdpp_tables(P, Q, Y, Bu, Bi, f32)
-    check(lib.qrec_svdpp_epoch_usermajor_f32(pP, pQ, pY, pBu, pBi, d, row_order.shape[0],
+    d = _svdpp_shapes(P, Q, Y, Bu, Bi)
+    check(lib.qrec_svdpp_epoch_usermajor_f32(_dev(P, f32, 'P'), _dev(Q, f32, 'Q'), _dev(Y, f32, 'Y'), _dev(Bu, f32, 'Bu'),
+                                             _dev(Bi, f32, 'Bi'), d, row_order.shape[0],
                                              _dev(row_order, torch.int32, 'row_order'), _dev(rowptr, torch.int64, 'rowptr'),
                                              _dev(cols, torch.int32, 'cols'), _dev(vals, f32, 'vals'), float(lr),
                                              float(reg_u), float(reg_i), float(reg_b), float(reg_y), float(global_mean),
@@ -1580,22 +1594,24 @@ def knn_squares(rowptr, vals, means, metric):
     return np.array([x ** 2 for x in vals.tolist()], dtype=np.float64)
 
 
-def _knn_csr(name, rowptr, cols, n_cols):
-    """Host checks of a CSR: rowptr int64 rising from 0 to len(cols), columns int32 in [0, n_cols), distinct within
-    each row.  Returns the number of rows."""
+def _knn_rows(name, rowptr, cols):
+    """The shapes of a CSR the KNN wrappers read: rowptr a 1-D int64 tensor of n_rows + 1 entries, cols 1-D int32.
+    Returns n_rows."""
     torch = _torch()
     if rowptr.dtype != torch.int64 or rowptr.dim() != 1 or rowptr.shape[0] < 1:
         raise QRecError('%s: rowptr must be a 1-D int64 tensor of n_rows + 1 entries' % name)
-    if cols.dtype != torch.int32 or cols.dim() != 1:
-        raise QRecError('%s: cols must be a 1-D int32 tensor' % name)
-    n, nnz = rowptr.shape[0] - 1, cols.shape[0]
-    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
-        raise QRecError('%s: rowptr must rise from 0 to len(cols) = %d' % (name, nnz))
-    if nnz and (int(cols.min()) < 0 or int(cols.max()) >= n_cols):
-        raise QRecError('%s: a column is outside [0, %d)' % (name, n_cols))
+    _vector(name, 'cols', cols, torch.int32)
+    return rowptr.shape[0] - 1
+
+
+def _knn_row_contents(name, rowptr, cols, n_cols):
+    """The contents of a CSR the KNN wrappers read: rowptr rises from 0 to len(cols), every column lies in
+    [0, n_cols), and the rows and columns fit the int32 ids."""
+    _rowptr(name, 'rowptr', rowptr, cols.shape[0])
+    _ids(name, 'a column', cols, n_cols)
+    n = rowptr.shape[0] - 1
     if n + n_cols >= 2 ** 31:
         raise QRecError('%s: %d rows and %d columns exceed the int32 ids' % (name, n, n_cols))
-    return n
 
 
 def _knn_sorted(rowptr, cols, n_cols, *payload):
@@ -1611,21 +1627,22 @@ def _knn_sorted(rowptr, cols, n_cols, *payload):
     return (sc,) + tuple(p[order].contiguous() for p in payload) + (order,)
 
 
-def _knn_queries(name, queries, n_rows):
-    torch = _torch()
-    if queries.dtype != torch.int32 or queries.dim() != 1:
-        raise QRecError('%s: queries must be a 1-D int32 tensor' % name)
-    if queries.numel() and (int(queries.min()) < -1 or int(queries.max()) >= n_rows):
-        raise QRecError('%s: a query is outside [0, %d) and not -1 (cold)' % (name, n_rows))
+def _knn_ascending(name, rowptr, sorted_cols):
+    """The columns of every row of a sorted view (knn_sorted_view) rise strictly."""
+    if sorted_cols.numel() > 1:
+        torch = _torch()
+        row = torch.repeat_interleave(torch.arange(rowptr.shape[0] - 1, device=sorted_cols.device),
+                                      rowptr[1:] - rowptr[:-1])
+        if bool(((sorted_cols[1:] <= sorted_cols[:-1]) & (row[1:] == row[:-1])).any()):
+            raise QRecError('%s: sorted_cols must rise strictly within each row (knn_sorted_view)' % name)
+
+
+def _knn_queried_once(name, queries, n_rows):
+    """Every query names a row, or is -1 (cold), and no row is queried twice."""
+    _ids(name, 'a query', queries, n_rows, lo=-1)
     warm = queries[queries >= 0]
-    if warm.numel() != torch.unique(warm).numel():
+    if warm.numel() != _torch().unique(warm).numel():
         raise QRecError('%s: a row is queried twice' % name)
-
-
-def _f64_vec(name, t, n):
-    torch = _torch()
-    if t.dtype != torch.float64 or t.shape != (n,):
-        raise QRecError('%s must be float64 [%d], got %s %s' % (name, n, t.dtype, tuple(t.shape)))
 
 
 def knn_neighbours(rowptr, cols, vals, sq, means, n_cols, queries, metric, K, max_ctas=0):
@@ -1643,18 +1660,23 @@ def knn_neighbours(rowptr, cols, vals, sq, means, n_cols, queries, metric, K, ma
     list of a large set."""
     torch = _torch()
     i32, i64, f64 = torch.int32, torch.int64, torch.float64
+    name = 'knn_neighbours'
     if metric not in (0, 1, 2):
-        raise QRecError('knn_neighbours: metric must be 0 (pcc), 1 (cos) or 2 (euclidean), got %r' % (metric,))
+        raise QRecError('%s: metric must be 0 (pcc), 1 (cos) or 2 (euclidean), got %r' % (name, metric))
     if int(K) != K or K < 0:
-        raise QRecError('knn_neighbours: K must be an integer >= 0, got %r' % (K,))
-    n = _knn_csr('knn_neighbours', rowptr, cols, n_cols)
-    for t, name in ((vals, 'vals'), (sq, 'sq')):
-        _f64_vec('knn_neighbours: ' + name, t, cols.shape[0])
-    _f64_vec('knn_neighbours: means', means, n)
-    _knn_queries('knn_neighbours', queries, n)
+        raise QRecError('%s: K must be an integer >= 0, got %r' % (name, K))
+    n = _knn_rows(name, rowptr, cols)
+    _vector(name, 'vals', vals, f64, cols.shape[0])
+    _vector(name, 'sq', sq, f64, cols.shape[0])
+    _vector(name, 'means', means, f64, n)
+    _vector(name, 'queries', queries, i32)
     Q, K = queries.shape[0], int(K)
     if Q + n >= 2 ** 31:
-        raise QRecError('knn_neighbours: %d queries and %d rows exceed the int32 list positions' % (Q, n))
+        raise QRecError('%s: %d queries and %d rows exceed the int32 list positions' % (name, Q, n))
+    ptr = _ptrs(name, [(rowptr, i64, 'rowptr'), (cols, i32, 'cols'), (vals, f64, 'vals'), (sq, f64, 'sq'),
+                       (means, f64, 'means'), (queries, i32, 'queries')])
+    _knn_row_contents(name, rowptr, cols, n_cols)
+    _knn_queried_once(name, queries, n)
     dev = cols.device
     _knn_sorted(rowptr, cols, n_cols)
     # the entries by column: their rows and their indices
@@ -1668,11 +1690,10 @@ def knn_neighbours(rowptr, cols, vals, sq, means, n_cols, queries, metric, K, ma
     ids = torch.empty((Q, K), dtype=i32, device=dev)
     sims = torch.empty((Q, K), dtype=f64, device=dev)
     cnt = torch.empty(Q, dtype=i32, device=dev)
-    check(lib.qrec_knn_neighbours_f64(int(metric), _dev(rowptr, i64, 'rowptr'), _dev(cols, i32, 'cols'),
-                                      _dev(vals, f64, 'vals'), _dev(sq, f64, 'sq'), _dev(means, f64, 'means'), n,
-                                      int(n_cols), crowptr.data_ptr(), crows.data_ptr(), ent.data_ptr(),
-                                      _dev(queries, i32, 'queries'), pos_of_row.data_ptr(),
-                                      Q, K, ids.data_ptr(), sims.data_ptr(), cnt.data_ptr(), int(max_ctas), _stream()),
+    check(lib.qrec_knn_neighbours_f64(int(metric), ptr['rowptr'], ptr['cols'], ptr['vals'], ptr['sq'], ptr['means'], n,
+                                      int(n_cols), crowptr.data_ptr(), crows.data_ptr(), ent.data_ptr(), ptr['queries'],
+                                      pos_of_row.data_ptr(), Q, K, ids.data_ptr(), sims.data_ptr(), cnt.data_ptr(),
+                                      int(max_ctas), _stream()),
           'qrec_knn_neighbours_f64')
     return ids, sims, cnt
 
@@ -1680,9 +1701,11 @@ def knn_neighbours(rowptr, cols, vals, sq, means, n_cols, queries, metric, K, ma
 def knn_sorted_view(rowptr, cols, vals):
     """The view of the rows knn_predict searches: every row's columns ascending (int32), with their values (float64)
     in the same permutation.  Built once per model; a row that repeats a column raises QRecError."""
+    name = 'knn_sorted_view'
     n_cols = int(cols.max()) + 1 if cols.numel() else 1
-    _knn_csr('knn_sorted_view', rowptr, cols, n_cols)
-    _f64_vec('knn_sorted_view: vals', vals, cols.shape[0])
+    _knn_rows(name, rowptr, cols)
+    _knn_row_contents(name, rowptr, cols, n_cols)
+    _vector(name, 'vals', vals, _torch().float64, cols.shape[0])
     scols, svals, _ = _knn_sorted(rowptr, cols, n_cols, vals)
     return scols, svals
 
@@ -1697,40 +1720,34 @@ def knn_predict(rowptr, sorted_cols, sorted_vals, means, global_mean, queries, i
     status 0 normal, 1 the mean fallback, 2 the reference's ZeroDivisionError (sum != 0 over a zero denominator)."""
     torch = _torch()
     i32, i64, f64 = torch.int32, torch.int64, torch.float64
-    n = rowptr.shape[0] - 1
+    name = 'knn_predict'
     cols = sorted_cols
-    n_cols = int(cols.max()) + 1 if cols.numel() else 0
-    _knn_csr('knn_predict', rowptr, cols, n_cols)
-    _f64_vec('knn_predict: sorted_vals', sorted_vals, cols.shape[0])
-    _f64_vec('knn_predict: means', means, n)
-    if cols.numel() > 1:
-        row = torch.repeat_interleave(torch.arange(n, device=cols.device), rowptr[1:] - rowptr[:-1])
-        if bool(((cols[1:] <= cols[:-1]) & (row[1:] == row[:-1])).any()):
-            raise QRecError('knn_predict: sorted_cols must rise strictly within each row (knn_sorted_view)')
-    _knn_queries('knn_predict', queries, n)
+    n = _knn_rows(name, rowptr, cols)
+    _vector(name, 'sorted_vals', sorted_vals, f64, cols.shape[0])
+    _vector(name, 'means', means, f64, n)
+    _vector(name, 'queries', queries, i32)
     Q = queries.shape[0]
     if ids.dim() != 2 or ids.shape[0] != Q or sims.shape != ids.shape or counts.shape != (Q,):
-        raise QRecError('knn_predict: ids / sims must be [%d, K] and counts [%d]' % (Q, Q))
-    K = ids.shape[1]
-    if Q and (int(counts.min()) < 0 or int(counts.max()) > K):
-        raise QRecError('knn_predict: a count is outside [0, %d]' % K)
-    if K and Q and int(ids.max()) >= n:
-        raise QRecError('knn_predict: a neighbour id is outside [0, %d)' % n)
-    L = line_qpos.shape[0]
+        raise QRecError('%s: ids / sims must be [%d, K] and counts [%d]' % (name, Q, Q))
+    K, L = ids.shape[1], line_qpos.shape[0]
     if line_qpos.dtype != i32 or line_probe.dtype != i32 or line_probe.shape != (L,):
-        raise QRecError('knn_predict: line_qpos and line_probe must be int32 of one length')
-    if L and (int(line_qpos.min()) < 0 or int(line_qpos.max()) >= Q):
-        raise QRecError('knn_predict: a line query position is outside [0, %d)' % Q)
-    if L and int(line_probe.min()) < -1:
-        raise QRecError('knn_predict: a probe id is below -1')
+        raise QRecError('%s: line_qpos and line_probe must be int32 of one length' % name)
+    ptr = _ptrs(name, [(rowptr, i64, 'rowptr'), (cols, i32, 'sorted_cols'), (sorted_vals, f64, 'sorted_vals'),
+                       (means, f64, 'means'), (queries, i32, 'queries'), (ids, i32, 'ids'), (sims, f64, 'sims'),
+                       (counts, i32, 'counts'), (line_qpos, i32, 'line_qpos'), (line_probe, i32, 'line_probe')])
+    _knn_row_contents(name, rowptr, cols, int(cols.max()) + 1 if cols.numel() else 0)
+    _knn_ascending(name, rowptr, cols)
+    _knn_queried_once(name, queries, n)
+    _bounded(name, 'a count is outside [0, %d]' % K, counts, 0, K + 1)
+    _ids(name, 'a neighbour id', ids, n, lo=None)
+    _ids(name, 'a line query position', line_qpos, Q)
+    _bounded(name, 'a probe id is below -1', line_probe, lo=-1)
     pred = torch.empty(L, dtype=f64, device=cols.device)
     status = torch.empty(L, dtype=i32, device=cols.device)
-    check(lib.qrec_knn_predict_f64(_dev(rowptr, i64, 'rowptr'), _dev(cols, i32, 'sorted_cols'),
-                                   _dev(sorted_vals, f64, 'sorted_vals'),
-                                   _dev(means, f64, 'means'), float(global_mean), _dev(queries, i32, 'queries'), K,
-                                   _dev(ids, i32, 'ids'), _dev(sims, f64, 'sims'), _dev(counts, i32, 'counts'), L,
-                                   _dev(line_qpos, i32, 'line_qpos'), _dev(line_probe, i32, 'line_probe'),
-                                   int(bool(minus_one_unrated)), pred.data_ptr(), status.data_ptr(), _stream()),
+    check(lib.qrec_knn_predict_f64(ptr['rowptr'], ptr['sorted_cols'], ptr['sorted_vals'], ptr['means'],
+                                   float(global_mean), ptr['queries'], K, ptr['ids'], ptr['sims'], ptr['counts'], L,
+                                   ptr['line_qpos'], ptr['line_probe'], int(bool(minus_one_unrated)), pred.data_ptr(),
+                                   status.data_ptr(), _stream()),
           'qrec_knn_predict_f64')
     return pred, status
 
@@ -1744,31 +1761,26 @@ def knn_pair_similarity(rowptr, cols, vals, sq, means, sorted_cols, sorted_vals,
     torch = _torch()
     i32, i64, f64 = torch.int32, torch.int64, torch.float64
     name = 'knn_pair_similarity'
-    if rowptr.dtype != i64 or rowptr.dim() != 1 or rowptr.shape[0] < 1:
-        raise QRecError('%s: rowptr must be a 1-D int64 tensor of n_rows + 1 entries' % name)
     if cols.dtype != i32 or cols.dim() != 1 or sorted_cols.dtype != i32 or sorted_cols.shape != cols.shape:
         raise QRecError('%s: cols and sorted_cols must be 1-D int32 tensors of one length' % name)
-    n, nnz = rowptr.shape[0] - 1, cols.shape[0]
-    for t, tname in ((vals, 'vals'), (sq, 'sq'), (sorted_vals, 'sorted_vals'), (sorted_sq, 'sorted_sq')):
-        _f64_vec('%s: %s' % (name, tname), t, nnz)
-    _f64_vec(name + ': means', means, n)
+    n, nnz = _knn_rows(name, rowptr, cols), cols.shape[0]
+    for t, label in ((vals, 'vals'), (sq, 'sq'), (sorted_vals, 'sorted_vals'), (sorted_sq, 'sorted_sq')):
+        _vector(name, label, t, f64, nnz)
+    _vector(name, 'means', means, f64, n)
     if a.dtype != i32 or b.dtype != i32 or a.dim() != 1 or b.shape != a.shape:
         raise QRecError('%s: a and b must be int32 of one length' % name)
-    _f64_vec(name + ': w', w, a.shape[0])
-    tensors = ((rowptr, i64, 'rowptr'), (cols, i32, 'cols'), (vals, f64, 'vals'), (sq, f64, 'sq'),
-               (means, f64, 'means'), (sorted_cols, i32, 'sorted_cols'), (sorted_vals, f64, 'sorted_vals'),
-               (sorted_sq, f64, 'sorted_sq'), (a, i32, 'a'), (b, i32, 'b'), (w, f64, 'w'))
-    ptr = [_dev(t, dt, '%s: %s' % (name, tname)) for t, dt, tname in tensors]
-    if int(rowptr[0]) != 0 or int(rowptr[-1]) != nnz or (n and bool((rowptr[1:] < rowptr[:-1]).any())):
-        raise QRecError('%s: rowptr must rise from 0 to len(cols) = %d' % (name, nnz))
-    if nnz > 1:   # the bisection needs every row of the sorted view ascending
-        row = torch.repeat_interleave(torch.arange(n, device=cols.device), rowptr[1:] - rowptr[:-1])
-        if bool(((sorted_cols[1:] <= sorted_cols[:-1]) & (row[1:] == row[:-1])).any()):
-            raise QRecError('%s: sorted_cols must rise strictly within each row (knn_sorted_view)' % name)
-    _ids_below(a, n, name + ': a row id is outside [0, %d)')
-    _ids_below(b, n, name + ': a row id is outside [0, %d)')
+    _vector(name, 'w', w, f64, a.shape[0])
+    ptr = _ptrs(name, [(rowptr, i64, 'rowptr'), (cols, i32, 'cols'), (vals, f64, 'vals'), (sq, f64, 'sq'),
+                       (means, f64, 'means'), (sorted_cols, i32, 'sorted_cols'), (sorted_vals, f64, 'sorted_vals'),
+                       (sorted_sq, f64, 'sorted_sq'), (a, i32, 'a'), (b, i32, 'b'), (w, f64, 'w')])
+    _rowptr(name, 'rowptr', rowptr, nnz)
+    _knn_ascending(name, rowptr, sorted_cols)       # the bisection needs every row of the sorted view ascending
+    _ids(name, 'a row id', a, n)
+    _ids(name, 'a row id', b, n)
     out = torch.empty(a.shape[0], dtype=f64, device=cols.device)
-    check(lib.qrec_knn_pair_similarity_f64(*ptr[:8], a.shape[0], *ptr[8:], out.data_ptr(), _stream()),
+    check(lib.qrec_knn_pair_similarity_f64(ptr['rowptr'], ptr['cols'], ptr['vals'], ptr['sq'], ptr['means'],
+                                           ptr['sorted_cols'], ptr['sorted_vals'], ptr['sorted_sq'], a.shape[0], ptr['a'],
+                                           ptr['b'], ptr['w'], out.data_ptr(), _stream()),
           'qrec_knn_pair_similarity_f64')
     return out
 
@@ -1782,24 +1794,29 @@ def slopeone_predict(item_rowptr, item_users, item_vals, item_means, user_rowptr
     the mean fallbacks.  max_ctas > 0 caps the grid (the result does not depend on it)."""
     torch = _torch()
     i32, i64, f64 = torch.int32, torch.int64, torch.float64
-    n_items, n_users = item_rowptr.shape[0] - 1, user_rowptr.shape[0] - 1
-    _knn_csr('slopeone_predict: item rows', item_rowptr, item_users, n_users)
-    _knn_csr('slopeone_predict: user rows', user_rowptr, user_items, n_items)
+    name = 'slopeone_predict'
+    n_items = _knn_rows(name + ': item rows', item_rowptr, item_users)
+    n_users = _knn_rows(name + ': user rows', user_rowptr, user_items)
     if item_users.shape[0] != user_items.shape[0]:
-        raise QRecError('slopeone_predict: the item and user rows hold different numbers of ratings')
-    _f64_vec('slopeone_predict: item_vals', item_vals, item_users.shape[0])
-    _f64_vec('slopeone_predict: user_vals', user_vals, user_items.shape[0])
-    _f64_vec('slopeone_predict: item_means', item_means, n_items)
-    _f64_vec('slopeone_predict: user_means', user_means, n_users)
-    _knn_queries('slopeone_predict', test_items, n_items)
-    _knn_sorted(item_rowptr, item_users, max(n_users, 1))
+        raise QRecError('%s: the item and user rows hold different numbers of ratings' % name)
+    _vector(name, 'item_vals', item_vals, f64, item_users.shape[0])
+    _vector(name, 'user_vals', user_vals, f64, user_items.shape[0])
+    _vector(name, 'item_means', item_means, f64, n_items)
+    _vector(name, 'user_means', user_means, f64, n_users)
+    _vector(name, 'queries', test_items, i32)
     Q, L = test_items.shape[0], line_qpos.shape[0]
     if line_qpos.dtype != i32 or line_user.dtype != i32 or line_user.shape != (L,):
-        raise QRecError('slopeone_predict: line_qpos and line_user must be int32 of one length')
-    if L and (int(line_qpos.min()) < 0 or int(line_qpos.max()) >= Q):
-        raise QRecError('slopeone_predict: a line position is outside [0, %d)' % Q)
-    if L and (int(line_user.min()) < -1 or int(line_user.max()) >= n_users):
-        raise QRecError('slopeone_predict: a user is outside [0, %d) and not -1 (cold)' % n_users)
+        raise QRecError('%s: line_qpos and line_user must be int32 of one length' % name)
+    ptr = _ptrs(name, [(item_rowptr, i64, 'item_rowptr'), (item_users, i32, 'item_users'), (item_vals, f64, 'item_vals'),
+                       (item_means, f64, 'item_means'), (user_rowptr, i64, 'user_rowptr'), (user_items, i32, 'user_items'),
+                       (user_vals, f64, 'user_vals'), (user_means, f64, 'user_means'), (test_items, i32, 'test_items'),
+                       (line_qpos, i32, 'line_qpos'), (line_user, i32, 'line_user')])
+    _knn_row_contents(name + ': item rows', item_rowptr, item_users, n_users)
+    _knn_row_contents(name + ': user rows', user_rowptr, user_items, n_items)
+    _knn_queried_once(name, test_items, n_items)
+    _knn_sorted(item_rowptr, item_users, max(n_users, 1))
+    _ids(name, 'a line position', line_qpos, Q)
+    _ids(name, 'a user', line_user, n_users, lo=-1)
     dev = item_users.device
     line_out = torch.argsort(line_qpos.to(i64), stable=True)
     line_rowptr = torch.zeros(Q + 1, dtype=i64, device=dev)
@@ -1807,12 +1824,10 @@ def slopeone_predict(item_rowptr, item_users, item_vals, item_means, user_rowptr
     by_item_user = line_user[line_out].contiguous()
     pred = torch.empty(L, dtype=f64, device=dev)
     status = torch.empty(L, dtype=i32, device=dev)
-    check(lib.qrec_slopeone_predict_f64(_dev(item_rowptr, i64, 'item_rowptr'), _dev(item_users, i32, 'item_users'),
-                                        _dev(item_vals, f64, 'item_vals'), _dev(item_means, f64, 'item_means'),
-                                        _dev(user_rowptr, i64, 'user_rowptr'), _dev(user_items, i32, 'user_items'),
-                                        _dev(user_vals, f64, 'user_vals'), _dev(user_means, f64, 'user_means'),
-                                        float(global_mean), n_items, _dev(test_items, i32, 'test_items'), Q,
-                                        line_rowptr.data_ptr(), by_item_user.data_ptr(), line_out.data_ptr(),
-                                        pred.data_ptr(), status.data_ptr(), int(max_ctas), _stream()),
+    check(lib.qrec_slopeone_predict_f64(ptr['item_rowptr'], ptr['item_users'], ptr['item_vals'], ptr['item_means'],
+                                        ptr['user_rowptr'], ptr['user_items'], ptr['user_vals'], ptr['user_means'],
+                                        float(global_mean), n_items, ptr['test_items'], Q, line_rowptr.data_ptr(),
+                                        by_item_user.data_ptr(), line_out.data_ptr(), pred.data_ptr(), status.data_ptr(),
+                                        int(max_ctas), _stream()),
           'qrec_slopeone_predict_f64')
     return pred, status
