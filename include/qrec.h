@@ -609,7 +609,13 @@ int64_t qrec_mf_order_depth(int64_t n, const int32_t* u, const int32_t* i, int32
  * Its wait arrays are qrec_mf_order_prepare(n, u, v, num_users, num_users, ...); it takes no bias vectors.
  * kind 4 is SocialMF's rating pass (model/rating/SocialMF.py:15-24): kind 1 on copies of both rows,
  *   P[u] += lr*(e*Q[i] - regU*P[u]);  Q[i] += lr*(e*P[u](old) - regI*Q[i]);  loss += e^2.
- * It takes no bias vectors either.  qrec_mf_sgd_batch_f32 takes kinds 0..2 only. */
+ * It takes no bias vectors either.
+ * kind 5 is EE's rating pass (model/rating/EE.py:15-36, 81-87), a Euclidean embedding with biases:
+ *   dist = |P[u]-Q[i]|^2;  e = r - (((global_mean + Bi[i]) + Bu[u]) - dist);
+ *   P[u] -= (lr*(e+regU))*(P[u]-Q[i]);  Q[i] += (lr*(e+regI))*(P[u](new)-Q[i]);
+ *   Bu[u] += lr*(e - regB*Bu[u]);  Bi[i] += lr*(e - regB*Bi[i]) (both from the biases before the step);
+ *   loss += e^2 + regU*dist.  It needs the bias vectors.
+ * qrec_mf_sgd_batch_f32 takes kinds 0..2 only. */
 int qrec_mf_sgd_ordered_f64(int32_t kind, double* dev_P, double* dev_Q, int32_t d, int64_t n,
                             const int32_t* dev_u, const int32_t* dev_i, const double* dev_r,
                             const int32_t* dev_wait_u, const int32_t* dev_wait_i, int32_t* dev_ver_p,
@@ -690,7 +696,7 @@ int qrec_rste_predict_pairs_f32(const float* dev_P, const float* dev_Q, int32_t 
 
 /* =====================================================================================
  * K17 -- the trust-neighbourhood user pass of SocialMF (kind 0, model/rating/SocialMF.py:26-43) and SoReg (kind 1,
- * model/rating/SoReg.py:54-72).  The users visit[0..n) in order (the reference's social.user restricted to training
+ * model/rating/SoReg.py:54-72), and SREE's (qrec_sree_user_pass_*, below).  The users visit[0..n) in order (the reference's social.user restricted to training
  * users, each at most once), each updating its own row of P from its followees f (f_rowptr[num_users+1] / f_cols /
  * f_val, in the cleaned followee dict's order) and, for SoReg, its followers g (g_rowptr / g_cols / g_val, in the
  * cleaned follower dict's order); a self-follow reads the row before the update:
@@ -720,6 +726,21 @@ int qrec_social_user_pass_f32(int32_t kind, float* dev_P, int32_t d, int64_t n, 
                               const float* dev_f_val, const int64_t* dev_g_rowptr, const int32_t* dev_g_cols,
                               const float* dev_g_val, int32_t* dev_done, unsigned long long* dev_ticket, float lr,
                               float coef, double* dev_loss, int32_t n_warps, void* stream);
+/* SREE's user pass (model/rating/SREE.py:48-61) over the same visiting order, schedule and waits as kind 0: each
+ * followee f of u in turn, with weight w_f (f_w), moves the row as the followees before it left it,
+ *   P[u] -= ((lr*alpha)*w_f)*(P[u]-P[f]);  loss += (alpha*w_f)*|P[u]-P[f]|^2 (after the step);
+ * a self-follow moves nothing.  The follower CSR (g_rowptr / g_cols) only orders the waits.  done[num_users] and
+ * ticket[1] must be zero on entry.  The result does not depend on n_warps (0 = fill the GPU). */
+int qrec_sree_user_pass_f64(double* dev_P, int32_t d, int64_t n, const int32_t* dev_visit, const int32_t* dev_pos,
+                            const int64_t* dev_f_rowptr, const int32_t* dev_f_cols, const double* dev_f_w,
+                            const int64_t* dev_g_rowptr, const int32_t* dev_g_cols, int32_t* dev_done,
+                            unsigned long long* dev_ticket, double lr, double alpha, double* dev_loss, int32_t n_warps,
+                            void* stream);
+int qrec_sree_user_pass_f32(float* dev_P, int32_t d, int64_t n, const int32_t* dev_visit, const int32_t* dev_pos,
+                            const int64_t* dev_f_rowptr, const int32_t* dev_f_cols, const float* dev_f_w,
+                            const int64_t* dev_g_rowptr, const int32_t* dev_g_cols, int32_t* dev_done,
+                            unsigned long long* dev_ticket, float lr, float alpha, double* dev_loss, int32_t n_warps,
+                            void* stream);
 
 /* =====================================================================================
  * K10 -- WRMF (implicit-feedback ALS, model/ranking/WRMF.py:19-61).  A half-epoch solves every row of one

@@ -94,6 +94,10 @@ SIGNATURES = {
                                   [C.c_double] * 2 + [vp, C.c_int32, vp]),
     'qrec_social_user_pass_f32': (C.c_int, [C.c_int32, vp, C.c_int32, C.c_int64] + [vp] * 10 +
                                   [C.c_float] * 2 + [vp, C.c_int32, vp]),
+    'qrec_sree_user_pass_f64': (C.c_int, [vp, C.c_int32, C.c_int64] + [vp] * 9 + [C.c_double] * 2 +
+                                [vp, C.c_int32, vp]),
+    'qrec_sree_user_pass_f32': (C.c_int, [vp, C.c_int32, C.c_int64] + [vp] * 9 + [C.c_float] * 2 +
+                                [vp, C.c_int32, vp]),
     'qrec_als_gram_workspace_bytes': (C.c_int64, [C.c_int64, C.c_int32]),
     'qrec_als_gram_f32': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),
     'qrec_als_gram_f64': (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, C.c_int64, vp]),

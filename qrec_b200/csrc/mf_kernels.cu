@@ -3,7 +3,8 @@
 //   reference: model/rating/BasicMF.py:13-23 (kind 0), model/rating/PMF.py:13-22 (kind 1),
 //              model/rating/SVD.py:17-32 + predictForRating SVD.py:84-90 (kind 2),
 //              model/rating/SoRec.py:42-60 (kind 3: the trust-edge pass, on the tables (P, Z)),
-//              model/rating/SocialMF.py:15-24 (kind 4: kind 1 on copies of the rows)
+//              model/rating/SocialMF.py:15-24 (kind 4: kind 1 on copies of the rows),
+//              model/rating/EE.py:15-36 + predictForRating EE.py:81-87 (kind 5: Euclidean embedding)
 //
 //   e = r - P[u].Q[i]                (SVD: - globalMean - Bi[i] - Bu[u], added in that order)
 //   kind 0:  P[u] += (lr*e)*Q[i];                  Q[i] += (lr*e)*P[u](new)
@@ -13,7 +14,10 @@
 //            (regS / regZ in the reg_u / reg_i slots, no bias vectors; the parity kernel only)
 //   kind 4:  P[u] += lr*(e*Q[i] - regU*P[u]);      Q[i] += lr*(e*P[u](old) - regI*Q[i](old))
 //            (no bias vectors; the parity kernel only)
-//   loss += e^2  (kind 3: regS*e^2)
+//   kind 5:  dist = |P[u]-Q[i]|^2,  e = r - (((globalMean + Bi[i]) + Bu[u]) - dist)
+//            P[u] -= (lr*(e+regU))*(P[u]-Q[i]);     Q[i] += (lr*(e+regI))*(P[u](new)-Q[i])
+//            Bu / Bi as kind 2 (from the biases before the update; the parity kernel only)
+//   loss += e^2  (kind 3: regS*e^2; kind 5: e^2 + regU*dist)
 //
 // `p = self.P[u]` is a numpy view in the reference, so the item row is updated from the already
 // updated user row -- both kernels keep that.  SocialMF copies both rows first (kind 4).
@@ -66,14 +70,19 @@ mf_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
       if (c < d) {
         p[e] = __ldcg(pr + c);  // L2-coherent: the row was last written by another SM
         q[e] = __ldcg(qr + c);
-        dot += p[e] * q[e];
+        if (KIND == 5) {
+          const T df = p[e] - q[e];
+          dot += df * df;
+        } else {
+          dot += p[e] * q[e];
+        }
       } else {
         p[e] = q[e] = 0;
       }
     }
     dot = warp_sum(dot);
     T bu = 0, bi = 0;
-    if (KIND == 2) {
+    if (KIND == 2 || KIND == 5) {
       bu = __ldcg(Bu + uu);
       bi = __ldcg(Bi + ii);
     }
@@ -89,13 +98,13 @@ mf_sgd_ordered_kernel(T* __restrict__ P, T* __restrict__ Q, int d, long long n,
         __stcg(qr + c, qn);
       }
     }
-    if (KIND == 2) {
+    if (KIND == 2 || KIND == 5) {
       if (lane == 0) __stcg(Bu + uu, qrec::mf_bias_parity<T>(bu, err, lr, reg_b));
       if (lane == 1) __stcg(Bi + ii, qrec::mf_bias_parity<T>(bi, err, lr, reg_b));
     }
     warp_fence();
     if (lane < 2) red_release_gpu_add(const_cast<int*>(vp), 1);
-    if (lane == 0) local_loss += qrec::mf_loss_term<T, KIND>(err, reg_u);
+    if (lane == 0) local_loss += qrec::mf_loss_term<T, KIND>(err, reg_u, dot);
   }
   if (lane == 0 && local_loss != 0.0) atomicAdd(loss, local_loss);
 }
@@ -210,11 +219,12 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
                    const int* wu, const int* wi, int* ver_p, int* ver_q, unsigned long long* ticket, T lr,
                    T reg_u, T reg_i, T* Bu, T* Bi, T reg_b, T global_mean, double* loss, int n_warps,
                    cudaStream_t st) {
-  QREC_REQUIRE(kind >= 0 && kind <= 4, "mf_sgd_ordered: kind=%d (0 BasicMF, 1 PMF, 2 SVD, 3 SoRec edges, 4 SocialMF)",
-               kind);
+  QREC_REQUIRE(kind >= 0 && kind <= 5,
+               "mf_sgd_ordered: kind=%d (0 BasicMF, 1 PMF, 2 SVD, 3 SoRec edges, 4 SocialMF, 5 EE)", kind);
   QREC_REQUIRE(P && Q && loss && ticket && ver_p && ver_q, "mf_sgd_ordered: null pointer");
   QREC_REQUIRE(kind != 2 || (Bu && Bi), "mf_sgd_ordered: kind 2 needs the bias vectors");
-  QREC_REQUIRE(kind < 3 || (!Bu && !Bi), "mf_sgd_ordered: kind %d takes no bias vectors", kind);
+  QREC_REQUIRE(kind != 5 || (Bu && Bi), "mf_sgd_ordered: kind 5 needs the bias vectors");
+  QREC_REQUIRE((kind != 3 && kind != 4) || (!Bu && !Bi), "mf_sgd_ordered: kind %d takes no bias vectors", kind);
   QREC_REQUIRE(d >= 1 && d <= 256, "mf_sgd_ordered: d=%d unsupported (1..256)", d);
   QREC_REQUIRE(n >= 0, "mf_sgd_ordered: n < 0");
   if (n == 0) return QREC_OK;
@@ -226,7 +236,8 @@ int launch_ordered(int kind, T* P, T* Q, int d, long long n, const int* u, const
                         : kind == 1 ? mf_sgd_ordered_kernel<T, E, 1>
                         : kind == 2 ? mf_sgd_ordered_kernel<T, E, 2>
                         : kind == 3 ? mf_sgd_ordered_kernel<T, E, 3>
-                                    : mf_sgd_ordered_kernel<T, E, 4>;
+                        : kind == 4 ? mf_sgd_ordered_kernel<T, E, 4>
+                                    : mf_sgd_ordered_kernel<T, E, 5>;
     kernel<<<grid, 256, 0, st>>>(P, Q, d, n, u, i, r, wu, wi, ver_p, ver_q, ticket, lr, reg_u, reg_i, Bu, Bi, reg_b,
                                  global_mean, loss);
   });

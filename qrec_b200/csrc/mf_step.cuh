@@ -9,6 +9,10 @@
 //                              P[u] += lr*(g*z) ;  Z[v] += lr*(g*P[u] - regZ*z) ;  loss += regS*e^2
 //   kind 4  SocialMF.py:15-24  kind 1 on copies of both rows: the item step reads the user row as it was before
 //                              P[u] += lr*(e*q - regU*p) ;  Q[i] += lr*(e*p - regI*q)
+//   kind 5  EE.py:15-36        Euclidean embedding with biases; `dot` is dist = |p-q|^2 and the
+//                              prediction ((globalMean + Bi[i]) + Bu[u]) - dist:
+//                              P[u] -= (lr*(e+regU))*(p-q) ;  Q[i] += (lr*(e+regI))*(P[u]-q) ;
+//                              loss += e^2 + regU*dist
 #pragma once
 
 namespace qrec {
@@ -22,6 +26,7 @@ __device__ __forceinline__ double mf_sub(double a, double b) { return __dsub_rn(
 
 template <typename T, int KIND>
 __device__ __forceinline__ T mf_prediction(T dot, T global_mean, T bi, T bu) {
+  if (KIND == 5) return mf_sub(mf_add(mf_add(global_mean, bi), bu), dot);
   return KIND == 2 ? mf_add(mf_add(mf_add(dot, global_mean), bi), bu) : dot;
 }
 
@@ -43,16 +48,20 @@ __device__ __forceinline__ void mf_update_parity(T p, T q, T err, T g, T lr, T r
   } else if (KIND == 4) {
     pn = mf_add(p, mf_mul(lr, mf_sub(mf_mul(err, q), mf_mul(reg_u, p))));
     qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(err, p), mf_mul(reg_i, q))));
+  } else if (KIND == 5) {
+    pn = mf_sub(p, mf_mul(mf_mul(lr, mf_add(err, reg_u)), mf_sub(p, q)));
+    qn = mf_add(q, mf_mul(mf_mul(lr, mf_add(err, reg_i)), mf_sub(pn, q)));
   } else {
     pn = mf_add(p, mf_mul(lr, mf_sub(mf_mul(err, q), mf_mul(reg_u, p))));
     qn = mf_add(q, mf_mul(lr, mf_sub(mf_mul(err, pn), mf_mul(reg_i, q))));
   }
 }
 
-// the entry's term of the epoch loss: e^2, regS*e^2 for a trust edge (kind 3)
+// the entry's term of the epoch loss: e^2, regS*e^2 for a trust edge (kind 3), e^2 + regU*dist for EE (kind 5)
 template <typename T, int KIND>
-__device__ __forceinline__ double mf_loss_term(T err, T reg_u) {
+__device__ __forceinline__ double mf_loss_term(T err, T reg_u, T dist = T(0)) {
   const double sq = (double)err * (double)err;
+  if (KIND == 5) return sq + (double)reg_u * (double)dist;
   return KIND == 3 ? (double)reg_u * sq : sq;
 }
 

@@ -11,6 +11,9 @@
 //     P[u] += lr*((-alpha)*(f1+f2))
 //     loss += simSum after every followee, simSum += Sim[u][f]*|P[u]-P[f]|^2 (the running sum, as the reference)
 //   P[u] on the right-hand sides is u's row before the update, also where u follows itself.
+//   SREE.py:48-61, one training user u, its cleaned followees f with weights w_f in dict order, one after another:
+//     P[u] -= ((lr*alpha)*w_f)*(P[u]-P[f]) ;  loss += (alpha*w_f)*|P[u]-P[f]|^2 with the updated P[u]
+//   Here P[u] is the row as moved by the followees before f; a self-follow reads that row and moves nothing.
 #pragma once
 
 #include "rste_step.cuh"
@@ -45,6 +48,12 @@ __device__ __forceinline__ T soreg_add(T f, T s, T p, T pv) {
 template <typename T>
 __device__ __forceinline__ T soreg_step(T p, T lr, T alpha, T f1, T f2) {
   return mf_add(p, mf_mul(lr, mf_mul(-alpha, mf_add(f1, f2))));
+}
+
+// SREE: one followee's step on one component, P[u] -= (lr_alpha*w)*(p - pf), lr_alpha = lr*alpha formed first
+template <typename T>
+__device__ __forceinline__ T sree_step(T p, T lr_alpha, T w, T pf) {
+  return mf_sub(p, mf_mul(mf_mul(lr_alpha, w), mf_sub(p, pf)));
 }
 
 }  // namespace qrec

@@ -992,6 +992,7 @@ def mask_rated(scores, users, rowptr, cols, value=0.0):
 MF_KINDS = {'BasicMF': 0, 'PMF': 1, 'SVD': 2}
 SOREC_EDGES = 3    # kind 3: SoRec's trust-edge pass on (P, Z), regS / regZ in the reg_u / reg_i slots
 SOCIALMF_RATINGS = 4    # kind 4: SocialMF's rating pass, kind 1 on copies of both rows
+EE_RATINGS = 5    # kind 5: EE's rating pass, a Euclidean embedding with biases (the parity kernel only)
 
 
 def mf_sgd_ordered(kind, P, Q, u, i, r, wu, wi, lr, reg_u, reg_i, loss, Bu=None, Bi=None, reg_b=0.0,
@@ -1011,6 +1012,8 @@ def mf_sgd_ordered(kind, P, Q, u, i, r, wu, wi, lr, reg_u, reg_i, loss, Bu=None,
         _ids(name, 'an edge target', i, Q.shape[0])
     if kind == SOCIALMF_RATINGS and (Bu is not None or Bi is not None):
         raise QRecError('%s: kind 4 (SocialMF ratings) takes no bias vectors' % name)
+    if kind == EE_RATINGS and (Bu is None or Bi is None):
+        raise QRecError('%s: kind 5 (EE ratings) needs the bias vectors' % name)
     fn, dt = _entry('qrec_mf_sgd_ordered', P.dtype)
     d = P.shape[1]
     assert Q.shape[1] == d and u.shape[0] == i.shape[0] == r.shape[0]
@@ -1149,7 +1152,7 @@ def _rste_followees(name, P, Q, f_rowptr, f_cols, f_w, denom):
 
 
 # ---------------------------------------------------------------------------------------------
-# K17: the trust-neighbourhood user pass of SocialMF and SoReg
+# K17: the trust-neighbourhood user pass of SocialMF and SoReg, and SREE's
 # ---------------------------------------------------------------------------------------------
 SOCIAL_PASS_KINDS = {'SocialMF': 0, 'SoReg': 1}
 
@@ -1180,12 +1183,39 @@ def social_user_pass(kind, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_c
     followees / followers, coef: alpha).  visit (int32): the visiting order; pos: social_order_prepare's; f_* / g_*:
     the followee / follower CSRs (rowptr int64, cols int32); g_val may be None for kind 0.  loss (float64) += the
     pass's loss terms."""
-    torch = _torch()
     name = 'social_user_pass'
     if kind not in (0, 1):
         raise QRecError('%s: kind must be 0 (SocialMF) or 1 (SoReg), got %r' % (name, kind))
     if kind == 1 and g_val is None:
         raise QRecError('%s: SoReg needs the followers\' similarities (g_val)' % name)
+    d, n, ptr = _social_pass_args(name, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_cols, g_val, loss)
+    done, ticket = _order_counters(P.device, P.shape[0])
+    fn, _ = _entry('qrec_social_user_pass', P.dtype)
+    check(fn(int(kind), ptr['P'], d, n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'],
+             ptr['f_val'], ptr['g_rowptr'], ptr['g_cols'], ptr['g_val'], done.data_ptr(), ticket.data_ptr(),
+             float(lr), float(coef), ptr['loss'], int(n_warps), _stream()), 'qrec_social_user_pass')
+    return loss
+
+
+def sree_user_pass(P, visit, pos, f_rowptr, f_cols, f_w, g_rowptr, g_cols, lr, alpha, loss, n_warps=0):
+    """SREE's user pass, sequential-equivalent, in place on P (float32 or float64): every followee f of each visited
+    user u in turn moves P[u] -= ((lr*alpha)*w_f)*(P[u]-P[f]), and loss (float64) += (alpha*w_f)*|P[u]-P[f]|^2 after
+    the step.  The arguments are social_user_pass's: f_w are the followee weights, and the follower CSR (no values)
+    only orders the waits."""
+    name = 'sree_user_pass'
+    d, n, ptr = _social_pass_args(name, P, visit, pos, f_rowptr, f_cols, f_w, g_rowptr, g_cols, None, loss)
+    done, ticket = _order_counters(P.device, P.shape[0])
+    fn, _ = _entry('qrec_sree_user_pass', P.dtype)
+    check(fn(ptr['P'], d, n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'], ptr['f_val'],
+             ptr['g_rowptr'], ptr['g_cols'], done.data_ptr(), ticket.data_ptr(), float(lr), float(alpha), ptr['loss'],
+             int(n_warps), _stream()), 'qrec_sree_user_pass')
+    return loss
+
+
+def _social_pass_args(name, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_cols, g_val, loss):
+    """The checks the K17 wrappers share, in their three steps.  Returns (d, the number of visits, the pointers by
+    label); the values go under the labels f_val and g_val, and g_val may be None."""
+    torch = _torch()
     d = _tables(name, ((P, 'P'),), 256)
     U = P.shape[0]
     if visit.dim() != 1 or visit.shape[0] > U:
@@ -1210,12 +1240,7 @@ def social_user_pass(kind, P, visit, pos, f_rowptr, f_cols, f_val, g_rowptr, g_c
     # every wait reads pos: it must name exactly the visit positions
     if int((pos >= 0).sum()) != n or (n and not bool((pos[visit.long()] == torch.arange(n, device=pos.device)).all())):
         raise QRecError('%s: pos does not match the visiting order' % name)
-    done, ticket = _order_counters(P.device, U)
-    fn, _ = _entry('qrec_social_user_pass', dt)
-    check(fn(int(kind), ptr['P'], d, n, ptr['visit'], ptr['pos'], ptr['f_rowptr'], ptr['f_cols'],
-             ptr['f_val'], ptr['g_rowptr'], ptr['g_cols'], ptr['g_val'], done.data_ptr(), ticket.data_ptr(),
-             float(lr), float(coef), ptr['loss'], int(n_warps), _stream()), 'qrec_social_user_pass')
-    return loss
+    return d, n, ptr
 
 
 # =============================================================================================

@@ -1,4 +1,4 @@
-"""Shared pieces of the social rating models SoRec, RSTE, SocialMF and SoReg on the H100 engine.
+"""Shared pieces of the social rating models SoRec, RSTE, SocialMF, SoReg and SREE on the H100 engine.
 
 Both train in the reference's order with the in-order kernels, in float64 (`engine=-precision f64`, the default) or
 float32 (`-precision f32`; `-mode fast` runs the same kernels in float32, as WRMF and CoFactor do).  There is no

@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""SoRec's trust-edge pass (K9 kind 3), RSTE's rating pass (K16), the user passes of SocialMF and SoReg (K17) and SoReg's
-pair similarities (qrec_knn_pair_similarity_f64), in float64 as the parity path runs them, on the two synthetic shapes of bench_serec.py (qrec_b200.synthetic, Zipf-skewed item popularity):
+"""SoRec's trust-edge pass (K9 kind 3), RSTE's rating pass (K16), EE's rating pass (K9 kind 5), the user passes of
+SocialMF, SoReg and SREE (K17) and SoReg's pair similarities (qrec_knn_pair_similarity_f64), in float64 as the parity path runs them, on the two synthetic shapes of bench_serec.py (qrec_b200.synthetic, Zipf-skewed item popularity):
   * lastfm-like: 1,892 users x 17,632 items, 40 entries per user, d = 20;
   * yelp2018-like: 31,668 users x 38,048 items, 36 entries per user, d = 64.
 Followee counts are bench_serec.py's draw (a fifth of the users follow nobody, the rest a log-normal count); the
 followees are drawn uniformly among the other users, weight 1.  The entry stream and the edge list are shuffled.
 
 Timed with CUDA events, one launch per pass: SoRec's edge pass, RSTE's rating pass, and K9 PMF (kind 1) on the same
-entry stream, so that the cost of the followee reads shows; SocialMF's and SoReg's user passes over a shuffled visiting
-order of all users (followers are the transpose of the followees; SoReg's similarities are drawn uniformly); and the
+entry stream, so that the cost of the followee reads shows; EE's rating pass beside K9 SVD (kind 2) on the same entry
+stream and bias vectors, so that the cost of the distance form shows; SocialMF's, SoReg's and SREE's user passes over a
+shuffled visiting order of all users (followers are the transpose of the followees; SoReg's similarities are drawn uniformly); and the
 Pearson similarity of every trust edge over the users' rated rows (half-step ratings), built once per model.  The host wait numbers are prepared beforehand.  The passes
 are launched through the C entry points: the engine wrappers' input checks read device values back (ids, CSR bounds),
 which would put host round trips inside the timed window of some passes and not others.  Each pass zeroes its row
@@ -104,6 +105,19 @@ def main():
                 ptr(pmf_cnt) + 4 * U, ptr(tickets) + 8, 1e-3, 1e-3, 1e-3, None, None, 0.0, 0.0, ptr(loss), pmf_n, st),
                 'qrec_mf_sgd_ordered_f64')
 
+        Bu = torch.rand(U, device=dev, dtype=f64, generator=g) / 10
+        Bi = torch.rand(I, device=dev, dtype=f64, generator=g) / 10
+        btickets = torch.zeros(2, dtype=torch.int64, device=dev)
+
+        def biased(kind, slot):                                         # K9 kind 2 (SVD) or kind 5 (EE)
+            def run():
+                pmf_cnt.zero_(); btickets[slot:slot + 1].zero_()
+                E.check(E.lib.qrec_mf_sgd_ordered_f64(
+                    kind, ptr(P), ptr(Q), D, n, ptr(du), ptr(di), ptr(r), ptr(mwu), ptr(mwi), ptr(pmf_cnt),
+                    ptr(pmf_cnt) + 4 * U, ptr(btickets) + 8 * slot, 1e-3, 1e-3, 1e-3, ptr(Bu), ptr(Bi), 1e-3, 3.0,
+                    ptr(loss), pmf_n, st), 'qrec_mf_sgd_ordered_f64')
+            return run
+
         def edges():
             edge_cnt.zero_(); tickets[2:3].zero_()
             E.check(E.lib.qrec_mf_sgd_ordered_f64(
@@ -123,7 +137,7 @@ def main():
         sim_g = torch.rand(cols.shape[0], device=dev, dtype=f64, generator=g)
         social_n = width(U, social_depth)
         done = torch.zeros(U, dtype=torch.int32, device=dev)
-        stickets = torch.zeros(2, dtype=torch.int64, device=dev)
+        stickets = torch.zeros(3, dtype=torch.int64, device=dev)
 
         def user_pass(kind):
             def run():
@@ -133,6 +147,13 @@ def main():
                     ptr(social[2]) if kind == 0 else ptr(sim_f), ptr(sdev[2]), ptr(sdev[3]), ptr(sim_g), ptr(done),
                     ptr(stickets) + 8 * kind, 1e-3, 0.1, ptr(loss), social_n, st), 'qrec_social_user_pass_f64')
             return run
+
+        def sree():
+            done.zero_(); stickets[2:3].zero_()
+            E.check(E.lib.qrec_sree_user_pass_f64(
+                ptr(P), D, U, ptr(sdev[0]), ptr(sdev[1]), ptr(social[0]), ptr(social[1]), ptr(social[2]), ptr(sdev[2]),
+                ptr(sdev[3]), ptr(done), ptr(stickets) + 16, 1e-3, 0.5, ptr(loss), social_n, st),
+                'qrec_sree_user_pass_f64')
 
         # SoReg's similarities: one per trust edge, over each user's distinct rated items
         up = np.unique(np.stack([u, i]), axis=1)
@@ -151,10 +172,12 @@ def main():
                     'qrec_knn_pair_similarity_f64')
 
         socialmf, soreg = user_pass(0), user_pass(1)
-        for fn in (rste, pmf, edges, socialmf, soreg, pair_sims):      # warm-up
+        svd, ee = biased(2, 0), biased(E.EE_RATINGS, 1)
+        for fn in (rste, pmf, edges, socialmf, soreg, pair_sims, svd, ee, sree):      # warm-up
             fn()
         t_rste, t_pmf, t_edges = timed(torch, rste, reps), timed(torch, pmf, reps), timed(torch, edges, reps)
         t_socialmf, t_soreg, t_sims = timed(torch, socialmf, reps), timed(torch, soreg, reps), timed(torch, pair_sims, reps)
+        t_svd, t_ee, t_sree = timed(torch, svd, reps), timed(torch, ee, reps), timed(torch, sree, reps)
         print(json.dumps(dict(
             shape=label, users=U, items=I, entries=n, d=D, dtype='float64', edges=int(eu.shape[0]),
             followee_reads=int(np.diff(rowptr)[u].sum()), deg_mean=round(float(np.diff(rowptr).mean()), 2),
@@ -164,7 +187,10 @@ def main():
             ms_soreg_pair_similarity=round(t_sims, 3),
             depth_sorec_edges=edge_depth, depth_rste=rste_depth, depth_pmf=pmf_depth, depth_social_users=social_depth,
             entries_per_s_sorec_edges=round(eu.shape[0] / (t_edges / 1e3)), entries_per_s_rste=round(n / (t_rste / 1e3)),
-            entries_per_s_pmf=round(n / (t_pmf / 1e3)), gpu=name, power_limit=limit)), flush=True)
+            entries_per_s_pmf=round(n / (t_pmf / 1e3)),
+            ms_svd_pass=round(t_svd, 3), ms_ee_pass=round(t_ee, 3), ms_sree_user_pass=round(t_sree, 3),
+            entries_per_s_svd=round(n / (t_svd / 1e3)), entries_per_s_ee=round(n / (t_ee / 1e3)),
+            gpu=name, power_limit=limit)), flush=True)
 
 
 if __name__ == '__main__':

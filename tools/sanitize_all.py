@@ -99,6 +99,8 @@ def main():
         for kind in (0, 1, 2):
             E.mf_sgd_batch(kind, P, Q, dev(u9), dev(i9), r9, 0.01, 0.01, 0.01, loss, Bu, Bi, 0.01, 2.0)
             E.mf_sgd_ordered(kind, P, Q, dev(u9), dev(i9), r9, dev(wu9), dev(wi9), 0.01, 0.01, 0.01, loss, Bu, Bi, 0.01, 2.0)
+        E.mf_sgd_ordered(E.EE_RATINGS, P, Q, dev(u9), dev(i9), r9, dev(wu9), dev(wi9), 0.01, 0.01, 0.01, loss, Bu, Bi,
+                         0.01, 2.0)
         E.mf_predict_pairs(P, Q, dev(u9), dev(i9), Bu, Bi, 2.0)
         Hv2 = torch.empty(B, 320, device='cuda')
         E.tc_gemm_v2(A0, W1, Hv2, epilogue=E.EPI_BIAS_RELU, bias=b1)
@@ -227,8 +229,8 @@ def main():
                                dev((np.arange(300) % nu).astype(np.int32)), max_ctas=c)
         torch.cuda.synchronize()
         print('sanitize_all: + K15, launched', E.launch_count(), 'kernels')
-        # K17 (SocialMF / SoReg user pass) on a ring-with-chords trust graph with self-follows, both kinds and dtypes,
-        # one CTA and a full grid; SoReg's pair similarities over the K15 user rows
+        # K17 (SocialMF / SoReg / SREE user pass) on a ring-with-chords trust graph with self-follows, every kind and
+        # both dtypes, one CTA and a full grid; SoReg's pair similarities over the K15 user rows
         fol = [sorted({(a + 1) % nu, (7 * a + 3) % nu, a}) for a in range(nu)]
         frp = np.concatenate([[0], np.cumsum([len(x) for x in fol])]).astype(np.int64)
         fcol = np.array([v for x in fol for v in x], np.int32)
@@ -244,6 +246,9 @@ def main():
                     E.social_user_pass(kind, torch.rand(nu, 33, device='cuda').to(dt), dev(visit), dev(spos), dev(frp),
                                        dev(fcol), vals, dev(grp), dev(gcol), vals[torch.from_numpy(back).cuda()], 0.05,
                                        0.1, torch.zeros(1, dtype=torch.float64, device='cuda'), n_warps=nw)
+                E.sree_user_pass(torch.rand(nu, 33, device='cuda').to(dt), dev(visit), dev(spos), dev(frp), dev(fcol),
+                                 vals, dev(grp), dev(gcol), 0.05, 0.5, torch.zeros(1, dtype=torch.float64, device='cuda'),
+                                 n_warps=nw)
         ksq = dev(E.knn_squares(rp_h, kv.cpu().numpy(), km.cpu().numpy(), 0))
         pa = dev(np.arange(0, nu, 3).astype(np.int32))
         E.knn_pair_similarity(krp, kcol, kv, ksq, km, *E.knn_sorted_view(krp, kcol, kv),
