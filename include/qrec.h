@@ -286,8 +286,11 @@ int qrec_table_gather_merge_p2p_f32(const float* const* peer_S, int32_t world, f
 /* K8 (SURVEY 8f-1): batched ranking evaluation, replaces the per-user loop of Recommender.evalRanking
  * (base/recommender.py:143-152) + find_k_largest (util/qmath.py:134-146).  For every row r of the block:
  * scores = V . U[user_ids[r]] (fp32), rated items of that user (sorted CSR) score `rated_value` (the reference
- * writes 0, it does not remove them), the N best (score descending, ties by ascending item id) go to
- * out_ids / out_scores [n_rows, N].  The score matrix is never materialised.  1 <= N <= 100. */
+ * writes 0, it does not remove them), the N best (score descending, ties by ascending item id, -0.0 and +0.0 one
+ * score written as +0.0) go to out_ids / out_scores [n_rows, N].  The score matrix is never materialised.
+ * 1 <= N <= 101: the reference ranks at most 100, and a caller may ask for one key past the cut to see a tie
+ * across it.  The tie order is not the reference heap's (find_k_largest keeps later ids at a tie across the cut
+ * and heap order inside a tie); qrec_b200/evaluate.py ranks the rows with equal scores again on the host. */
 int qrec_score_topn_f32(const float* dev_U, const float* dev_V, int32_t d, int32_t n_items,
                         const int32_t* dev_user_ids, int32_t n_rows, const int64_t* dev_rated_rowptr,
                         const int32_t* dev_rated_cols, float rated_value, int32_t N, int32_t* dev_out_ids,

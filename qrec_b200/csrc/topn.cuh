@@ -5,8 +5,9 @@
 
 namespace qrec {
 
-__device__ __forceinline__ uint32_t ord_of(float s) {          // monotone float -> uint
-  const uint32_t u = __float_as_uint(s);
+// monotone float -> uint; -0.0 and +0.0 are one score (the reference compares them equal), both map to +0.0's key
+__device__ __forceinline__ uint32_t ord_of(float s) {
+  const uint32_t u = __float_as_uint(s) == 0x80000000u ? 0u : __float_as_uint(s);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 __device__ __forceinline__ float score_of(uint32_t o) {

@@ -10,10 +10,10 @@
 // row's candidate list (256 keys, L2-resident scratch) and a warp-level bitonic sort compacts a row back to N
 // whenever its list could overflow.  Nothing of the [users x items] score matrix is written to memory.
 //
-// Ordering: (score descending, item id ascending) -- a total order, so the result does not depend on the
-// scan order.  It agrees with the reference heap on which items survive a tie at the cut (the heap keeps the
-// earlier item: strict `>`), and makes the order among equal scores deterministic (the heap's is an
-// implementation detail of heapq).
+// Ordering: (score descending, item id ascending), -0.0 and +0.0 one score -- a total order, so the result does
+// not depend on the scan order.  It is not the reference heap's: at a tie across the cut the heap can keep later
+// ids, and inside a tie it keeps heap order.  evaluate.batched_top_n asks for one key more than it needs and ranks
+// the rows with equal scores again on the host, so `-eval gpu` returns the heap's lists on the device's fp32 scores.
 #include "common.h"
 #include "topn.cuh"
 
@@ -22,7 +22,7 @@ namespace {
 using namespace qrec;
 
 constexpr int CAP = 256;   // candidate slots per user (>= N_max + items per tile)
-constexpr int NMAX = 100;  // base/recommender.py:131-134 clamps N to <= 100
+constexpr int NMAX = 101;  // base/recommender.py:131-134 clamps N to <= 100; evaluate.py asks for one key past the cut
 
 // ---------------------------------------------------------------------------------------------------------------
 // The kernel: 128 users x 128 items per tile, 8 x 8 register tile per thread, double-buffered k-chunks of 16

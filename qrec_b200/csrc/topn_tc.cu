@@ -41,7 +41,7 @@ constexpr int TRIG_EXTRA = 96;   // a list is cut back to its N best once it hol
 constexpr int SORTN = 256; // keys of the final per-row sort (two lists of at most N_max keys)
 constexpr int NT = 256;    // multiplying and selecting threads per CTA: two warpgroups (a 9th warp drives the bulk copies)
 constexpr int SIGW = 16;   // 32-bit words of a row's rated-set signature (512 bits) kept in shared memory
-constexpr int NMAX = 100;  // base/recommender.py:131-134 clamps N to <= 100
+constexpr int NMAX = 101;  // base/recommender.py:131-134 clamps N to <= 100; evaluate.py asks for one key past the cut
 constexpr int TM = 128, TN = 128;
 constexpr int KBLK = TM * 128;                       // bytes of one k-block (32 fp32 = 128 B per row) of a 128-row operand
 constexpr int SP = TN + 4;                           // row pitch (floats) of a warpgroup's score tile: conflict-free row reads

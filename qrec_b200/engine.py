@@ -519,7 +519,9 @@ def table_gather_merge_p2p(peer_S_ptrs, Q, B, D):
 
 def score_topn(U, V, user_ids, rated_rowptr, rated_cols, N, rated_value=0.0, out_ids=None, out_scores=None, tensor_cores=None):
     """K8: the N best items of every listed user in one kernel (scores, rated -> rated_value, top-N; nothing
-    materialised).  Returns (ids int32 [n, N], scores fp32 [n, N]), best first, ties by ascending item id.
+    materialised).  1 <= N <= min(101, items).  Returns (ids int32 [n, N], scores fp32 [n, N]), best first, ties by
+    ascending item id (-0.0 and +0.0 one score, written +0.0).  That is not the reference heap's tie rule:
+    evaluate.batched_top_n, the `-eval gpu` path, reproduces the heap's lists on top of this kernel.
     tensor_cores: True = the wgmma 3xTF32 kernel (csrc/topn_tc.cu; d <= 64, multiple of 4), False = the fp32 SIMT kernel
     (csrc/topn_kernels.cu), None = the tensor-core kernel where the width allows it, else the SIMT kernel."""
     torch = _torch()

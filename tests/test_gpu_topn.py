@@ -95,7 +95,9 @@ def test_topn_bad_arguments(torch, E):
     with pytest.raises(E.QRecError):
         E.score_topn(U, V, u, rp, co, 6)                   # N > items
     with pytest.raises(E.QRecError):
-        E.score_topn(U, V, u, rp, co, 101)
+        E.score_topn(torch.ones(4, 8, device='cuda'), torch.ones(200, 8, device='cuda'), u, rp, co, 102)   # N > 101
+    with pytest.raises(E.QRecError):
+        E.score_topn(torch.ones(4, 8, device='cuda'), torch.ones(200, 8, device='cuda'), u, rp, co, 102, tensor_cores=False)
     ids, _ = E.score_topn(U, V, u[:0], rp, co, 3)          # empty block
     assert ids.shape == (0, 3)
     with pytest.raises(E.QRecError):
