@@ -204,13 +204,6 @@ int qrec_bpr_sgd_batch_f32(float* dev_P, float* dev_Q, int32_t d, int64_t n,
                            const int32_t* dev_u, const int32_t* dev_i, const int32_t* dev_j,
                            float lr, float reg_u, float reg_i, double* dev_loss, void* stream);
 
-/* Same step and semantics as qrec_bpr_sgd_batch_f32 for d = 64, with the scatter-add done by the
- * bulk-copy (TMA) engine: row deltas are staged in shared memory and reduced into the tables with
- * cp.reduce.async.bulk...add.f32 (one 256-byte operation per row) instead of per-lane REDG. */
-int qrec_bpr_sgd_batch_tma_f32(float* dev_P, float* dev_Q, int32_t d, int64_t n,
-                               const int32_t* dev_u, const int32_t* dev_i, const int32_t* dev_j,
-                               float lr, float reg_u, float reg_i, double* dev_loss, void* stream);
-
 /* Throughput mode in the reference's own order (model/ranking/BPR.py:31-33: users in id order, each
  * user's positives in CSR order): a lane group keeps P[u] in registers across the user's triples, so
  * P[u] is updated sequentially inside a user -- as in the reference -- and read/written once per
@@ -535,15 +528,6 @@ int qrec_tc_gemm_tf32(int32_t b_is_nk, int32_t M, int32_t N, int32_t K, const fl
                       int32_t lda, const float* dev_B, int32_t ldb, float* dev_C, int32_t ldc,
                       int32_t epilogue, const float* dev_bias, const float* dev_mask,
                       int32_t ldmask, void* stream);
-/* The same product through a persistent, warp-specialised pipeline: one CTA per SM keeps a 64-column
- * block of B resident in shared memory, A arrives by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B tensor
- * map) through a 4-stage mbarrier ring, two consumer warpgroups take the row tiles in turn (wgmma,
- * accumulators in registers) and write their epilogues while the other multiplies.  Same arguments and epilogues; K <= 320, N <= 64 x #SMs.
- * A is consumed as raw fp32 bits (TF32 truncation, error <= 2^-10 per operand; v1 rounds to nearest). */
-int qrec_tc_gemm_tf32_v2(int32_t b_is_nk, int32_t M, int32_t N, int32_t K, const float* dev_A,
-                         int32_t lda, const float* dev_B, int32_t ldb, float* dev_C, int32_t ldc,
-                         int32_t epilogue, const float* dev_bias, const float* dev_mask,
-                         int32_t ldmask, void* stream);
 
 /* =====================================================================================
  * K5 -- NeuMF (model/ranking/NeuMF.py:12-123): row gather / scatter-add around the tensor-core

@@ -131,8 +131,6 @@ SIGNATURES = {
                                                  vp]),
     'qrec_bpr_sgd_batch_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float,
                                          C.c_float, C.c_float, vp, vp]),
-    'qrec_bpr_sgd_batch_tma_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float,
-                                             C.c_float, C.c_float, vp, vp]),
     'qrec_bpr_sgd_usermajor_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int64, C.c_int32, vp, vp, vp, C.c_float,
                                              C.c_float, C.c_float, vp, vp]),
     'qrec_bpr_epoch_usermajor_f32': (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp, C.c_int32,
@@ -199,8 +197,6 @@ SIGNATURES = {
                                       vp, vp, vp, vp, vp, vp, vp, vp]),
     'qrec_mask_rated_f32': (C.c_int, [vp, C.c_int32, C.c_int64, vp, vp, vp, C.c_float, vp]),
     'qrec_tc_gemm_tf32': (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int32, vp, C.c_int32, vp,
-                                    C.c_int32, C.c_int32, vp, vp, C.c_int32, vp]),
-    'qrec_tc_gemm_tf32_v2': (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int32, vp, C.c_int32, vp,
                                     C.c_int32, C.c_int32, vp, vp, C.c_int32, vp]),
 }
 

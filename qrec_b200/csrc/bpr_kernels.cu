@@ -228,113 +228,6 @@ bpr_sgd_staged_kernel(float* __restrict__ P, int nvec, long long n, const int* _
 
 
 // ------------------------------------------------------------------------------------------
-// throughput mode, TMA scatter variant (d = 64): identical gather/compute, but the three row deltas
-// of a triple are parked in shared memory and added to the tables by the bulk-copy engine
-//   cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [row], [smem], 256
-// (one instruction per 256-byte row, issued by one lane, executed by the TMA unit against L2)
-// instead of 16 lanes x REDG.E.ADD.F32x4 through the LSU/L1TEX path that bounds the plain kernel.
-// Shared memory: per warp 2 buffers x (UNROLL*TPW triples x 3 rows x 256 B); a buffer is rewritten
-// only after cp.async.bulk.wait_group.read shows that the engine has read it.
-// ------------------------------------------------------------------------------------------
-// TMA_MASK selects which rows go through the bulk engine (bit 0: P[u], bit 1: Q[i], bit 2: Q[j]);
-// the others keep the REDG path, so the two scatter paths can run side by side.
-template <int UNROLL, int TMA_MASK>
-__global__ void __launch_bounds__(256)
-bpr_sgd_batch_tma_kernel(float* __restrict__ P, float* __restrict__ Q, long long n,
-                         const int* __restrict__ u, const int* __restrict__ i,
-                         const int* __restrict__ j, float lr, float reg_u, float reg_i,
-                         double* loss) {
-  constexpr int LPR = 16, TPW = 2, D = 64;
-  constexpr int ROWS = ((TMA_MASK >> 0) & 1) + ((TMA_MASK >> 1) & 1) + ((TMA_MASK >> 2) & 1);
-  constexpr int SLOT_P = 0, SLOT_I = (TMA_MASK & 1), SLOT_J = (TMA_MASK & 1) + ((TMA_MASK >> 1) & 1);
-  constexpr int SLOT_FLOATS = UNROLL * TPW * ROWS * D;         // per warp, per buffer
-  extern __shared__ __align__(128) float stage[];              // [8 warps][2 buffers][SLOT_FLOATS]
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int sub = lane / LPR, l = lane % LPR;
-  const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-  const float a_u = lr * reg_u, a_i = lr * reg_i;
-  float* my_stage = stage + (size_t)wib * 2 * SLOT_FLOATS;
-  float lsum = 0.f;
-  int buf = 0;
-
-  for (long long base = warp * 32; base < n; base += nwarps * 32) {
-    const long long k = base + lane;
-    int mu = 0, mi = 0, mj = 0;
-    if (k < n) {
-      mu = __ldg(u + k);
-      mi = __ldg(i + k);
-      mj = __ldg(j + k);
-    }
-    const int cnt = (n - base) < 32 ? (int)(n - base) : 32;
-    for (int s0 = 0; s0 < cnt; s0 += TPW * UNROLL) {
-      float4 p[UNROLL], qi[UNROLL], qj[UNROLL];
-      int uu[UNROLL], ii[UNROLL], jj[UNROLL];
-      bool ok[UNROLL];
-#pragma unroll
-      for (int r = 0; r < UNROLL; ++r) {
-        const int t = s0 + r * TPW + sub;
-        uu[r] = __shfl_sync(0xffffffffu, mu, t & 31);
-        ii[r] = __shfl_sync(0xffffffffu, mi, t & 31);
-        jj[r] = __shfl_sync(0xffffffffu, mj, t & 31);
-        ok[r] = t < cnt;
-        if (ok[r]) {
-          p[r] = *reinterpret_cast<const float4*>(P + (size_t)uu[r] * D + l * 4);
-          qi[r] = *reinterpret_cast<const float4*>(Q + (size_t)ii[r] * D + l * 4);
-          qj[r] = *reinterpret_cast<const float4*>(Q + (size_t)jj[r] * D + l * 4);
-        } else {
-          p[r] = qi[r] = qj[r] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-      // the engine must have finished READING the buffer we are about to overwrite (issued two
-      // iterations ago by lanes 0..2 of each lane group; bulk groups are tracked per thread)
-      if (l < 3) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      __syncwarp();
-      float* slot = my_stage + (size_t)buf * SLOT_FLOATS;
-#pragma unroll
-      for (int r = 0; r < UNROLL; ++r) {
-        float x = dot4(p[r], qi[r]) - dot4(p[r], qj[r]);
-        x = group_sum<LPR>(x);
-        const float s = fast_sigmoid(x);
-        const float g = lr * (1.0f - s);
-        if (ok[r]) {
-          if (l == 0) lsum += fast_neg_log(s);
-          float4 dp, dqi, dqj;
-          bpr_step4(p[r], qi[r], qj[r], g, a_u, a_i, dp, dqi, dqj);
-          float* trip = slot + (size_t)(r * TPW + sub) * ROWS * D;
-          if (TMA_MASK & 1) *reinterpret_cast<float4*>(trip + SLOT_P * D + l * 4) = dp;
-          else red_add_v4(P + (size_t)uu[r] * D + l * 4, dp);
-          if (TMA_MASK & 2) *reinterpret_cast<float4*>(trip + SLOT_I * D + l * 4) = dqi;
-          else red_add_v4(Q + (size_t)ii[r] * D + l * 4, dqi);
-          if (TMA_MASK & 4) *reinterpret_cast<float4*>(trip + SLOT_J * D + l * 4) = dqj;
-          else red_add_v4(Q + (size_t)jj[r] * D + l * 4, dqj);
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // st.shared -> visible to the bulk engine
-      __syncwarp();
-      if (l < 3 && ((TMA_MASK >> l) & 1)) {
-        const int srow = (l == 0) ? SLOT_P : (l == 1 ? SLOT_I : SLOT_J);
-#pragma unroll
-        for (int r = 0; r < UNROLL; ++r) {
-          if (ok[r]) {
-            float* dst = (l == 0) ? (P + (size_t)uu[r] * D) : (Q + (size_t)(l == 1 ? ii[r] : jj[r]) * D);
-            const float* src = slot + (size_t)(r * TPW + sub) * ROWS * D + srow * D;
-            asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(dst),
-                         "r"((uint32_t)__cvta_generic_to_shared(src)), "n"(D * 4)
-                         : "memory");
-          }
-        }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-      buf ^= 1;
-    }
-  }
-  if (l < 3) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all reductions performed
-  block_add_loss(lsum, loss);
-}
-
-
-// ------------------------------------------------------------------------------------------
 // throughput mode, user-major (P-stationary): the reference's own iteration order
 // (model/ranking/BPR.py:31-33: for user: for item).  A lane group takes one user, keeps P[u] in
 // registers across that user's triples -- so P[u] is updated SEQUENTIALLY inside a user exactly as
@@ -611,25 +504,6 @@ int qrec_bpr_sgd_batch_f32(float* P, float* Q, int32_t d, int64_t n, const int32
                            const int32_t* i, const int32_t* j, float lr, float reg_u,
                            float reg_i, double* loss, void* stream) {
   return qrec::launch_bpr_batch(P, Q, d, n, u, i, j, lr, reg_u, reg_i, loss, (cudaStream_t)stream);
-}
-
-int qrec_bpr_sgd_batch_tma_f32(float* P, float* Q, int32_t d, int64_t n, const int32_t* u,
-                               const int32_t* i, const int32_t* j, float lr, float reg_u,
-                               float reg_i, double* loss, void* stream) {
-  QREC_REQUIRE(P && Q && loss, "qrec_bpr_sgd_batch_tma_f32: null pointer");
-  QREC_REQUIRE(d == 64, "qrec_bpr_sgd_batch_tma_f32: only d=64 (got %d); use qrec_bpr_sgd_batch_f32", d);
-  QREC_REQUIRE(n >= 0, "qrec_bpr_sgd_batch_tma_f32: n < 0");
-  if (n == 0) return QREC_OK;
-  QREC_REQUIRE(u && i && j, "qrec_bpr_sgd_batch_tma_f32: null index pointer");
-  // only P's row goes through the bulk engine (TMA_MASK 1: the fewest bytes through the copy engine); the item rows
-  // keep REDG
-  constexpr int UN = 4, MASK = 1;
-  constexpr int smem = 8 * 2 * UN * 2 * 64 * 4;   // 8 warps x 2 buffers x UN*2 triples x one 256-byte row
-  QREC_CUDA(allow_dynamic_smem((const void*)bpr_sgd_batch_tma_kernel<UN, MASK>, smem));
-  const int grid = capped_grid(((n + 31) / 32 + 7) / 8, 2);
-  bpr_sgd_batch_tma_kernel<UN, MASK><<<grid, 256, smem, (cudaStream_t)stream>>>(P, Q, n, u, i, j, lr, reg_u, reg_i, loss);
-  QREC_LAUNCH_CHECK();
-  return QREC_OK;
 }
 
 }  // extern "C" (reopened below)

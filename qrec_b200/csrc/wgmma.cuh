@@ -1,7 +1,7 @@
-// Hopper (sm_90a) warpgroup MMA, TF32 in / fp32 accumulate, for the tensor-core kernels (tc_gemm.cu, tc_gemm_v2.cu,
-// topn_tc.cu).  Both operands are read from shared memory in the canonical K-major SWIZZLE_128B layout: rows of
-// 32 fp32 (128 B), 8-row 1024 B atoms, 16-byte chunk index XOR row % 8 -- what sw_off() writes and what a TMA copy
-// with CU_TENSOR_MAP_SWIZZLE_128B produces.  A 128 x K tile is two m64 halves 8 KB apart per 32-wide k-block.
+// Hopper (sm_90a) warpgroup MMA, TF32 in / fp32 accumulate, for the tensor-core kernels (tc_gemm.cu, topn_tc.cu).
+// Both operands are read from shared memory in the canonical K-major SWIZZLE_128B layout: rows of 32 fp32 (128 B),
+// 8-row 1024 B atoms, 16-byte chunk index XOR row % 8 -- what sw_off() writes and what a TMA copy with
+// CU_TENSOR_MAP_SWIZZLE_128B produces.  A 128 x K tile is two m64 halves 8 KB apart per 32-wide k-block.
 //
 // Accumulator fragment of one m64nN instruction (N / 2 floats per thread of the warpgroup): element e of thread
 // (warp w of the warpgroup, lane l) is row 16 w + l / 4 + 8 ((e >> 1) & 1), column 8 (e >> 2) + 2 (l % 4) + (e & 1).

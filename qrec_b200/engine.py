@@ -387,15 +387,13 @@ def bpr_sgd_ordered(P, Q, u, i, j, wu, wi, wj, lr, reg_u, reg_i, loss, n_warps=0
     return loss
 
 
-def bpr_sgd_batch(P, Q, u, i, j, lr, reg_u, reg_i, loss, tma=False):
-    """Throughput mode: fused gather-dot-sigmoid-update-scatter-add over device triples.
-    tma=True (d=64 only) scatters through the bulk-copy engine instead of per-lane REDG."""
+def bpr_sgd_batch(P, Q, u, i, j, lr, reg_u, reg_i, loss):
+    """Throughput mode: fused gather-dot-sigmoid-update-scatter-add over device triples."""
     torch = _torch()
     n = u.shape[0]
     d = P.shape[1]
     assert Q.shape[1] == d and i.shape[0] == n and j.shape[0] == n
-    fn = lib.qrec_bpr_sgd_batch_tma_f32 if tma else lib.qrec_bpr_sgd_batch_f32
-    check(fn(_dev(P, torch.float32, 'P'), _dev(Q, torch.float32, 'Q'), d, n,
+    check(lib.qrec_bpr_sgd_batch_f32(_dev(P, torch.float32, 'P'), _dev(Q, torch.float32, 'Q'), d, n,
                                      _dev(u, torch.int32, 'u'), _dev(i, torch.int32, 'i'),
                                      _dev(j, torch.int32, 'j'), float(lr), float(reg_u),
                                      float(reg_i), _dev(loss, torch.float64, 'loss'), _stream()),
@@ -933,21 +931,6 @@ def tc_gemm(A, B, C, b_is_nk=False, epilogue=EPI_NONE, bias=None, mask=None):
                                 int(epilogue), _opt(bias, torch.float32, 'bias'),
                                 _opt(mask, torch.float32, 'mask'),
                                 _ld(mask) if mask is not None else 0, _stream()), 'qrec_tc_gemm_tf32')
-    return C
-
-
-def tc_gemm_v2(A, B, C, b_is_nk=False, epilogue=EPI_NONE, bias=None, mask=None):
-    """tc_gemm through the persistent TMA-fed pipeline (K <= 320; A taken as raw fp32 bits = TF32
-    truncation).  1.4-1.7 x the v1 kernel at M = 327 680, slower below M ~ 50 000 (persistent pipeline start-up)."""
-    torch = _torch()
-    M, K = A.shape
-    N = B.shape[0] if b_is_nk else B.shape[1]
-    assert (B.shape[1] if b_is_nk else B.shape[0]) == K and tuple(C.shape) == (M, N)
-    check(lib.qrec_tc_gemm_tf32_v2(int(b_is_nk), M, N, K, _dev(A, torch.float32, 'A'), _ld(A),
-                                   _dev(B, torch.float32, 'B'), _ld(B), _dev(C, torch.float32, 'C'), _ld(C),
-                                   int(epilogue), _opt(bias, torch.float32, 'bias'),
-                                   _opt(mask, torch.float32, 'mask'),
-                                   _ld(mask) if mask is not None else 0, _stream()), 'qrec_tc_gemm_tf32_v2')
     return C
 
 

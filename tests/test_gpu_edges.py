@@ -25,7 +25,6 @@ def test_empty_inputs_are_noops(torch, E):
     z32 = torch.zeros(0, dtype=torch.int32, device='cuda')
     loss = torch.zeros(1, dtype=torch.float64, device='cuda')
     E.bpr_sgd_batch(P, Q, z32, z32, z32, 0.1, 0.1, 0.1, loss)
-    E.bpr_sgd_batch(P, Q, z32, z32, z32, 0.1, 0.1, 0.1, loss, tma=True)
     gU, gV = torch.zeros_like(P), torch.zeros_like(Q)
     E.bpr_grad_scatter(P, Q, z32, z32, z32, 1e-7, 0.1, gU, gV, loss)
     rp0 = torch.zeros(1, dtype=torch.int64, device='cuda')

@@ -24,7 +24,7 @@ def _check(torch, C, ref, A, B_kn):
 
 
 @pytest.mark.parametrize('M,N,K', [(128, 64, 32), (128, 64, 64), (256, 128, 128), (10240, 320, 128), (200, 100, 36),
-                                   (1, 1, 4), (129, 65, 68), (10240, 64, 128)])
+                                   (1, 1, 4), (129, 65, 68), (10240, 64, 128), (327680, 320, 128), (10240, 160, 320)])
 def test_forward_layout_bias_relu(torch, E, M, N, K):
     g = torch.Generator(device='cuda'); g.manual_seed(M * 7 + N * 3 + K)
     A = torch.randn(M, K, device='cuda', generator=g)

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """K1 variants on the benchmark workload (50 M triples, 1M x 100K, d=64): the user-major epoch with given and with
-fused-sampled negatives, the stand-alone sampler, and the batch kernel on shuffled triples with REDG scatter vs
-bulk-copy-engine (TMA) scatter.  One JSON line each."""
+fused-sampled negatives, the stand-alone sampler, and the batch kernel on shuffled triples.  One JSON line each."""
 import json
 import os
 import sys
@@ -69,18 +68,17 @@ def main():
         b.record()
         torch.cuda.synchronize()
         print(json.dumps({'kernel': fn_name, 'ms_per_50M': a.elapsed_time(b) / 10}))
-    for name, tma in (('red', False), ('tma', True)):
-        for _ in range(3):
-            E.bpr_sgd_batch(P, Q, u, i, j, 0.01, 0.001, 0.001, loss, tma=tma)
-        torch.cuda.synchronize()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(10):
-            E.bpr_sgd_batch(P, Q, u, i, j, 0.01, 0.001, 0.001, loss, tma=tma)
-        b.record()
-        torch.cuda.synchronize()
-        ms = a.elapsed_time(b) / 10
-        print(json.dumps({'k1_variant': name, 'ms_per_50M': ms, 'G_triples_s': 50 / ms, 'algorithmic_TBs': 50e6 * 1548 / ms / 1e9}))
+    for _ in range(3):
+        E.bpr_sgd_batch(P, Q, u, i, j, 0.01, 0.001, 0.001, loss)
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(10):
+        E.bpr_sgd_batch(P, Q, u, i, j, 0.01, 0.001, 0.001, loss)
+    b.record()
+    torch.cuda.synchronize()
+    ms = a.elapsed_time(b) / 10
+    print(json.dumps({'k1_variant': 'red', 'ms_per_50M': ms, 'G_triples_s': 50 / ms, 'algorithmic_TBs': 50e6 * 1548 / ms / 1e9}))
 
 
 if __name__ == '__main__':

@@ -24,27 +24,23 @@ def main():
             W = torch.randn((N, K) if nk else (K, N), device='cuda', generator=g)
             bias = torch.randn(N, device='cuda', generator=g)
             C = torch.empty(B, N, device='cuda')
-            impls = [('tc_gemm_tf32', E.tc_gemm)]
-            if True:                                                    # v2 validated in round 2
-                impls.append(('tc_gemm_tf32_v2', E.tc_gemm_v2))
-            for name, gemm in impls:
-                fn = ((lambda: gemm(A, W, C, b_is_nk=True)) if nk
-                      else (lambda: gemm(A, W, C, epilogue=E.EPI_BIAS_RELU, bias=bias)))
-                for _ in range(3):
-                    fn()
-                torch.cuda.synchronize()
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record()
-                for _ in range(20):
-                    fn()
-                b.record()
-                torch.cuda.synchronize()
-                ms = a.elapsed_time(b) / 20
-                flops = 2.0 * B * K * N
-                bytes_ = 4.0 * (B * K + K * N + B * N)
-                print(json.dumps({'kernel': name, 'M': B, 'N': N, 'K': K, 'b_is_nk': nk, 'ms': ms,
-                                  'TFLOPs': flops / ms / 1e9, 'GBs': bytes_ / ms / 1e6,
-                                  'note': 'tf32 dense peak is half the bf16 peak (%.0f TF/s measured bf16)' % peak}))
+            fn = ((lambda: E.tc_gemm(A, W, C, b_is_nk=True)) if nk
+                  else (lambda: E.tc_gemm(A, W, C, epilogue=E.EPI_BIAS_RELU, bias=bias)))
+            for _ in range(3):
+                fn()
+            torch.cuda.synchronize()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(20):
+                fn()
+            b.record()
+            torch.cuda.synchronize()
+            ms = a.elapsed_time(b) / 20
+            flops = 2.0 * B * K * N
+            bytes_ = 4.0 * (B * K + K * N + B * N)
+            print(json.dumps({'kernel': 'tc_gemm_tf32', 'M': B, 'N': N, 'K': K, 'b_is_nk': nk, 'ms': ms,
+                              'TFLOPs': flops / ms / 1e9, 'GBs': bytes_ / ms / 1e6,
+                              'note': 'tf32 dense peak is half the bf16 peak (%.0f TF/s measured bf16)' % peak}))
 
 
 if __name__ == '__main__':

@@ -102,9 +102,6 @@ def main():
         E.mf_sgd_ordered(E.EE_RATINGS, P, Q, dev(u9), dev(i9), r9, dev(wu9), dev(wi9), 0.01, 0.01, 0.01, loss, Bu, Bi,
                          0.01, 2.0)
         E.mf_predict_pairs(P, Q, dev(u9), dev(i9), Bu, Bi, 2.0)
-        Hv2 = torch.empty(B, 320, device='cuda')
-        E.tc_gemm_v2(A0, W1, Hv2, epilogue=E.EPI_BIAS_RELU, bias=b1)
-        E.tc_gemm_v2(H1, W1, dX, b_is_nk=True, epilogue=E.EPI_RELU_MASK, mask=A0)
         sig = E.rated_signature(dev(csr.sorted_rowptr), dev(csr.sorted_cols))
         E.bpr_epoch_usermajor_sig(P, Q, dev(csr.pos_rowptr), dev(csr.pos_cols), dev(csr.sorted_rowptr),
                                   dev(csr.sorted_cols), sig, ni, 5, 0, 0.01, 0.001, 0.001, loss)
