@@ -43,22 +43,14 @@ namespace {
 
 using namespace qrec;
 
-constexpr int kThreads = 256;
-constexpr int kStage = 32;         // z rows staged in shared memory at a time
-constexpr int kGramChunk = 2048;   // rows per partial Gram
-constexpr int kMaxD = 128;
-
-__host__ __device__ inline int pad4(int d) { return (d + 3) & ~3; }
-__host__ __device__ inline int tiles_of(int d) { const int nb = pad4(d) / 4; return nb * (nb + 1) / 2; }
-
 // Shared-memory carve-up (doubles): A [d][ld] (ld = pad4(d)+1: odd, so column walks are conflict-free),
 // Zs [kStage][dp], W [kStage], x_old [dp], b [dp], s [dp].
 __host__ __device__ inline int a_words(int d) { return (d * (pad4(d) + 1) + 1) & ~1; }
 inline size_t smem_bytes(int d) { return sizeof(double) * ((size_t)a_words(d) + (size_t)(kStage + 3) * pad4(d) + kStage); }
 
-// The upper-triangle 4x4 tiles of A, split into work items (tile, group): group g accumulates the staged entries
-// k = g, g + ngroups, ...  Small d has few tiles, so the entries are spread over several groups, reduced in group
-// order.  Every tile has a group-0 item (NT * kThreads >= tiles).
+// The upper-triangle 4x4 tiles of A (tiles_of, als_step.cuh), split into work items (tile, group): group g
+// accumulates the staged entries k = g, g + ngroups, ... (als_groups).  Small d has few tiles, so the entries are
+// spread over several groups, reduced in group order.  Every tile has a group-0 item (NT * kThreads >= tiles).
 template <int NT>
 struct Tiles {
   double acc[NT][16];
@@ -67,8 +59,7 @@ struct Tiles {
 
   __device__ void setup(int d) {
     const int nb = pad4(d) / 4, nt = tiles_of(d);
-    ngroups = NT * kThreads / nt;
-    if (ngroups > kStage) ngroups = kStage;
+    ngroups = als_groups(NT, d);
 #pragma unroll
     for (int s = 0; s < NT; ++s) {
       const int id = threadIdx.x + s * kThreads;
@@ -725,12 +716,12 @@ int persistent_grid(K kernel, size_t bytes, long long work, int max_ctas, int* g
 }
 
 // Launches kernel_of(std::integral_constant<int, NT>{})(args...) on its persistent grid, with the tile count NT of a
-// d-wide system: 1 when the upper triangle's 4x4 tiles fit one per thread, else 3 (d <= kMaxD).
+// d-wide system (als_tiles_per_thread).
 template <class KernelOf, class... Args>
 int launch_rows(KernelOf kernel_of, int d, size_t bytes, long long work, int max_ctas, cudaStream_t st,
                 Args... args) {
-  const auto kernel = tiles_of(d) <= kThreads ? kernel_of(std::integral_constant<int, 1>{})
-                                              : kernel_of(std::integral_constant<int, 3>{});
+  const auto kernel = als_tiles_per_thread(d) == 1 ? kernel_of(std::integral_constant<int, 1>{})
+                                                   : kernel_of(std::integral_constant<int, 3>{});
   int grid = 0;
   const int rc = persistent_grid(kernel, bytes, work, max_ctas, &grid);
   if (rc) return rc;

@@ -17,6 +17,23 @@
 
 namespace qrec {
 
+// Tile layout of the ALS-family row solves (als_kernels.cu), stated once for the kernels and for the CPU suite.
+constexpr int kThreads = 256;      // threads per CTA
+constexpr int kStage = 32;         // z rows staged in shared memory at a time
+constexpr int kGramChunk = 2048;   // rows per partial Gram
+constexpr int kMaxD = 128;
+
+// Columns padded to whole 4x4 tiles, and the number of upper-triangle tiles of a d x d system.
+__host__ __device__ inline int pad4(int d) { return (d + 3) & ~3; }
+__host__ __device__ inline int tiles_of(int d) { const int nb = pad4(d) / 4; return nb * (nb + 1) / 2; }
+// Tiles per thread NT of a d-wide system: 1 when the tiles fit one per thread, else 3 (d <= kMaxD).
+__host__ __device__ inline int als_tiles_per_thread(int d) { return tiles_of(d) <= kThreads ? 1 : 3; }
+// Groups the kStage staged rows are split over at NT tiles per thread: group g takes rows g, g + ngroups, ...
+__host__ __device__ inline int als_groups(int nt, int d) {
+  const int g = nt * kThreads / tiles_of(d);
+  return g > kStage ? kStage : g;
+}
+
 // confidence term alpha * v of one entry (WRMF.py:34: 10 * r_ui), and its right-hand-side weight 1 + alpha * v
 template <typename T>
 __host__ __device__ __forceinline__ double als_conf(T v, double alpha) { return alpha * (double)v; }

@@ -66,4 +66,14 @@ int32_t host_als_side_f32(float* X, const float* Z, int d, int64_t n_rows, int64
   return side<float>(X, Z, d, n_rows, n_z, rowptr, cols, vals, lambda, alpha, loss);
 }
 
+// The kernels' tile layout (als_step.cuh), for the CPU suite's shape tables.
+int host_als_pad4(int d) { return qrec::pad4(d); }
+int host_als_tiles_of(int d) { return qrec::tiles_of(d); }
+int host_als_tiles_per_thread(int d) { return qrec::als_tiles_per_thread(d); }
+int host_als_groups(int nt, int d) { return qrec::als_groups(nt, d); }
+int host_als_threads() { return qrec::kThreads; }
+int host_als_stage() { return qrec::kStage; }
+int host_als_gram_chunk() { return qrec::kGramChunk; }
+int host_als_max_d() { return qrec::kMaxD; }
+
 }  // extern "C"

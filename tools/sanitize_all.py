@@ -126,12 +126,13 @@ def main():
         E.simgcl_perturb(X, 0.1, 7, 1, 1, acc=acc, acc_scale=0.5, d_valid=62, row_offset=12345)
         torch.cuda.synchronize()
         print('sanitize_all: + round 2, launched', E.launch_count(), 'kernels')
-        # K10 (WRMF): Gram + row solve, both table types, the one-tile-per-thread and three-tiles-per-thread builds
+        # K10 (WRMF): Gram + row solve, both table types, the one-tile-per-thread and three-tiles-per-thread builds, with
+        # whole and padded tiles (d = 37: NT = 1, four groups; d = 97: NT = 3, two groups)
         rp_u = torch.from_numpy(np.bincount(u, minlength=nu).cumsum()).cuda()
         rowptr = torch.cat([torch.zeros(1, dtype=torch.int64, device='cuda'), rp_u])
         cols = dev(i[np.argsort(u, kind='stable')])
         order = dev(E.als_row_order(rowptr.cpu().numpy()))
-        for dd in (20, 128):
+        for dd in (20, 37, 97, 128):
             for dt in (torch.float64, torch.float32):
                 Xs, Ys = torch.rand(nu, dd, device='cuda', dtype=dt), torch.rand(ni, dd, device='cuda', dtype=dt)
                 G = E.als_gram(Ys)
@@ -162,7 +163,7 @@ def main():
         irp = torch.from_numpy(np.concatenate([[0], np.bincount(pairs[0], minlength=ni).cumsum()])).cuda()
         icol = dev(pairs[1].astype(np.int32))
         srp, scol, sval = E.sppmi_csr(irp, icol, nu, 5, 0)
-        for dd in (20, 128):
+        for dd in (20, 37, 97, 128):
             for dt in (torch.float64, torch.float32):
                 Y, G = torch.rand(ni, dd, device='cuda', dtype=dt), torch.rand(ni, dd, device='cuda', dtype=dt)
                 w, c = torch.rand(ni, device='cuda', dtype=dt), torch.rand(ni, device='cuda', dtype=dt)
@@ -173,7 +174,7 @@ def main():
         print('sanitize_all: + K12, launched', E.launch_count(), 'kernels', 'SPPMI nnz', scol.shape[0])
         # K13 (ExpoMF): the user half (mu by column) and the item half with the prior (mu by row), for both tile
         # builds, over the same interactions (users with no entries included)
-        for dd in (20, 128):
+        for dd in (20, 37, 97, 128):
             th, be = torch.rand(nu, dd, device='cuda') * 0.1, torch.rand(ni, dd, device='cuda') * 0.1
             mu, mu_out = torch.full((ni,), 0.01, device='cuda'), torch.empty(ni, device='cuda')
             E.expomf_half_epoch(th, be, rowptr, cols, mu, False, 1e-5, 1.0, order)
@@ -186,7 +187,7 @@ def main():
         # item half reads the prior with its rows as users, over the entries of the first nu items
         deg = torch.randint(0, 40, (nu,), dtype=torch.int32, device='cuda') * (torch.rand(nu, device='cuda') < 0.5)
         iord = dev(E.als_row_order(irp.cpu().numpy()))
-        for dd in (20, 128):
+        for dd in (20, 37, 97, 128):
             th, be = torch.rand(nu, dd, device='cuda') * 0.1, torch.rand(ni, dd, device='cuda') * 0.1
             A, A_out = None, torch.empty(ni, dtype=torch.float64, device='cuda')
             for _ in range(2):
