@@ -23,6 +23,7 @@ class IterativeRecommender(Recommender):
         super(IterativeRecommender, self).__init__(conf, trainingSet, testSet, fold)
         self.bestPerformance = []
         self.earlyStop = 0
+        self._device_scores = None
 
     def readConfiguration(self):
         super(IterativeRecommender, self).readConfiguration()
@@ -51,6 +52,30 @@ class IterativeRecommender(Recommender):
         dev = torch.device('cuda', self.engine_device)
         torch.cuda.set_device(dev)
         return dev
+
+    def _engine_dtype(self):
+        """The dtype of the device tables: float32 under `-mode fast` or `-precision f32`, else float64."""
+        import torch
+        return torch.float32 if (self.engine_mode == 'fast' or self.engine_precision == 'f32') else torch.float64
+
+    def _upload(self, a, dev, pad=False):
+        """The host array `a` as a table on `dev` in the engine's dtype.  With `pad`, under `-mode fast` a 2-D table
+        gets zero columns up to a multiple of 4: the fast kernels move rows as 16-byte slices, the zero columns stay
+        zero under their updates, and _host drops them."""
+        import torch
+        t = torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=self._engine_dtype())
+        d = t.shape[-1]
+        if not (pad and self.engine_mode == 'fast' and d % 4):
+            return t
+        padded = torch.zeros(t.shape[0], d + (4 - d % 4), device=dev, dtype=t.dtype)
+        padded[:, :d] = t
+        return padded
+
+    def _host(self, t):
+        """A device table as a float64 numpy array, without _upload's padding columns."""
+        if t.dim() == 2:
+            t = t[:, :self.emb_size]
+        return np.ascontiguousarray(t.double().cpu().numpy())
 
     def printAlgorConfig(self):
         super(IterativeRecommender, self).printAlgorConfig()
@@ -119,9 +144,25 @@ class IterativeRecommender(Recommender):
         return converged
 
     def rating_performance(self):
+        """iterativeRecommender.py:104-113.  While a model's tables are resident on the device it may set
+        `_device_scores(tu, ti)`, the predictions of the test set's known (user id, item id) pairs computed there;
+        every other line is predicted by predictForRating."""
+        scored = {}
+        if self._device_scores is not None:
+            if not hasattr(self, '_test_pairs'):
+                import torch
+                dev = self._device()
+                known = [k for k, (un, it, _) in enumerate(self.data.testData)
+                         if self.data.containsUser(un) and self.data.containsItem(it)]
+                tu = np.array([self.data.user[self.data.testData[k][0]] for k in known], dtype=np.int32)
+                ti = np.array([self.data.item[self.data.testData[k][1]] for k in known], dtype=np.int32)
+                self._test_pairs = (known, torch.from_numpy(tu).to(dev), torch.from_numpy(ti).to(dev))
+            known, tu, ti = self._test_pairs
+            scored = dict(zip(known, self._device_scores(tu, ti).double().cpu().tolist()))
         res = []
-        for user, item, rating in self.data.testData:
-            res.append([user, item, rating, self.checkRatingBoundary(self.predictForRating(user, item))])
+        for k, (user, item, rating) in enumerate(self.data.testData):
+            pred = scored[k] if k in scored else self.predictForRating(user, item)
+            res.append([user, item, rating, self.checkRatingBoundary(pred)])
         self.measure = Measure.ratingMeasure(res)
         return self.measure
 

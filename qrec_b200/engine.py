@@ -357,6 +357,12 @@ def _order_counters(device, *lengths):
             + [torch.zeros(1, dtype=torch.int64, device=device)])
 
 
+def ordered_warps(n, depth):
+    """n_warps of an in-order launch over a stream of n entries whose longest dependency chain is `depth`: 16 per unit
+    of the stream's average parallel width n / depth, clamped to the bounds below."""
+    return int(min(2368, max(64, 16 * n / max(1, depth))))
+
+
 def sample_neg_philox(u, sorted_rowptr, sorted_cols, num_items, seed, epoch, out=None):
     torch = _torch()
     n = u.shape[0]

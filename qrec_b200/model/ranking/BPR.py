@@ -30,17 +30,8 @@ class BPR(IterativeRecommender):
         csr = self.data.rated_csr()
         dev = self._device()
         fast = self.engine_mode == 'fast'
-        dtype = torch.float32 if (fast or self.engine_precision == 'f32') else torch.float64
         d = self.emb_size
-        # the fused kernel moves rows as 16-byte slices: pad d to a multiple of 4 with zero columns
-        # (they stay exactly zero under BPR.py:45-52, so the first d columns are unaffected)
-        dpad = d if (not fast or d % 4 == 0) else d + (4 - d % 4)
-
-        def upload(a):
-            t = torch.zeros(a.shape[0], dpad, device=dev, dtype=dtype)
-            t[:, :d] = torch.from_numpy(a).to(device=dev, dtype=dtype)
-            return t.contiguous()
-        P, Q = upload(self.P), upload(self.Q)
+        P, Q = self._upload(self.P, dev, pad=True), self._upload(self.Q, dev, pad=True)
         acc = torch.zeros(3, dtype=torch.float64, device=dev)
         mt = E.MT19937()
         print('training...')
@@ -51,7 +42,7 @@ class BPR(IterativeRecommender):
             random.setstate(mt.getstate())
             du, di, dj = (torch.from_numpy(x).to(dev) for x in (u, i, j))
             acc.zero_()
-            if fast and dpad <= 128:
+            if fast and P.shape[1] <= 128:
                 # the sampler's stream is user-major (BPR.py:31-33): P[u] stays in registers per user
                 E.bpr_sgd_usermajor(P, Q, torch.from_numpy(csr.pos_rowptr).to(dev), di, dj, self.lRate, self.regU,
                                     self.regI, acc[0:1])
@@ -59,10 +50,10 @@ class BPR(IterativeRecommender):
                 E.bpr_sgd_batch(P, Q, du, di, dj, self.lRate, self.regU, self.regI, acc[0:1])
             else:
                 wu, wi, wj = E.bpr_order_prepare(u, i, j, self.num_users, self.num_items)
-                width = len(u) / max(1, E.bpr_order_depth(u, i, j, self.num_users, self.num_items))
+                depth = E.bpr_order_depth(u, i, j, self.num_users, self.num_items)
                 E.bpr_sgd_ordered(P, Q, du, di, dj, torch.from_numpy(wu).to(dev), torch.from_numpy(wi).to(dev),
                                   torch.from_numpy(wj).to(dev), self.lRate, self.regU, self.regI, acc[0:1],
-                                  n_warps=int(min(2368, max(64, 16 * width))))
+                                  n_warps=E.ordered_warps(len(u), depth))
             E.sumsq(P, acc[1:2])
             E.sumsq(Q, acc[2:3])
             a = acc.cpu().numpy()

@@ -70,16 +70,14 @@ class CoFactor(IterativeRecommender):
         import torch
         from ... import engine as E
         dev = self._device()
-        f32 = self.engine_mode == 'fast' or self.engine_precision == 'f32'
-        dtype = torch.float32 if f32 else torch.float64
+        dtype = self._engine_dtype()
         self.X = self.P * 10
         self.Y = self.Q * 10
         self.w = np.random.rand(self.num_items) / 10
         self.c = np.random.rand(self.num_items) / 10
         self.G = np.random.rand(self.num_items, self.emb_size) / 10
         print('training...')
-        X, Y, G, w, c = (torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dtype)
-                         for a in (self.X, self.Y, self.G, self.w, self.c))
+        X, Y, G, w, c = (self._upload(a, dev) for a in (self.X, self.Y, self.G, self.w, self.c))
         rowptr, cols, vals = self.data.rating_csr('user')
         urp, ucol, uval = torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev), \
             torch.from_numpy(vals).to(device=dev, dtype=dtype)
@@ -105,13 +103,9 @@ class CoFactor(IterativeRecommender):
             self.loss = float(loss.item())
             epoch += 1
             print('epoch:', epoch, 'loss:', self.loss)
-        self._sync_host_tables(X, Y, G, w, c)
+        self.X, self.Y, self.G, self.w, self.c = (self._host(t) for t in (X, Y, G, w, c))
 
     buildModel = trainModel
-
-    def _sync_host_tables(self, X, Y, G, w, c):
-        for name, t in (('X', X), ('Y', Y), ('G', G), ('w', w), ('c', c)):
-            setattr(self, name, np.ascontiguousarray(t.double().cpu().numpy()))
 
     def device_tables(self):
         import torch

@@ -172,15 +172,8 @@ class TBPR(SocialRecommender):
                     self.positiveSet[user][item] = 1
         dev = self._device()
         fast = self.engine_mode == 'fast'
-        dtype = torch.float32 if (fast or self.engine_precision == 'f32') else torch.float64
         d = self.emb_size
-        dpad = d if (not fast or d % 4 == 0) else d + (4 - d % 4)
-
-        def upload(a):
-            t = torch.zeros(a.shape[0], dpad, device=dev, dtype=dtype)
-            t[:, :d] = torch.from_numpy(a).to(device=dev, dtype=dtype)
-            return t.contiguous()
-        P, Q = upload(self.P), upload(self.Q)
+        P, Q = self._upload(self.P, dev, pad=True), self._upload(self.Q, dev, pad=True)
         acc = torch.zeros(3, dtype=torch.float64, device=dev)
         print('Training...')
         epoch = 0
@@ -200,7 +193,7 @@ class TBPR(SocialRecommender):
                 ids = np.fromiter((self.data.user[x] for x in self.positiveSet), np.int64, len(self.positiveSet))
                 rowptr[ids + 1] = per_user
                 rowptr = np.cumsum(rowptr)
-                kernel = E.bpr_sgd_usermajor if dpad <= 128 else None
+                kernel = E.bpr_sgd_usermajor if P.shape[1] <= 128 else None
                 da, db = torch.from_numpy(a).to(dev), torch.from_numpy(b).to(dev)
                 if kernel is not None and np.all(np.diff(u) >= 0):
                     kernel(P, Q, torch.from_numpy(rowptr).to(dev), da, db, self.lRate, self.regU, self.regI, acc[0:1])

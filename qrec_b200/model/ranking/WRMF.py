@@ -37,10 +37,8 @@ class WRMF(IterativeRecommender):
         from ... import engine as E
         print('training...')
         dev = self._device()
-        f32 = self.engine_mode == 'fast' or self.engine_precision == 'f32'
-        dtype = torch.float32 if f32 else torch.float64
-        X = torch.from_numpy(np.ascontiguousarray(self.X)).to(device=dev, dtype=dtype)
-        Y = torch.from_numpy(np.ascontiguousarray(self.Y)).to(device=dev, dtype=dtype)
+        dtype = self._engine_dtype()
+        X, Y = self._upload(self.X, dev), self._upload(self.Y, dev)
         sides = []
         for by in ('user', 'item'):
             rowptr, cols, vals = self.data.rating_csr(by)
@@ -66,13 +64,9 @@ class WRMF(IterativeRecommender):
             # with item.ranking off, isConverged scores ratings from P / Q, which WRMF never trains (as in the reference)
             if self.isConverged(epoch):
                 break
-        self._sync_host_tables(X, Y)
+        self.X, self.Y = self._host(X), self._host(Y)
 
     buildModel = trainModel
-
-    def _sync_host_tables(self, X, Y):
-        self.X = np.ascontiguousarray(X.double().cpu().numpy())
-        self.Y = np.ascontiguousarray(Y.double().cpu().numpy())
 
     def device_tables(self):
         import torch

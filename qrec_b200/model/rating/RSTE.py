@@ -9,12 +9,12 @@ shuffles the list, as in the reference.  The per-epoch test evaluation scores th
 (qrec_rste_predict_pairs_*).  P and Q are float64 numpy arrays between epochs."""
 import numpy as np
 
+from ...base.socialRecommender import SocialRecommender
 from ...util import config
-from ...util.measure import Measure
-from ._social_rating import SocialRatingMF, followee_csr
+from ._social_rating import followee_csr
 
 
-class RSTE(SocialRatingMF):
+class RSTE(SocialRecommender):
     def __init__(self, conf, trainingSet=None, testSet=None, relation=list(), fold='[1]'):
         super(RSTE, self).__init__(conf, trainingSet, testSet, relation, fold)
 
@@ -37,58 +37,32 @@ class RSTE(SocialRatingMF):
         import torch
         from ... import engine as E
         dev = self._device()
-        dtype = self._engine_dtype()
-        U, d = self.num_users, self.emb_size
-        P, Q = self._upload(self.P, dev, dtype, d), self._upload(self.Q, dev, dtype, d)
+        U = self.num_users
+        P, Q = self._upload(self.P, dev), self._upload(self.Q, dev)
         rowptr, cols, w, denom = self._followees()
-        social = (torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev),
-                  torch.from_numpy(w).to(device=dev, dtype=dtype), torch.from_numpy(denom).to(device=dev, dtype=dtype))
+        social = (torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev), self._upload(w, dev),
+                  self._upload(denom, dev))
         acc = torch.zeros(3, dtype=torch.float64, device=dev)
-        self._device_state = (P, Q, social)
+        # the per-epoch test evaluation scores the known pairs from the resident tables
+        self._device_scores = lambda tu, ti: E.rste_predict_pairs(P, Q, tu, ti, *social, self.alpha)
         epoch = 0
         while epoch < self.maxEpoch:
             u, i, r = self.data.training_ids()                     # current (shuffled) list order
             wu, wi, wr, pos_rowptr, pos, depth = E.rste_order_prepare(u, i, U, self.num_items, rowptr, cols)
             dv = [torch.from_numpy(a).to(dev) for a in (u, i, wu, wi, wr, pos_rowptr, pos)]
             acc.zero_()
-            E.rste_sgd_ordered(P, Q, dv[0], dv[1], torch.from_numpy(r).to(device=dev, dtype=dtype), dv[2], dv[3], dv[4],
-                               dv[5], dv[6], *social, self.lRate, self.regU, self.regI, self.alpha, acc[0:1],
-                               n_warps=self._launch_width(len(u), depth))
+            E.rste_sgd_ordered(P, Q, dv[0], dv[1], self._upload(r, dev), dv[2], dv[3], dv[4], dv[5], dv[6], *social,
+                               self.lRate, self.regU, self.regI, self.alpha, acc[0:1],
+                               n_warps=E.ordered_warps(len(u), depth))
             E.sumsq(P, acc[1:2]); E.sumsq(Q, acc[2:3])
             a = acc.cpu().numpy()
             self.loss = float(a[0] + (self.regU * a[1] + self.regI * a[2]))
             self.P, self.Q = self._host(P), self._host(Q)
             epoch += 1
             self.isConverged(epoch)                                # RSTE.py:39: the verdict is not used
-        self._device_state = None
+        self._device_scores = None
 
     buildModel = trainModel
-
-    # ------------------------------------------------------------------ evaluation
-    def rating_performance(self):
-        """iterativeRecommender.py:104-113 with the known test pairs scored on the device from the resident
-        tables; a line with an unknown user or item predicts globalMean (RSTE.py:63-64)."""
-        state = getattr(self, '_device_state', None)
-        if state is None:
-            return super(RSTE, self).rating_performance()
-        import torch
-        from ... import engine as E
-        P, Q, social = state
-        if not hasattr(self, '_test_pairs'):
-            known = [k for k, (un, it, _) in enumerate(self.data.testData)
-                     if self.data.containsUser(un) and self.data.containsItem(it)]
-            tu = np.array([self.data.user[self.data.testData[k][0]] for k in known], dtype=np.int32)
-            ti = np.array([self.data.item[self.data.testData[k][1]] for k in known], dtype=np.int32)
-            self._test_pairs = (known, torch.from_numpy(tu).to(P.device), torch.from_numpy(ti).to(P.device))
-        known, tu, ti = self._test_pairs
-        scores = E.rste_predict_pairs(P, Q, tu, ti, *social, self.alpha).double().cpu().numpy()
-        pos = dict(zip(known, range(len(known))))
-        res = []
-        for k, (user, item, rating) in enumerate(self.data.testData):
-            pred = float(scores[pos[k]]) if k in pos else self.data.globalMean
-            res.append([user, item, rating, self.checkRatingBoundary(pred)])
-        self.measure = Measure.ratingMeasure(res)
-        return self.measure
 
     def predictForRating(self, u, i):
         """RSTE.py:41-64 on the host tables, for the final evaluation and single pairs."""

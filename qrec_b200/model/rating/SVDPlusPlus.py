@@ -24,7 +24,6 @@ import numpy as np
 
 from ._pointwise import PointwiseMF
 from ...util.config import OptionConf
-from ...util.measure import Measure
 
 
 class SVDPlusPlus(PointwiseMF):
@@ -62,22 +61,25 @@ class SVDPlusPlus(PointwiseMF):
         from ... import engine as E
         dev = self._device()
         fast = self.engine_mode == 'fast'
-        dtype = torch.float32 if (fast or self.engine_precision == 'f32') else torch.float64
-        d = self.emb_size
-        dpad = d if (not fast or d % 4 == 0) else d + (4 - d % 4)      # zero columns stay zero under the update
-        P, Q, Y = (self._upload(t, dev, dtype, dpad) for t in (self.P, self.Q, self.Y))
-        Bu, Bi = self._upload(self.Bu, dev, dtype), self._upload(self.Bi, dev, dtype)
+        P, Q, Y = (self._upload(t, dev, pad=True) for t in (self.P, self.Q, self.Y))
+        Bu, Bi = self._upload(self.Bu, dev), self._upload(self.Bi, dev)
         gm = float(self.data.globalMean)
         rowptr, cols, vals = self.data.rating_csr('user')
         drp, dcols = torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev)
         acc = torch.zeros(6, dtype=torch.float64, device=dev)
-        self._device_state = None
         if fast:
-            dvals = torch.from_numpy(vals).to(device=dev, dtype=dtype)
+            dvals = torch.from_numpy(vals).to(device=dev, dtype=P.dtype)
             order = torch.from_numpy(E.als_row_order(rowptr)).to(dev)
             top_share = np.bincount(cols, minlength=self.num_items).max() / float(max(1, self.num_users))
-            ivals = torch.from_numpy(1.0 / np.repeat(np.diff(rowptr), np.diff(rowptr))).to(device=dev, dtype=dtype)
-            self._device_state = (P, Q, Y, Bu, Bi, gm, drp, dcols, ivals)
+            ivals = torch.from_numpy(1.0 / np.repeat(np.diff(rowptr), np.diff(rowptr))).to(device=dev, dtype=P.dtype)
+
+            def scores(tu, ti):
+                """Test pairs scored from the resident tables: Z = D^-1 R Y (the mean implicit row of every user,
+                qrec_spmm_csr_f32 with values 1/w), then Z[u].Q[i] + (P[u].Q[i] + mean + Bi[i] + Bu[u])."""
+                Z = torch.empty_like(P)
+                E.spmm_csr(drp, dcols, ivals, Y, Z)
+                return E.mf_predict_pairs(Z, Q, tu, ti).double() + E.mf_predict_pairs(P, Q, tu, ti, Bu, Bi, gm).double()
+            self._device_scores = scores
         epoch = 0
         while epoch < self.maxEpoch:
             acc.zero_()
@@ -88,55 +90,23 @@ class SVDPlusPlus(PointwiseMF):
             else:
                 u, i, r = self.data.training_ids()                  # current (shuffled) list order
                 E.svdpp_sgd_ordered(P, Q, Y, Bu, Bi, torch.from_numpy(u).to(dev), torch.from_numpy(i).to(dev),
-                                    torch.from_numpy(r).to(device=dev, dtype=dtype), drp, dcols, self.lRate, self.regU,
-                                    self.regI, self.regB, self.regY, gm, acc[0:1])
+                                    torch.from_numpy(r).to(device=dev, dtype=P.dtype), drp, dcols, self.lRate,
+                                    self.regU, self.regI, self.regB, self.regY, gm, acc[0:1])
             for k, t in enumerate((P, Q, Y, Bu, Bi)):
                 E.sumsq(t, acc[k + 1:k + 2])
             a = acc.cpu().numpy()
             self.loss = float(a[0] + (self.regU * a[1] + self.regI * a[2] + self.regY * a[3]
                                       + self.regB * (a[4] + a[5])))
             if not fast:
-                self._sync_host_tables(P, Q, Y, Bu, Bi)             # rating_performance reads the host tables
+                self.Y = self._host(Y)                              # rating_performance reads the host tables
+                self._sync_host_tables(P, Q, Bu, Bi)
             epoch += 1
             self.isConverged(epoch)                                 # SVDPlusPlus.py:67: never stops training
-        self._sync_host_tables(P, Q, Y, Bu, Bi)
-        self._device_state = None
+        self.Y = self._host(Y)
+        self._sync_host_tables(P, Q, Bu, Bi)
+        self._device_scores = None
 
     buildModel = trainModel
-
-    def _sync_host_tables(self, P, Q, Y, Bu, Bi):
-        super(SVDPlusPlus, self)._sync_host_tables(P, Q, Bu, Bi)
-        self.Y = np.ascontiguousarray(Y[:, :self.emb_size].double().cpu().numpy())
-
-    # ------------------------------------------------------------------ evaluation
-    def rating_performance(self):
-        """iterativeRecommender.py:104-113.  In fast mode the known (user, item) pairs of the test set are scored on
-        the device: Z = D^-1 R Y (the mean implicit row of every user, qrec_spmm_csr_f32 with values 1/w), then
-        Z[u].Q[i] + (P[u].Q[i] + mean + Bi[i] + Bu[u]) with qrec_mf_predict_pairs_f32; other pairs get the global
-        mean, as in predictForRating."""
-        state = getattr(self, '_device_state', None)
-        if state is None:
-            return super(PointwiseMF, self).rating_performance()
-        import torch
-        from ... import engine as E
-        P, Q, Y, Bu, Bi, gm, drp, dcols, ivals = state
-        if not hasattr(self, '_test_pairs'):
-            known = [k for k, (un, it, _) in enumerate(self.data.testData)
-                     if self.data.containsUser(un) and self.data.containsItem(it)]
-            tu = np.array([self.data.user[self.data.testData[k][0]] for k in known], dtype=np.int32)
-            ti = np.array([self.data.item[self.data.testData[k][1]] for k in known], dtype=np.int32)
-            self._test_pairs = (known, torch.from_numpy(tu).to(P.device), torch.from_numpy(ti).to(P.device))
-        known, tu, ti = self._test_pairs
-        Z = torch.empty_like(P)
-        E.spmm_csr(drp, dcols, ivals, Y, Z)
-        scores = (E.mf_predict_pairs(Z, Q, tu, ti).double() + E.mf_predict_pairs(P, Q, tu, ti, Bu, Bi, gm).double())
-        scores = scores.cpu().numpy()
-        res, pos = [], dict(zip(known, range(len(known))))
-        for k, (user, item, rating) in enumerate(self.data.testData):
-            pred = float(scores[pos[k]]) if k in pos else self.predictForRating(user, item)
-            res.append([user, item, rating, self.checkRatingBoundary(pred)])
-        self.measure = Measure.ratingMeasure(res)
-        return self.measure
 
     def predictForRating(self, u, i):
         """SVDPlusPlus.py:70-88, in its order: sequential row sum, /w, dot, then P.Q + mean + Bi + Bu."""

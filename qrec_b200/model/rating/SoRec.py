@@ -11,11 +11,12 @@ import math
 
 import numpy as np
 
+from ...base.socialRecommender import SocialRecommender
 from ...util import config
-from ._social_rating import SocialRatingMF
+from ._pointwise import ordered_rating_pass
 
 
-class SoRec(SocialRatingMF):
+class SoRec(SocialRecommender):
     def __init__(self, conf, trainingSet=None, testSet=None, relation=list(), fold='[1]'):
         super(SoRec, self).__init__(conf, trainingSet, testSet, relation, fold)
 
@@ -52,24 +53,18 @@ class SoRec(SocialRatingMF):
         import torch
         from ... import engine as E
         dev = self._device()
-        dtype = self._engine_dtype()
-        U, d = self.num_users, self.emb_size
-        P, Q, Z = (self._upload(t, dev, dtype, d) for t in (self.P, self.Q, self.Z))
+        U = self.num_users
+        P, Q, Z = (self._upload(t, dev) for t in (self.P, self.Q, self.Z))
         eu, ev, et = self.edge_targets()
         ewu, ewv = E.mf_order_prepare(eu, ev, U, U)
         edges = [torch.from_numpy(a).to(dev) for a in (eu, ev, ewu, ewv)]
-        dt_edge = torch.from_numpy(et).to(device=dev, dtype=dtype)
-        edge_warps = self._launch_width(len(eu), E.mf_order_depth(eu, ev, U, U))
+        dt_edge = self._upload(et, dev)
+        edge_warps = E.ordered_warps(len(eu), E.mf_order_depth(eu, ev, U, U))
         acc = torch.zeros(5, dtype=torch.float64, device=dev)
         epoch = 0
         while epoch < self.maxEpoch:
-            u, i, r = self.data.training_ids()                     # current (shuffled) list order
-            wu, wi = E.mf_order_prepare(u, i, U, self.num_items)
             acc.zero_()
-            E.mf_sgd_ordered(1, P, Q, torch.from_numpy(u).to(dev), torch.from_numpy(i).to(dev),
-                             torch.from_numpy(r).to(device=dev, dtype=dtype), torch.from_numpy(wu).to(dev),
-                             torch.from_numpy(wi).to(dev), self.lRate, self.regU, self.regI, acc[0:1],
-                             n_warps=self._launch_width(len(u), E.mf_order_depth(u, i, U, self.num_items)))
+            ordered_rating_pass(self, 1, P, Q, acc[0:1])
             E.mf_sgd_ordered(E.SOREC_EDGES, P, Z, edges[0], edges[1], dt_edge, edges[2], edges[3], self.lRate,
                              self.regS, self.regZ, acc[1:2], n_warps=edge_warps)
             E.sumsq(P, acc[2:3]); E.sumsq(Q, acc[3:4]); E.sumsq(Z, acc[4:5])

@@ -14,11 +14,13 @@ from collections import defaultdict
 
 import numpy as np
 
+from ...base.socialRecommender import SocialRecommender
 from ...util import config
-from ._social_rating import SocialRatingMF, follower_csr, visit_order
+from ._pointwise import ordered_rating_pass
+from ._social_rating import user_pass_setup
 
 
-class SoReg(SocialRatingMF):
+class SoReg(SocialRecommender):
     def __init__(self, conf, trainingSet=None, testSet=None, relation=list(), fold='[1]'):
         super(SoReg, self).__init__(conf, trainingSet, testSet, relation, fold)
 
@@ -71,26 +73,14 @@ class SoReg(SocialRatingMF):
         import torch
         from ... import engine as E
         dev = self._device()
-        dtype = self._engine_dtype()
-        U, d = self.num_users, self.emb_size
-        P, Q = self._upload(self.P, dev, dtype, d), self._upload(self.Q, dev, dtype, d)
-        rowptr, cols, sim_f = self.followee_sims()
-        grp, gcols, sim_g = follower_csr(self.data, self.social, self.Sim)
-        visit = visit_order(self.data, self.social)
-        pos, depth = E.social_order_prepare(visit, U, rowptr, cols, grp, gcols)
-        t = lambda a: torch.from_numpy(a).to(dev)                    # noqa: E731
-        v = lambda a: torch.from_numpy(a).to(device=dev, dtype=dtype)   # noqa: E731
-        social = (t(visit), t(pos), t(rowptr), t(cols), v(sim_f), t(grp), t(gcols), v(sim_g))
-        pass_warps = self._launch_width(len(visit), depth)
+        P, Q = self._upload(self.P, dev), self._upload(self.Q, dev)
+        social, sim_g, pass_warps = user_pass_setup(self, P, self.Sim)
         acc = torch.zeros(4, dtype=torch.float64, device=dev)
         epoch = 0
         while epoch < self.maxEpoch:
-            u, i, r = self.data.training_ids()                     # current (shuffled) list order
-            wu, wi = E.mf_order_prepare(u, i, U, self.num_items)
             acc.zero_()
-            E.mf_sgd_ordered(1, P, Q, t(u), t(i), v(r), t(wu), t(wi), self.lRate, self.regU, self.regI, acc[0:1],
-                             n_warps=self._launch_width(len(u), E.mf_order_depth(u, i, U, self.num_items)))
-            E.social_user_pass(E.SOCIAL_PASS_KINDS['SoReg'], P, *social, self.lRate, self.alpha, acc[1:2],
+            ordered_rating_pass(self, 1, P, Q, acc[0:1])
+            E.social_user_pass(E.SOCIAL_PASS_KINDS['SoReg'], P, *social, sim_g, self.lRate, self.alpha, acc[1:2],
                                n_warps=pass_warps)
             E.sumsq(P, acc[2:3]); E.sumsq(Q, acc[3:4])
             a = acc.cpu().numpy()
@@ -101,17 +91,3 @@ class SoReg(SocialRatingMF):
                 break
 
     buildModel = trainModel
-
-    def followee_sims(self):
-        """The cleaned followee dicts as a CSR over the training users' ids with Sim[u][f] as values."""
-        U = len(self.data.user)
-        rowptr = np.zeros(U + 1, np.int64)
-        cols, vals = [], []
-        for k in range(U):
-            name = self.data.id2user[k]
-            for f in self.social.getFollowees(name):
-                if self.data.containsUser(f):
-                    cols.append(self.data.user[f])
-                    vals.append(self.Sim[name][f])
-            rowptr[k + 1] = len(cols)
-        return rowptr, np.array(cols, np.int32), np.array(vals, np.float64)

@@ -8,10 +8,12 @@ An epoch is the reference's two passes, each one in-order launch:
     weights sum to 0), P[u] -= (lr*regS)*rl.
 The loss is sum e^2 + regS*sum |rl|^2 + regU|P|^2 + regI|Q|^2, and training stops when isConverged says so, as in
 the reference.  `-tf` is the base class's behaviour.  P and Q are float64 numpy arrays between epochs."""
-from ._social_rating import SocialRatingMF, follower_csr, followee_csr, visit_order
+from ...base.socialRecommender import SocialRecommender
+from ._pointwise import ordered_rating_pass
+from ._social_rating import user_pass_setup
 
 
-class SocialMF(SocialRatingMF):
+class SocialMF(SocialRecommender):
     def __init__(self, conf, trainingSet=None, testSet=None, relation=None, fold='[1]'):
         super(SocialMF, self).__init__(conf, trainingSet, testSet, relation, fold)
 
@@ -22,27 +24,14 @@ class SocialMF(SocialRatingMF):
         import torch
         from ... import engine as E
         dev = self._device()
-        dtype = self._engine_dtype()
-        U, d = self.num_users, self.emb_size
-        P, Q = self._upload(self.P, dev, dtype, d), self._upload(self.Q, dev, dtype, d)
-        rowptr, cols, w, _ = followee_csr(self.data, self.social)
-        grp, gcols, _ = follower_csr(self.data, self.social)
-        visit = visit_order(self.data, self.social)
-        pos, depth = E.social_order_prepare(visit, U, rowptr, cols, grp, gcols)
-        t = lambda a: torch.from_numpy(a).to(dev)                    # noqa: E731
-        social = (t(visit), t(pos), t(rowptr), t(cols), torch.from_numpy(w).to(device=dev, dtype=dtype), t(grp),
-                  t(gcols), None)
-        pass_warps = self._launch_width(len(visit), depth)
+        P, Q = self._upload(self.P, dev), self._upload(self.Q, dev)
+        social, _, pass_warps = user_pass_setup(self, P)
         acc = torch.zeros(4, dtype=torch.float64, device=dev)
         epoch = 0
         while epoch < self.maxEpoch:
-            u, i, r = self.data.training_ids()                     # current (shuffled) list order
-            wu, wi = E.mf_order_prepare(u, i, U, self.num_items)
             acc.zero_()
-            E.mf_sgd_ordered(E.SOCIALMF_RATINGS, P, Q, t(u), t(i), torch.from_numpy(r).to(device=dev, dtype=dtype),
-                             t(wu), t(wi), self.lRate, self.regU, self.regI, acc[0:1],
-                             n_warps=self._launch_width(len(u), E.mf_order_depth(u, i, U, self.num_items)))
-            E.social_user_pass(E.SOCIAL_PASS_KINDS['SocialMF'], P, *social, self.lRate, self.regS, acc[1:2],
+            ordered_rating_pass(self, E.SOCIALMF_RATINGS, P, Q, acc[0:1])
+            E.social_user_pass(E.SOCIAL_PASS_KINDS['SocialMF'], P, *social, None, self.lRate, self.regS, acc[1:2],
                                n_warps=pass_warps)
             E.sumsq(P, acc[2:3]); E.sumsq(Q, acc[3:4])
             a = acc.cpu().numpy()

@@ -13,14 +13,11 @@ P, Q, Bu and Bi are refreshed after every epoch, because evaluation and ranking 
 `-eval gpu` ranks on the host."""
 import numpy as np
 
-from ._social_rating import SocialRatingMF
+from ._pointwise import ordered_rating_pass
 
 
 class EuclideanMF(object):
     """Mixin ahead of the reference's base class (IterativeRecommender for EE, the social one for SREE)."""
-    _engine_dtype = SocialRatingMF._engine_dtype
-    _host = staticmethod(SocialRatingMF._host)
-    _launch_width = staticmethod(SocialRatingMF._launch_width)
 
     def initModel(self):
         super(EuclideanMF, self).initModel()
@@ -28,7 +25,7 @@ class EuclideanMF(object):
         self.Bu = np.random.rand(self.data.trainingSize()[0]) / 10
         self.Bi = np.random.rand(self.data.trainingSize()[1]) / 10
 
-    def _user_pass(self, P, dev, dtype):
+    def _user_pass(self, P):
         """A callable adding the social pass of an epoch to a float64 loss slot, or None (EE)."""
         return None
 
@@ -36,22 +33,14 @@ class EuclideanMF(object):
         import torch
         from ... import engine as E
         dev = self._device()
-        dtype = self._engine_dtype()
-        tables = [torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dtype)
-                  for a in (self.P, self.Q, self.Bu, self.Bi)]
+        tables = [self._upload(a, dev) for a in (self.P, self.Q, self.Bu, self.Bi)]
         P, Q, Bu, Bi = tables
-        user_pass = self._user_pass(P, dev, dtype)
-        t = lambda a: torch.from_numpy(a).to(dev)                    # noqa: E731
-        gm = float(self.data.globalMean)
+        user_pass = self._user_pass(P)
         acc = torch.zeros(2, dtype=torch.float64, device=dev)
         epoch = 0
         while epoch < self.maxEpoch:
-            u, i, r = self.data.training_ids()                     # current (shuffled) list order
-            wu, wi = E.mf_order_prepare(u, i, self.num_users, self.num_items)
             acc.zero_()
-            E.mf_sgd_ordered(E.EE_RATINGS, P, Q, t(u), t(i), torch.from_numpy(r).to(device=dev, dtype=dtype), t(wu),
-                             t(wi), self.lRate, self.regU, self.regI, acc[0:1], Bu, Bi, self.regB, gm,
-                             n_warps=self._launch_width(len(u), E.mf_order_depth(u, i, self.num_users, self.num_items)))
+            ordered_rating_pass(self, E.EE_RATINGS, P, Q, acc[0:1], Bu, Bi)
             if user_pass is not None:
                 user_pass(acc[1:2])
             a = acc.cpu().numpy()

@@ -16,7 +16,21 @@ Here an epoch is one launch over the id-mapped (u, i, r) arrays of the list's cu
 import numpy as np
 
 from ...base.iterativeRecommender import IterativeRecommender
-from ...util.measure import Measure
+
+
+def ordered_rating_pass(model, kind, P, Q, loss, Bu=None, Bi=None):
+    """One in-order K9 launch of `kind` over model's training list in its current order: sequential-equivalent, in
+    place on the device tables P and Q (and the biases Bu / Bi, around globalMean), with model's learning rate and
+    regU / regI / regB.  loss (a float64 slot) += the pass's loss terms."""
+    import torch
+    from ... import engine as E
+    u, i, r = model.data.training_ids()
+    wu, wi = E.mf_order_prepare(u, i, model.num_users, model.num_items)
+    depth = E.mf_order_depth(u, i, model.num_users, model.num_items)
+    t = lambda a: torch.from_numpy(a).to(P.device)                  # noqa: E731
+    gm = 0.0 if Bu is None else float(model.data.globalMean)
+    E.mf_sgd_ordered(kind, P, Q, t(u), t(i), model._upload(r, P.device), t(wu), t(wi), model.lRate, model.regU,
+                     model.regI, loss, Bu, Bi, model.regB, gm, n_warps=E.ordered_warps(len(u), depth))
 
 
 class PointwiseMF(IterativeRecommender):
@@ -33,57 +47,38 @@ class PointwiseMF(IterativeRecommender):
         return self.regU * sums[0] + self.regI * sums[1]
 
     # ------------------------------------------------------------------ engine
-    def _upload(self, a, dev, dtype, dpad=None):
-        import torch
-        if a.ndim == 1:
-            return torch.from_numpy(a).to(device=dev, dtype=dtype).contiguous()
-        t = torch.zeros(a.shape[0], dpad, device=dev, dtype=dtype)
-        t[:, :a.shape[1]] = torch.from_numpy(a).to(device=dev, dtype=dtype)
-        return t.contiguous()
-
     def _sync_host_tables(self, P, Q, Bu, Bi):
-        d = self.emb_size
-        self.P = np.ascontiguousarray(P[:, :d].double().cpu().numpy())
-        self.Q = np.ascontiguousarray(Q[:, :d].double().cpu().numpy())
+        self.P, self.Q = self._host(P), self._host(Q)
         if Bu is not None:
-            self.Bu, self.Bi = Bu.double().cpu().numpy(), Bi.double().cpu().numpy()
+            self.Bu, self.Bi = self._host(Bu), self._host(Bi)
 
     def trainModel(self):
         import torch
         from ... import engine as E
         dev = self._device()
         fast = self.engine_mode == 'fast'
-        dtype = torch.float32 if (fast or self.engine_precision == 'f32') else torch.float64
-        d = self.emb_size
-        dpad = d if (not fast or d % 4 == 0) else d + (4 - d % 4)      # zero columns stay zero under the update
-        P, Q = self._upload(self.P, dev, dtype, dpad), self._upload(self.Q, dev, dtype, dpad)
+        P, Q = self._upload(self.P, dev, pad=True), self._upload(self.Q, dev, pad=True)
         biased = self.KIND == 2
-        Bu = self._upload(self.Bu, dev, dtype) if biased else None
-        Bi = self._upload(self.Bi, dev, dtype) if biased else None
+        Bu = self._upload(self.Bu, dev) if biased else None
+        Bi = self._upload(self.Bi, dev) if biased else None
         gm = float(self.data.globalMean) if biased else 0.0
         acc = torch.zeros(5, dtype=torch.float64, device=dev)
-        self._device_state = (P, Q, Bu, Bi, gm) if fast else None
-        top_share = 1.0
         if fast:
+            # test pairs are scored from the resident tables
+            self._device_scores = lambda tu, ti: E.mf_predict_pairs(P, Q, tu, ti, Bu, Bi, gm)
             u, i, _ = self.data.training_ids()
             top_share = max(int(np.bincount(u).max()), int(np.bincount(i).max())) / float(len(u))
             self.shuffle_training_data()                            # file order is user-sorted: spread the rows
         epoch = 0
         while epoch < self.maxEpoch:
-            u, i, r = self.data.training_ids()                      # current (shuffled) list order
-            window = self._fast_window(top_share)
-            du, di = torch.from_numpy(u).to(dev), torch.from_numpy(i).to(dev)
-            dr = torch.from_numpy(r).to(device=dev, dtype=dtype)
             acc.zero_()
             if fast:
-                E.mf_sgd_batch(self.KIND, P, Q, du, di, dr, self.lRate, self.regU, self.regI, acc[0:1], Bu, Bi,
-                               self.regB, gm, max_inflight=window)
+                u, i, r = self.data.training_ids()                  # current (shuffled) list order
+                E.mf_sgd_batch(self.KIND, P, Q, torch.from_numpy(u).to(dev), torch.from_numpy(i).to(dev),
+                               torch.from_numpy(r).to(device=dev, dtype=P.dtype), self.lRate, self.regU, self.regI,
+                               acc[0:1], Bu, Bi, self.regB, gm, max_inflight=self._fast_window(top_share))
             else:
-                wu, wi = E.mf_order_prepare(u, i, self.num_users, self.num_items)
-                width = len(u) / max(1, E.mf_order_depth(u, i, self.num_users, self.num_items))
-                E.mf_sgd_ordered(self.KIND, P, Q, du, di, dr, torch.from_numpy(wu).to(dev), torch.from_numpy(wi).to(dev),
-                                 self.lRate, self.regU, self.regI, acc[0:1], Bu, Bi, self.regB, gm,
-                                 n_warps=int(min(2368, max(64, 16 * width))))
+                ordered_rating_pass(self, self.KIND, P, Q, acc[0:1], Bu, Bi)
             if self.KIND != 0:
                 E.sumsq(P, acc[1:2]); E.sumsq(Q, acc[2:3])
                 if biased:
@@ -96,7 +91,7 @@ class PointwiseMF(IterativeRecommender):
             if self._epoch_end(epoch):
                 break
         self._sync_host_tables(P, Q, Bu, Bi)
-        self._device_state = None
+        self._device_scores = None
 
     buildModel = trainModel
 
@@ -108,29 +103,3 @@ class PointwiseMF(IterativeRecommender):
     def _epoch_end(self, epoch):
         """PMF / BasicMF stop when converged (PMF.py:26-27); SVD ignores the flag (SVD.py:36)."""
         return self.isConverged(epoch)
-
-    # ------------------------------------------------------------------ evaluation
-    def rating_performance(self):
-        """iterativeRecommender.py:104-113.  In fast mode the known (user, item) pairs of the test set are
-        scored on the device from the resident tables; unknown users / items fall back to the means as
-        in predictForRating (iterativeRecommender.py:66-73)."""
-        state = getattr(self, '_device_state', None)
-        if state is None:
-            return super(PointwiseMF, self).rating_performance()
-        import torch
-        from ... import engine as E
-        P, Q, Bu, Bi, gm = state
-        if not hasattr(self, '_test_pairs'):
-            known = [k for k, (un, it, _) in enumerate(self.data.testData)
-                     if self.data.containsUser(un) and self.data.containsItem(it)]
-            tu = np.array([self.data.user[self.data.testData[k][0]] for k in known], dtype=np.int32)
-            ti = np.array([self.data.item[self.data.testData[k][1]] for k in known], dtype=np.int32)
-            self._test_pairs = (known, torch.from_numpy(tu).to(P.device), torch.from_numpy(ti).to(P.device))
-        known, tu, ti = self._test_pairs
-        scores = E.mf_predict_pairs(P, Q, tu, ti, Bu, Bi, gm).double().cpu().numpy()
-        res, pos = [], dict(zip(known, range(len(known))))
-        for k, (user, item, rating) in enumerate(self.data.testData):
-            pred = float(scores[pos[k]]) if k in pos else self.predictForRating(user, item)
-            res.append([user, item, rating, self.checkRatingBoundary(pred)])
-        self.measure = Measure.ratingMeasure(res)
-        return self.measure
