@@ -85,6 +85,3 @@ class DeepRecommender(IterativeRecommender):
             out = mt.sample_pointwise(csr, u_all[b:b + self.batch_size], i_all[b:b + self.batch_size])
             random.setstate(mt.getstate())
             yield out
-
-    def predictForRanking(self, u):
-        pass

@@ -75,6 +75,51 @@ class DeviceCSR(object):
                                rowsplit=self.rowsplit)
 
 
+def sorted_unique_padded(x):
+    """The distinct values of an int32 vector as a same-length vector: sorted, every repeat replaced by -1.  Unlike
+    torch.unique the length does not depend on the data, so nothing has to be read back by the host."""
+    import torch
+    s, _ = torch.sort(x)
+    s[1:] = torch.where(s[1:] == s[:-1], torch.full_like(s[1:], -1), s[1:])
+    return s.int().contiguous()
+
+
+def batch_rows(u, i, j, num_users, width):
+    """The rows of the joint (users; items) table a minibatch of triples touches, as sorted_unique_padded lists them:
+    the only rows its losses read and the only rows where their gradients are non-zero.  None when the batch (more than
+    8192 triples) or the row width (more than 128) is beyond the row-list kernels."""
+    import torch
+    if u.shape[0] > 8192 or width > 128:
+        return None
+    return sorted_unique_padded(torch.cat([u, i + num_users, j + num_users]))
+
+
+def layer_sum(mats, src, acc, scale, bufs, need=None, nz=None, with_src=True):
+    """acc <- scale * (src + A_1 src + A_2 A_1 src + ... + A_n ... A_1 src) for the n operators `mats` (DeviceCSR),
+    each layer accumulated in the SpMM epilogue; with_src=False leaves out the src term (acc is zeroed instead).
+    bufs: two tables the layers alternate between.  need: the only rows of acc the caller reads -- the last layer,
+    whose output feeds no further layer, is then evaluated on those rows alone (from two layers on; the other rows of
+    acc lack its term).  nz: the only non-zero rows of src -- the first layer then scatters along their edges.  Row
+    lists are sorted, distinct and -1-padded (batch_rows)."""
+    from .. import engine
+    if with_src:
+        engine.axpby(acc, src, src, scale, 0.0)
+    else:
+        acc.zero_()
+    cur, n = src, len(mats)
+    for k in range(n):
+        nxt = bufs[k % 2]
+        if need is not None and k == n - 1 and k > 0:
+            mats[k].matmul_rows(cur, need, acc=acc, acc_scale=scale)
+            break
+        if nz is not None and k == 0:
+            mats[k].matmul_sparse_rows(cur, nz, nxt, acc=acc, acc_scale=scale)
+        else:
+            mats[k].matmul(cur, nxt, acc=acc, acc_scale=scale)
+        cur = nxt
+    return acc
+
+
 class GraphRecommender(DeepRecommender):
     def __init__(self, conf, trainingSet, testSet, fold='[1]'):
         super(GraphRecommender, self).__init__(conf, trainingSet, testSet, fold)
@@ -114,3 +159,8 @@ class GraphRecommender(DeepRecommender):
 
     def create_sparse_adj_tensor(self):
         return DeviceCSR(self.create_sparse_rating_matrix(), self._device())
+
+    def _export_tables(self, users, items):
+        """(U, V) for ranking: propagated user and item rows on the host as float32, cut to emb_size columns."""
+        d = self.emb_size
+        return users[:, :d].cpu().numpy(), items[:, :d].cpu().numpy()

@@ -19,6 +19,8 @@ from ..util.qmath import find_k_largest
 
 
 class IterativeRecommender(Recommender):
+    score_tables = ('P', 'Q')          # the (user, item) tables with score(u, i) = U[u] . V[i]
+
     def __init__(self, conf, trainingSet, testSet, fold='[1]'):
         super(IterativeRecommender, self).__init__(conf, trainingSet, testSet, fold)
         self.bestPerformance = []
@@ -71,6 +73,25 @@ class IterativeRecommender(Recommender):
         padded[:, :d] = t
         return padded
 
+    def _tables_on_device(self):
+        """The score_tables pair as contiguous float32 CUDA tensors on `engine=-device N`: what device_tables returns
+        in the models that rank on the device."""
+        import torch
+        dev = torch.device('cuda', self.engine_device)
+        return tuple(torch.from_numpy(np.ascontiguousarray(getattr(self, name), dtype=np.float32)).to(dev)
+                     for name in self.score_tables)
+
+    def _rating_csr_on_device(self, by, dev, with_vals):
+        """The training ratings by 'user' or by 'item' (Rating.rating_csr) on `dev` for the ALS-family row solves:
+        (rowptr, cols, vals in the engine's dtype, als_row_order), without vals unless `with_vals`."""
+        import torch
+        from .. import engine as E
+        rowptr, cols, vals = self.data.rating_csr(by)
+        csr = (torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev))
+        if with_vals:
+            csr += (torch.from_numpy(vals).to(device=dev, dtype=self._engine_dtype()),)
+        return csr + (torch.from_numpy(E.als_row_order(rowptr)).to(dev),)
+
     def _host(self, t):
         """A device table as a float64 numpy array, without _upload's padding columns."""
         if t.dim() == 2:
@@ -108,7 +129,8 @@ class IterativeRecommender(Recommender):
 
     def predictForRanking(self, u):
         if self.data.containsUser(u):
-            return self.Q.dot(self.P[self.data.user[u]])
+            U, V = (getattr(self, name) for name in self.score_tables)
+            return V.dot(U[self.data.user[u]])
         return [self.data.globalMean] * self.num_items
 
     def shuffle_training_data(self):

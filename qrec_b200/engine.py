@@ -1262,20 +1262,26 @@ def als_row_order(rowptr):
     return np.argsort(-lengths, kind='stable').astype(np.int32)
 
 
+def als_gram_workspace(n_rows, d, device):
+    """The uint8 workspace als_gram needs for tables of up to n_rows rows of width d, to be reused across calls."""
+    torch = _torch()
+    need = int(lib.qrec_als_gram_workspace_bytes(n_rows, d))
+    if need < 0:
+        check(need, 'qrec_als_gram_workspace_bytes')
+    return torch.empty(max(need, 1), dtype=torch.uint8, device=device)
+
+
 def als_gram(Z, G=None, workspace=None):
     """G = Z^T Z as a float64 [d, d] CUDA tensor for a float32 / float64 table Z (bitwise reproducible).
-    workspace: optional uint8 CUDA tensor of at least qrec_als_gram_workspace_bytes(n, d) bytes, reused across calls."""
+    workspace: optional als_gram_workspace of at least Z's rows and width, reused across calls."""
     torch = _torch()
     n, d = Z.shape
     if Z.dtype not in (torch.float32, torch.float64):
         raise QRecError('Z must be float32 or float64, got %s' % Z.dtype)
-    need = int(lib.qrec_als_gram_workspace_bytes(n, d))
-    if need < 0:
-        check(need, 'qrec_als_gram_workspace_bytes')
     if G is None:
         G = torch.empty(d, d, dtype=torch.float64, device=Z.device)
     if workspace is None:
-        workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=Z.device)
+        workspace = als_gram_workspace(n, d, Z.device)
     fn, _ = _entry('qrec_als_gram', Z.dtype)
     check(fn(_dev(Z, Z.dtype, 'Z'), n, d, _dev(G, torch.float64, 'G'), _dev(workspace, torch.uint8, 'workspace'),
              workspace.numel(), _stream()), 'qrec_als_gram')

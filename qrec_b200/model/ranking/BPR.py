@@ -121,12 +121,4 @@ class BPR(IterativeRecommender):
         self.P, self.Q = np.ascontiguousarray(U[:, :d].cpu().numpy()), np.ascontiguousarray(V[:, :d].cpu().numpy())
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.P, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.Q, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        if self.data.containsUser(u):
-            return self.Q.dot(self.P[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

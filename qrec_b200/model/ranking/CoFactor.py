@@ -32,6 +32,7 @@ from ...util.config import OptionConf
 
 class CoFactor(IterativeRecommender):
     ALPHA = 10.0
+    score_tables = ('X', 'Y')
 
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(CoFactor, self).__init__(conf, trainingSet, testSet, fold)
@@ -53,24 +54,17 @@ class CoFactor(IterativeRecommender):
         print('filter: %d' % self.filter)
         print('=' * 80)
 
-    def _item_csr(self):
-        import torch
-        dev = self._device()
-        rowptr, cols, vals = self.data.rating_csr('item')
-        return torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev), torch.from_numpy(vals).to(dev)
-
     def initModel(self):
         super(CoFactor, self).initModel()
         from ... import engine as E
         print('Constructing SPPMI matrix...')
-        rowptr, cols, _ = self._item_csr()
+        rowptr, cols, _ = self._rating_csr_on_device('item', self._device(), False)
         self.sppmi = E.sppmi_csr(rowptr, cols, self.num_users, self.negCount, self.filter)
 
     def trainModel(self):
         import torch
         from ... import engine as E
         dev = self._device()
-        dtype = self._engine_dtype()
         self.X = self.P * 10
         self.Y = self.Q * 10
         self.w = np.random.rand(self.num_items) / 10
@@ -78,18 +72,12 @@ class CoFactor(IterativeRecommender):
         self.G = np.random.rand(self.num_items, self.emb_size) / 10
         print('training...')
         X, Y, G, w, c = (self._upload(a, dev) for a in (self.X, self.Y, self.G, self.w, self.c))
-        rowptr, cols, vals = self.data.rating_csr('user')
-        urp, ucol, uval = torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev), \
-            torch.from_numpy(vals).to(device=dev, dtype=dtype)
-        uord = torch.from_numpy(E.als_row_order(rowptr)).to(dev)
-        irp, icol, ival = self._item_csr()
-        item_csr = (irp, icol, ival.to(dtype))
+        urp, ucol, uval, uord = self._rating_csr_on_device('user', dev, True)
+        item_csr = self._rating_csr_on_device('item', dev, True)[:3]
         srp, scol, sval = self.sppmi
-        sppmi = (srp, scol, sval.to(dtype))
+        sppmi = (srp, scol, sval.to(self._engine_dtype()))
         gram = torch.empty(self.emb_size, self.emb_size, dtype=torch.float64, device=dev)
-        n_big = max(self.num_users, self.num_items)
-        ws = torch.empty(max(1, int(E.lib.qrec_als_gram_workspace_bytes(n_big, self.emb_size))), dtype=torch.uint8,
-                         device=dev)
+        ws = E.als_gram_workspace(max(self.num_users, self.num_items), self.emb_size, dev)
         loss = torch.zeros(1, dtype=torch.float64, device=dev)
         stamps = torch.zeros(self.num_items, dtype=torch.int32, device=dev)
         epoch = 0
@@ -108,13 +96,4 @@ class CoFactor(IterativeRecommender):
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.X, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.Y, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        """invoked to rank all the items for the user"""
-        if self.data.containsUser(u):
-            return self.Y.dot(self.X[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

@@ -30,6 +30,8 @@ from ...base.iterativeRecommender import IterativeRecommender
 
 
 class ExpoMF(IterativeRecommender):
+    score_tables = ('theta', 'beta')
+
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(ExpoMF, self).__init__(conf, trainingSet, testSet, fold)
 
@@ -54,13 +56,8 @@ class ExpoMF(IterativeRecommender):
         theta, beta, mu = (torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(dev)
                            for a in (self.theta, self.beta, self.mu))
         mu_next = torch.empty_like(mu)
-        csr = {}
-        for by in ('user', 'item'):
-            rowptr, cols, _ = self.data.rating_csr(by)
-            csr[by] = (torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev),
-                       torch.from_numpy(E.als_row_order(rowptr)).to(dev))
-        urp, ucol, uord = csr['user']
-        irp, icol, iord = csr['item']
+        urp, ucol, uord = self._rating_csr_on_device('user', dev, False)
+        irp, icol, iord = self._rating_csr_on_device('item', dev, False)
         item_mu_by_row = self.num_users != self.num_items       # ExpoMF.py, _solve_batch: mu.size == X.shape[0]
         for epoch in range(self.maxEpoch):
             print('epoch #%d' % epoch)
@@ -75,13 +72,4 @@ class ExpoMF(IterativeRecommender):
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.theta)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.beta)).to(dev))
-
-    def predictForRanking(self, u):
-        """invoked to rank all the items for the user"""
-        if self.data.containsUser(u):
-            return self.beta.dot(self.theta[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

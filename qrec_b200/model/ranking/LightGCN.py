@@ -8,14 +8,14 @@ for EVERY minibatch (LightGCN.py:35-39: one sess.run per batch).  The same compu
   backward  dE0 = 1/(n+1) * sum_k A^k G            (A symmetric: the same K2 kernel)
   update    TF1 dense Adam on the ego table        (K4)
 """
-import numpy as np
-
-from ...base.graphRecommender import GraphRecommender
+from ...base.graphRecommender import GraphRecommender, batch_rows, layer_sum
 from ...util.config import OptionConf
 from ...util.loss import BPR_EPS
 
 
 class LightGCN(GraphRecommender):
+    score_tables = ('U', 'V')
+
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(LightGCN, self).__init__(conf, trainingSet, testSet, fold)
         args = OptionConf(self.config['LightGCN'])
@@ -44,45 +44,21 @@ class LightGCN(GraphRecommender):
         """mean(E0..En) into self._mean; returns (user rows, item rows) views (LightGCN.py:13-20).
         rows (int32, distinct, -1 padded): the only rows the caller will read -- the last layer, whose output feeds
         no further layer, is then evaluated on those rows alone (the other rows of the mean lack its term)."""
-        from ... import engine as E
-        s = 1.0 / (self.n_layers + 1)
-        E.axpby(self._mean, self.ego, self.ego, s, 0.0)
-        cur = self.ego
-        for k in range(self.n_layers):
-            nxt = self._buf[k % 2]
-            if rows is not None and k == self.n_layers - 1 and k > 0 and hasattr(self.norm_adj, 'matmul_rows'):
-                self.norm_adj.matmul_rows(cur, rows, acc=self._mean, acc_scale=s)
-                break
-            self.norm_adj.matmul(cur, nxt, acc=self._mean, acc_scale=s)
-            cur = nxt
+        layer_sum([self.norm_adj] * self.n_layers, self.ego, self._mean, 1.0 / (self.n_layers + 1), self._buf, need=rows)
         return self._mean[:self.num_users], self._mean[self.num_users:]
 
     def train_step(self, u, i, j):
         """One minibatch (LightGCN.py:28-39).  u,i,j: int32 CUDA tensors.  Returns the device loss."""
         from ... import engine as E
-        s = 1.0 / (self.n_layers + 1)
-        # the rows the batch touches: the loss reads the propagated embeddings there and nowhere else, and its
-        # gradient is zero everywhere else (sorted, repeats replaced by -1: no data-dependent length, no host sync)
-        batch_rows = None
-        if u.shape[0] <= 8192 and self.emb_pad <= 128 and hasattr(self.norm_adj, 'matmul_sparse_rows'):
-            from ...parallel import _sorted_unique_padded
-            import torch
-            batch_rows = _sorted_unique_padded(torch.cat([u, i + self.num_users, j + self.num_users]))
-        Ue, Ve = self.propagate(batch_rows)
+        # listed at every depth: even at one layer the backward pass scatters from the batch's rows
+        rows = batch_rows(u, i, j, self.num_users, self.emb_pad)
+        Ue, Ve = self.propagate(rows)
         self._grad.zero_()
         self._loss.zero_()
         E.bpr_grad_scatter(Ue, Ve, u, i, j, BPR_EPS, self.regU, self._grad[:self.num_users],
                            self._grad[self.num_users:], self._loss)
-        E.axpby(self._total, self._grad, self._grad, s, 0.0)
-        cur = self._grad
-        for k in range(self.n_layers):
-            nxt = self._buf[k % 2]
-            if k == 0 and batch_rows is not None:
-                # the loss gradient is non-zero only in the batch's rows: scatter along their edges
-                self.norm_adj.matmul_sparse_rows(cur, batch_rows, nxt, acc=self._total, acc_scale=s)
-            else:
-                self.norm_adj.matmul(cur, nxt, acc=self._total, acc_scale=s)
-            cur = nxt
+        # dE0 = 1/(n+1) sum_k A^k G (A symmetric); G is non-zero only in the batch's rows
+        layer_sum([self.norm_adj] * self.n_layers, self._grad, self._total, 1.0 / (self.n_layers + 1), self._buf, nz=rows)
         self._step += 1
         E.adam_dense_tf1(self.ego, self._adam_m, self._adam_v, self._total, self.lRate, self._step)
         return self._loss
@@ -95,19 +71,9 @@ class LightGCN(GraphRecommender):
                                        torch.from_numpy(j).to(self.device))
                 if n % 20 == 0:      # the reference prints every batch; rate-limited here
                     print(self.foldInfo, 'training:', epoch + 1, 'batch', n, 'loss:', float(loss.item()))
-        Ue, Ve = self.propagate()
-        d = self.emb_size
-        self.U, self.V = Ue[:, :d].cpu().numpy(), Ve[:, :d].cpu().numpy()
+        self.U, self.V = self._export_tables(*self.propagate())
 
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.U, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.V, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        if self.data.containsUser(u):
-            return self.V.dot(self.U[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

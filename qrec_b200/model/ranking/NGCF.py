@@ -11,8 +11,6 @@ by hand (checked against torch autograd in tests/test_gpu_models.py) and reuses 
 """
 import math
 
-import numpy as np
-
 from ...base.graphRecommender import GraphRecommender
 from ...util.loss import BPR_EPS
 
@@ -20,6 +18,8 @@ KEEP_PROB = 0.9           # NGCF.py:37
 
 
 class NGCF(GraphRecommender):
+    score_tables = ('U', 'V')
+
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(NGCF, self).__init__(conf, trainingSet, testSet, fold)
 
@@ -122,12 +122,4 @@ class NGCF(GraphRecommender):
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.U, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.V, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        if self.data.containsUser(u):
-            return self.V.dot(self.U[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

@@ -161,9 +161,3 @@ class SBPR(SocialRecommender):
                     print('training:', epoch + 1, 'batch', n, 'loss:', float(loss.item()))
         self.P = np.ascontiguousarray(U[:, :d].cpu().numpy())
         self.Q = np.ascontiguousarray(V[:, :d].cpu().numpy())
-
-    def predictForRanking(self, u):
-        'invoked to rank all the items for the user'
-        if self.data.containsUser(u):
-            return self.Q.dot(self.P[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items

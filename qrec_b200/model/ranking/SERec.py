@@ -73,6 +73,8 @@ def mu_text(A, deg, n_items, **kw):
 
 
 class SERec(SocialRecommender):
+    score_tables = ('theta', 'beta')
+
     def __init__(self, conf, trainingSet=None, testSet=None, relation=None, fold='[1]'):
         super(SERec, self).__init__(conf, trainingSet, testSet, relation, fold)
 
@@ -107,13 +109,8 @@ class SERec(SocialRecommender):
                        for a in (self.theta, self.beta))
         deg = torch.from_numpy(self.deg).to(dev)
         asum, asum_next = None, torch.empty(self.num_items, dtype=torch.float64, device=dev)
-        csr = {}
-        for by in ('user', 'item'):
-            rowptr, cols, _ = self.data.rating_csr(by)
-            csr[by] = (torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev),
-                       torch.from_numpy(E.als_row_order(rowptr)).to(dev))
-        urp, ucol, uord = csr['user']
-        irp, icol, iord = csr['item']
+        urp, ucol, uord = self._rating_csr_on_device('user', dev, False)
+        irp, icol, iord = self._rating_csr_on_device('item', dev, False)
         item_rows_are_users = self.num_users == self.num_items      # SERec.py, _solve_batch: mu.shape[1] == X.shape[0]
         kw = dict(mu0=self.init_mu, a=self.a, b=self.b, s=self.s)
         for epoch in range(self.maxEpoch):
@@ -133,13 +130,4 @@ class SERec(SocialRecommender):
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.theta)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.beta)).to(dev))
-
-    def predictForRanking(self, u):
-        """invoked to rank all the items for the user"""
-        if self.data.containsUser(u):
-            return self.beta.dot(self.theta[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

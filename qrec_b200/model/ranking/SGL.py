@@ -16,14 +16,14 @@ dropout per layer) and feeds them as SparseTensors; per minibatch it runs three 
   backward   each encoder is linear in E_0: d/dE_0 = 1/(n+1) (G + A_1 (G + A_2 (... + A_n G))) per view (Horner)
   update     TF1 dense Adam (K4) on the ego table
 """
-import numpy as np
-
-from ...base.graphRecommender import GraphRecommender, DeviceCSR
+from ...base.graphRecommender import GraphRecommender, DeviceCSR, batch_rows, layer_sum
 from ...util.config import OptionConf
-from ...util.loss import BPR_EPS
+from ...util.loss import BPR_EPS, infonce_step
 
 
 class SGL(GraphRecommender):
+    score_tables = ('U', 'V')
+
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(SGL, self).__init__(conf, trainingSet, testSet, fold)
 
@@ -90,18 +90,7 @@ class SGL(GraphRecommender):
         """out <- mean(E_0, A_1 E_0, A_2 A_1 E_0, ...) (SGL.py:56-76).
         rows (int32, distinct, -1 padded): the only rows of `out` the caller reads -- the last layer is then
         evaluated on those rows alone (the other rows of `out` lack its term)."""
-        from ... import engine as E
-        s = 1.0 / (self.n_layers + 1)
-        E.axpby(out, self.ego, self.ego, s, 0.0)
-        cur = self.ego
-        for k in range(self.n_layers):
-            nxt = self._buf[k % 2]
-            if rows is not None and k == self.n_layers - 1 and k > 0:
-                mats[k].matmul_rows(cur, rows, acc=out, acc_scale=s)
-                break
-            mats[k].matmul(cur, nxt, acc=out, acc_scale=s)
-            cur = nxt
-        return out
+        return layer_sum(mats, self.ego, out, 1.0 / (self.n_layers + 1), self._buf, need=rows)
 
     def _backprop(self, mats, G, rows=None):
         """self._total += 1/(n+1) (G + A_1 (G + A_2 (... + A_n G))): the encoder's transpose (A symmetric).
@@ -127,11 +116,8 @@ class SGL(GraphRecommender):
         main_mats = [self.norm_adj] * self.n_layers
         self._step += 1
         # the rows the batch touches: all the losses read of the encoders' outputs, and the only rows where their
-        # gradients are non-zero (sorted, repeats replaced by -1: no data-dependent length)
-        rows = None
-        if u.shape[0] <= 8192 and d <= 128 and self.n_layers > 1:
-            from ...parallel import _sorted_unique_padded
-            rows = _sorted_unique_padded(torch.cat([u, i + nu, j + nu]))
+        # gradients are non-zero; listed from two layers on
+        rows = batch_rows(u, i, j, nu, d) if self.n_layers > 1 else None
         m0 = self.encode(main_mats, self._mean[0], rows)
         m1 = self.encode(self.views[0], self._mean[1], rows)
         m2 = self.encode(self.views[1], self._mean[2], rows)
@@ -141,19 +127,7 @@ class SGL(GraphRecommender):
         E.bpr_grad_scatter(m0[:nu], m0[nu:], u, i, j, BPR_EPS, self.regU, self._grad[0][:nu], self._grad[0][nu:], self._loss[0:1])
         # calc_ssl_loss_v3: users and items of the batch in ONE InfoNCE (SGL.py:206-230)
         idx = torch.cat([torch.unique(u), torch.unique(i) + nu]).int().contiguous()
-        b, dev = idx.shape[0], self.device
-        Z1, Z2 = torch.empty(b, d, device=dev), torch.empty(b, d, device=dev)
-        n1, n2 = torch.empty(b, device=dev), torch.empty(b, device=dev)
-        E.gather_normalize(m1, idx, Z1, n1)
-        E.gather_normalize(m2, idx, Z2, n2)
-        S = torch.empty(b, b, device=dev)
-        E.sgemm(Z1, Z2, S, trans_b=True)
-        E.infonce_rows(S, self.ssl_temp, self._loss[1:2])            # S <- dLoss/dS
-        dZ1, dZ2 = torch.empty(b, d, device=dev), torch.empty(b, d, device=dev)
-        E.sgemm(S, Z2, dZ1)
-        E.sgemm(S, Z1, dZ2, trans_a=True)
-        E.normalize_bwd_scatter(dZ1, Z1, n1, idx, self.ssl_reg, self._grad[1])
-        E.normalize_bwd_scatter(dZ2, Z2, n2, idx, self.ssl_reg, self._grad[2])
+        infonce_step(m1, m2, idx, self.ssl_temp, self.ssl_reg, self._loss[1:2], self._grad[1], self._grad[2])
         self._total.zero_()
         self._backprop(main_mats, self._grad[0], rows)
         self._backprop(self.views[0], self._grad[1], rows)
@@ -167,8 +141,7 @@ class SGL(GraphRecommender):
 
     def saveModel(self):
         m0 = self.encode([self.norm_adj] * self.n_layers, self._mean[0])
-        d = self.emb_size
-        self.bestU, self.bestV = m0[:self.num_users, :d].cpu().numpy(), m0[self.num_users:, :d].cpu().numpy()
+        self.bestU, self.bestV = self._export_tables(m0[:self.num_users], m0[self.num_users:])
 
     def trainModel(self):
         import torch
@@ -180,20 +153,11 @@ class SGL(GraphRecommender):
                     rec, ssl = self.losses()
                     print('training:', epoch + 1, 'batch', n, 'rec_loss:', rec, 'ssl_loss', ssl)
             m0 = self.encode([self.norm_adj] * self.n_layers, self._mean[0])
-            self.U = m0[:self.num_users, :self.emb_size].cpu().numpy()
-            self.V = m0[self.num_users:, :self.emb_size].cpu().numpy()
+            self.U, self.V = self._export_tables(m0[:self.num_users], m0[self.num_users:])
             self.ranking_performance(epoch)
         self.U, self.V = self.bestU, self.bestV
 
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.U, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.V, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        if self.data.containsUser(u):
-            return self.V.dot(self.U[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

@@ -14,16 +14,16 @@ Adam step (SimGCL.py:22-38, 60-111).  Here:
 """
 import math
 
-import numpy as np
-
-from ...base.graphRecommender import GraphRecommender
+from ...base.graphRecommender import GraphRecommender, batch_rows, layer_sum
 from ...util.config import OptionConf
-from ...util.loss import BPR_EPS
+from ...util.loss import BPR_EPS, infonce_step
 
 TAU = 0.2                      # the literal in SimGCL.py:72-75
 
 
 class SimGCL(GraphRecommender):
+    score_tables = ('U', 'V')
+
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(SimGCL, self).__init__(conf, trainingSet, testSet, fold)
 
@@ -72,25 +72,22 @@ class SimGCL(GraphRecommender):
         noise) is then evaluated on those rows alone; the other rows of `out` lack its term."""
         from ... import engine as E
         s = 1.0 / self.n_layers
+        if not perturbed:
+            layer_sum([self.norm_adj] * self.n_layers, self.ego, out, s, self._buf, need=rows, with_src=False)
+            return out[:self.num_users], out[self.num_users:]
         out.zero_()
         cur = self.ego
         for k in range(self.n_layers):
             nxt = self._buf[k % 2]
             if rows is not None and k == self.n_layers - 1 and k > 0:
-                if perturbed:
-                    part = self._rows_block(rows.shape[0])
-                    self.norm_adj.matmul_rows(cur, rows, out=part, compact=True)
-                    E.simgcl_perturb_listed(part, rows, self.eps, self.noise_seed, perturbed * 16 + k, self._step, acc=out,
-                                            acc_scale=s, d_valid=self.emb_size)
-                else:
-                    self.norm_adj.matmul_rows(cur, rows, acc=out, acc_scale=s)
+                part = self._rows_block(rows.shape[0])
+                self.norm_adj.matmul_rows(cur, rows, out=part, compact=True)
+                E.simgcl_perturb_listed(part, rows, self.eps, self.noise_seed, perturbed * 16 + k, self._step, acc=out,
+                                        acc_scale=s, d_valid=self.emb_size)
                 break
-            if perturbed:
-                self.norm_adj.matmul(cur, nxt)
-                E.simgcl_perturb(nxt, self.eps, self.noise_seed, perturbed * 16 + k, self._step, acc=out, acc_scale=s,
-                                 d_valid=self.emb_size)
-            else:
-                self.norm_adj.matmul(cur, nxt, acc=out, acc_scale=s)
+            self.norm_adj.matmul(cur, nxt)
+            E.simgcl_perturb(nxt, self.eps, self.noise_seed, perturbed * 16 + k, self._step, acc=out, acc_scale=s,
+                             d_valid=self.emb_size)
             cur = nxt
         return out[:self.num_users], out[self.num_users:]
 
@@ -100,24 +97,6 @@ class SimGCL(GraphRecommender):
             self._rows_buf = torch.empty(n, self.emb_pad, device=self.device)
         return self._rows_buf[:n]
 
-    def _infonce(self, tab1, tab2, idx, grad_rows):
-        import torch
-        from ... import engine as E
-        b, d = idx.shape[0], self.emb_pad
-        dev = self.device
-        Z1, Z2 = torch.empty(b, d, device=dev), torch.empty(b, d, device=dev)
-        n1, n2 = torch.empty(b, device=dev), torch.empty(b, device=dev)
-        E.gather_normalize(tab1, idx, Z1, n1)
-        E.gather_normalize(tab2, idx, Z2, n2)
-        S = torch.empty(b, b, device=dev)
-        E.sgemm(Z1, Z2, S, trans_b=True)
-        E.infonce_rows(S, TAU, self._loss[1:2])                 # S <- dLoss/dS
-        dZ1, dZ2 = torch.empty(b, d, device=dev), torch.empty(b, d, device=dev)
-        E.sgemm(S, Z2, dZ1)
-        E.sgemm(S, Z1, dZ2, trans_a=True)
-        E.normalize_bwd_scatter(dZ1, Z1, n1, idx, self.cl_rate, grad_rows)
-        E.normalize_bwd_scatter(dZ2, Z2, n2, idx, self.cl_rate, grad_rows)
-
     def train_step(self, u, i, j):
         """One minibatch (SimGCL.py:92-108).  Returns (total, rec, cl) losses as floats lazily:
         the device tensor self._loss holds [rec, cl_unscaled]."""
@@ -126,11 +105,8 @@ class SimGCL(GraphRecommender):
         nu = self.num_users
         self._step += 1
         # the rows the batch touches: every loss term reads the encoders' outputs there and nowhere else, and the
-        # summed loss gradient is zero everywhere else (sorted, repeats replaced by -1: no data-dependent length)
-        rows = None
-        if u.shape[0] <= 8192 and self.emb_pad <= 128 and self.n_layers > 1 and hasattr(self.norm_adj, 'matmul_rows'):
-            from ...parallel import _sorted_unique_padded
-            rows = _sorted_unique_padded(torch.cat([u, i + nu, j + nu]))
+        # summed loss gradient is zero everywhere else; listed from two layers on
+        rows = batch_rows(u, i, j, nu, self.emb_pad) if self.n_layers > 1 else None
         mU, mV = self.encode(self._main, 0, rows)
         p1U, p1V = self.encode(self._pert[0], 1, rows)
         p2U, p2V = self.encode(self._pert[1], 2, rows)
@@ -139,19 +115,11 @@ class SimGCL(GraphRecommender):
         E.bpr_grad_scatter(mU, mV, u, i, j, BPR_EPS, self.regU, self._grad[:nu], self._grad[nu:], self._loss[0:1])
         uu = torch.unique(u).int()                                # tf.unique (order is irrelevant to the sums)
         ii = torch.unique(i).int()
-        self._infonce(p1U, p2U, uu, self._grad[:nu])
-        self._infonce(p1V, p2V, ii, self._grad[nu:])
+        infonce_step(p1U, p2U, uu, TAU, self.cl_rate, self._loss[1:2], self._grad[:nu], self._grad[:nu])
+        infonce_step(p1V, p2V, ii, TAU, self.cl_rate, self._loss[1:2], self._grad[nu:], self._grad[nu:])
         # backward through the encoders: total = 1/n * sum_{k=1..n} A^k G
-        self._total.zero_()
-        cur = self._grad
-        for k in range(self.n_layers):
-            nxt = self._buf[k % 2]
-            if k == 0 and rows is not None:
-                # the gradient is non-zero only in the batch's rows: scatter along their edges
-                self.norm_adj.matmul_sparse_rows(cur, rows, nxt, acc=self._total, acc_scale=1.0 / self.n_layers)
-            else:
-                self.norm_adj.matmul(cur, nxt, acc=self._total, acc_scale=1.0 / self.n_layers)
-            cur = nxt
+        layer_sum([self.norm_adj] * self.n_layers, self._grad, self._total, 1.0 / self.n_layers, self._buf, nz=rows,
+                  with_src=False)
         E.adam_dense_tf1(self.ego, self._adam_m, self._adam_v, self._total, self.lRate, self._step)
         return self._loss
 
@@ -161,9 +129,7 @@ class SimGCL(GraphRecommender):
         return rec + cl, rec, cl
 
     def saveModel(self):
-        mU, mV = self.encode(self._main, 0)
-        d = self.emb_size
-        self.bestU, self.bestV = mU[:, :d].cpu().numpy(), mV[:, :d].cpu().numpy()
+        self.bestU, self.bestV = self._export_tables(*self.encode(self._main, 0))
 
     def trainModel(self):
         import torch
@@ -173,20 +139,11 @@ class SimGCL(GraphRecommender):
                 if n % 20 == 0:
                     total, rec, cl = self.losses()
                     print('training:', epoch + 1, 'batch', n, 'total_loss:', total, 'rec_loss:', rec, 'cl_loss', cl)
-            mU, mV = self.encode(self._main, 0)
-            self.U, self.V = mU[:, :self.emb_size].cpu().numpy(), mV[:, :self.emb_size].cpu().numpy()
+            self.U, self.V = self._export_tables(*self.encode(self._main, 0))
             self.ranking_performance(epoch)
         self.U, self.V = self.bestU, self.bestV
 
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.U, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.V, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        if self.data.containsUser(u):
-            return self.V.dot(self.U[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

@@ -249,8 +249,3 @@ class TBPR(SocialRecommender):
         q -= self.lRate * self.regI * q
 
     buildModel = trainModel
-
-    def predictForRanking(self, u):
-        if self.data.containsUser(u):
-            return self.Q.dot(self.P[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items

@@ -16,13 +16,12 @@ Reference behaviour kept as is:
     (WRMF.py:37-38,63); the item side adds nothing to it.
   * X = 10*P, Y = 10*Q from the usual initModel draws (WRMF.py:12-15).
 """
-import numpy as np
-
 from ...base.iterativeRecommender import IterativeRecommender
 
 
 class WRMF(IterativeRecommender):
     ALPHA = 10.0
+    score_tables = ('X', 'Y')          # WRMF.py:69-75
 
     def __init__(self, conf, trainingSet=None, testSet=None, fold='[1]'):
         super(WRMF, self).__init__(conf, trainingSet, testSet, fold)
@@ -37,18 +36,10 @@ class WRMF(IterativeRecommender):
         from ... import engine as E
         print('training...')
         dev = self._device()
-        dtype = self._engine_dtype()
         X, Y = self._upload(self.X, dev), self._upload(self.Y, dev)
-        sides = []
-        for by in ('user', 'item'):
-            rowptr, cols, vals = self.data.rating_csr(by)
-            sides.append((torch.from_numpy(rowptr).to(dev), torch.from_numpy(cols).to(dev),
-                          torch.from_numpy(vals).to(device=dev, dtype=dtype),
-                          torch.from_numpy(E.als_row_order(rowptr)).to(dev)))
+        sides = [self._rating_csr_on_device(by, dev, True) for by in ('user', 'item')]
         G = torch.empty(self.emb_size, self.emb_size, dtype=torch.float64, device=dev)
-        n_big = max(self.num_users, self.num_items)
-        ws = torch.empty(max(1, int(E.lib.qrec_als_gram_workspace_bytes(n_big, self.emb_size))), dtype=torch.uint8,
-                         device=dev)
+        ws = E.als_gram_workspace(max(self.num_users, self.num_items), self.emb_size, dev)
         loss = torch.zeros(1, dtype=torch.float64, device=dev)
         epoch = 0
         while epoch < self.maxEpoch:
@@ -69,13 +60,4 @@ class WRMF(IterativeRecommender):
     buildModel = trainModel
 
     def device_tables(self):
-        import torch
-        dev = torch.device('cuda', self.engine_device)
-        return (torch.from_numpy(np.ascontiguousarray(self.X, dtype=np.float32)).to(dev),
-                torch.from_numpy(np.ascontiguousarray(self.Y, dtype=np.float32)).to(dev))
-
-    def predictForRanking(self, u):
-        """WRMF.py:69-75"""
-        if self.data.containsUser(u):
-            return self.Y.dot(self.X[self.data.getUserId(u)])
-        return [self.data.globalMean] * self.num_items
+        return self._tables_on_device()

@@ -13,6 +13,8 @@ Parity mode is a serial dependency chain and does not shard (replicas only).
 import torch
 import torch.distributed as dist
 
+from .base.graphRecommender import batch_rows, layer_sum, sorted_unique_padded
+
 
 def user_range(rank, world, num_users):
     """Contiguous, balanced user range of `rank`: sizes differ by at most one."""
@@ -508,14 +510,6 @@ def blocked_spmm(spmm, blocks, X, Y, scratch, acc, s):
         acc.add_(Y, alpha=s)
 
 
-def _sorted_unique_padded(x):
-    """The distinct values of an int32 vector as a same-length vector: sorted, every repeat replaced by -1.  Unlike
-    torch.unique the length does not depend on the data, so nothing has to be read back by the host."""
-    s, _ = torch.sort(x)
-    s[1:] = torch.where(s[1:] == s[:-1], torch.full_like(s[1:], -1), s[1:])
-    return s.int().contiguous()
-
-
 class UserShardedLightGCN(object):
     """LightGCN minibatch step (model/ranking/LightGCN.py:13-39 semantics) with the USER rows of the ego
     table partitioned over the ranks and the (25.6 MB at the benchmark scale) ITEM rows replicated.
@@ -652,9 +646,9 @@ class UserShardedLightGCN(object):
         nloc = self.Eu.shape[0]
         lu = u - self.lo
         lu = torch.where((lu >= 0) & (lu < nloc), lu, torch.full_like(lu, -1)).contiguous()
-        batch_rows = u.shape[0] <= 8192 and self._scatter is not None and self.Eu.shape[1] <= 128
-        rows_u = _sorted_unique_padded(lu) if batch_rows else None
-        rows_i = _sorted_unique_padded(torch.cat([i, j])) if batch_rows else None
+        listed = u.shape[0] <= 8192 and self._scatter is not None and self.Eu.shape[1] <= 128
+        rows_u = sorted_unique_padded(lu) if listed else None
+        rows_i = sorted_unique_padded(torch.cat([i, j])) if listed else None
         self._propagate(self.Eu, self.Ei, self.mean_u, self.mean_i, need_u=rows_u, need_i=rows_i)
         self.gu.zero_(); self.gi.zero_(); self.loss.zero_()
         self._grad(self.mean_u, self.mean_i, lu, i, j, self.gu, self.gi, self.loss)
@@ -806,28 +800,13 @@ class ColumnShardedLightGCN(object):
 
     def _propagate(self, src, acc, need=None, nz=None):
         """acc <- s * sum_{k=0..n} A^k src on this rank's columns; need / nz: row lists of the restricted layers."""
-        E, s = self.E, 1.0 / (self.n_layers + 1)
-        E.axpby(acc, src, src, s, 0.0)
-        cur = src
-        for k in range(self.n_layers):
-            nxt = self.buf[k % 2]
-            if need is not None and k == self.n_layers - 1 and k > 0:
-                self.adj.matmul_rows(cur, need, acc=acc, acc_scale=s)
-                break
-            if nz is not None and k == 0:
-                self.adj.matmul_sparse_rows(cur, nz, nxt, acc=acc, acc_scale=s)
-            else:
-                self.adj.matmul(cur, nxt, acc=acc, acc_scale=s)
-            cur = nxt
-        return acc
+        return layer_sum([self.adj] * self.n_layers, src, acc, 1.0 / (self.n_layers + 1), self.buf, need=need, nz=nz)
 
     def train_step(self, u, i, j):
         """u, i, j: the WHOLE minibatch (global ids, int32 device tensors), identical on every rank."""
         E, nu = self.E, self.nu
         B = u.shape[0]
-        rows = None
-        if B <= 8192 and self.ego.shape[1] <= 128 and hasattr(self.adj, 'matmul_rows'):
-            rows = _sorted_unique_padded(torch.cat([u, i + nu, j + nu]))
+        rows = batch_rows(u, i, j, nu, self.ego.shape[1])
         self._propagate(self.ego, self.mean, need=rows)
         if B not in self._y:
             self._y[B] = torch.empty(B, dtype=torch.float32, device=self.ego.device)
@@ -1032,7 +1011,7 @@ class UserShardedSimGCL(UserShardedLightGCN):
         if u.shape[0] <= 8192 and self.Eu.shape[1] <= 128 and self.n_layers > 1 and self._rows is not None:
             lu_all = u - self.lo
             lu_all = torch.where((lu_all >= 0) & (lu_all < nloc), lu_all, torch.full_like(lu_all, -1))
-            rows_u, rows_i = _sorted_unique_padded(lu_all), _sorted_unique_padded(torch.cat([i, j]))
+            rows_u, rows_i = sorted_unique_padded(lu_all), sorted_unique_padded(torch.cat([i, j]))
         self._encode(self.mean_u, self.mean_i, 0, rows_u, rows_i)
         self._encode(self.p_u[0], self.p_i[0], 1, rows_u, rows_i)
         self._encode(self.p_u[1], self.p_i[1], 2, rows_u, rows_i)

@@ -1,4 +1,5 @@
-"""bpr_loss of the reference (util/loss.py:3-6), executed by the engine.
+"""bpr_loss of the reference (util/loss.py:3-6), executed by the engine, and the InfoNCE step of the contrastive
+graph models.
 
 The reference builds a TF graph node; here the same quantity -- and its gradient, which is what
 training actually needs -- comes from the fused K3 kernel (qrec_bpr_grad_scatter_f32)."""
@@ -17,3 +18,22 @@ def bpr_loss(user_table, item_table, u_idx, pos_idx, neg_idx, reg=0.0, grad_user
     gV = grad_item if grad_item is not None else torch.zeros_like(item_table)
     engine.bpr_grad_scatter(user_table, item_table, u_idx, pos_idx, neg_idx, BPR_EPS, reg, gU, gV, loss)
     return loss
+
+
+def infonce_step(tab1, tab2, idx, tau, scale, loss, grad1, grad2):
+    """InfoNCE between two views on their rows `idx` (SGL.py:206-230, SimGCL.py:60-78): with z1, z2 the l2-normalised
+    rows, loss += sum_r logsumexp_c(z1_r . z2_c / tau) - z1_r . z2_r / tau, and scale times its gradient w.r.t. tab1 /
+    tab2 is scatter-added into grad1 / grad2 (which may be the same buffer)."""
+    b, d, dev = idx.shape[0], tab1.shape[1], tab1.device
+    Z1, Z2 = torch.empty(b, d, device=dev), torch.empty(b, d, device=dev)
+    n1, n2 = torch.empty(b, device=dev), torch.empty(b, device=dev)
+    engine.gather_normalize(tab1, idx, Z1, n1)
+    engine.gather_normalize(tab2, idx, Z2, n2)
+    S = torch.empty(b, b, device=dev)
+    engine.sgemm(Z1, Z2, S, trans_b=True)
+    engine.infonce_rows(S, tau, loss)                       # S <- dLoss/dS
+    dZ1, dZ2 = torch.empty(b, d, device=dev), torch.empty(b, d, device=dev)
+    engine.sgemm(S, Z2, dZ1)
+    engine.sgemm(S, Z1, dZ2, trans_a=True)
+    engine.normalize_bwd_scatter(dZ1, Z1, n1, idx, scale, grad1)
+    engine.normalize_bwd_scatter(dZ2, Z2, n2, idx, scale, grad2)

@@ -121,7 +121,7 @@ def spmm_case(launcher, d, structure):
         acc0 = rng.standard_normal((n_rows, d)).astype(np.float32)
     rows = None
     if launcher in ('spmm_scatter_rows', 'spmm_rows'):
-        # distinct rows, sorted, every fifth slot -1 padding (parallel._sorted_unique_padded's output has that form)
+        # distinct rows, sorted, every fifth slot -1 padding (graphRecommender.sorted_unique_padded's output has that form)
         listed = np.sort(rng.choice(n_rows, n_rows * 3 // 4 if structure == 'tails' else n_rows - 40, replace=False))
         if structure == 'long':
             listed = np.union1d(listed, np.nonzero(lengths > CHUNK)[0])

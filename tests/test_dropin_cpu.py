@@ -159,6 +159,20 @@ def test_device_csr_constructors_agree():
     assert DeviceCSR(long_row, 'cpu').rowsplit is False
 
 
+def test_sorted_unique_padded_is_a_fixed_length_unique():
+    """graphRecommender.sorted_unique_padded: the distinct values, sorted, repeats replaced by -1 -- same multiset of
+    non-negative values as torch.unique, length independent of the data (no host synchronisation in the step)."""
+    import torch
+    from qrec_b200.base.graphRecommender import sorted_unique_padded
+    g = torch.Generator().manual_seed(0)
+    for n, hi in ((1, 5), (50, 7), (4096, 100000), (300, 3)):
+        x = torch.randint(-1, hi, (n,), generator=g, dtype=torch.int32)
+        s = sorted_unique_padded(x)
+        assert s.shape == x.shape and s.dtype == torch.int32
+        kept = s[s >= 0]
+        assert torch.equal(kept, torch.unique(x[x >= 0]).int())
+
+
 def test_graph_recommender_adj_tensor_method_on_cpu_tensors(golden_graph, tmp_path, monkeypatch):
     """GraphRecommender.create_joint_sparse_adj_tensor end to end with the device stubbed to 'cpu':
     the DeviceCSR it returns holds the reference's matrix."""

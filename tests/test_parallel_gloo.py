@@ -745,15 +745,3 @@ def test_user_sharded_neumf_matches_autograd_world2():
     out = mgr.dict()
     mp.spawn(_neumf_worker, args=(2, port, out), nprocs=2, join=True)
     assert dict(out) == {0: 1, 1: 1}
-
-
-def test_sorted_unique_padded_is_a_fixed_length_unique():
-    """parallel._sorted_unique_padded: the distinct values, sorted, repeats replaced by -1 -- same multiset of
-    non-negative values as torch.unique, length independent of the data (no host synchronisation in the step)."""
-    g = torch.Generator().manual_seed(0)
-    for n, hi in ((1, 5), (50, 7), (4096, 100000), (300, 3)):
-        x = torch.randint(-1, hi, (n,), generator=g, dtype=torch.int32)
-        s = parallel._sorted_unique_padded(x)
-        assert s.shape == x.shape and s.dtype == torch.int32
-        kept = s[s >= 0]
-        assert torch.equal(kept, torch.unique(x[x >= 0]).int())

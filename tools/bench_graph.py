@@ -65,22 +65,17 @@ def main():
     if args.spmm_only:
         return
     # full LightGCN steps through the drop-in class's step function
+    from qrec_b200.base.graphRecommender import DeviceCSR
     from qrec_b200.model.ranking.LightGCN import LightGCN
 
     class Shell(LightGCN):            # engine state only; no Rating object needed for the step
         def __init__(self):
             pass
     m = Shell()
-    m.num_users, m.num_items, m.emb_size, m.n_layers = U, I, D, args.layers
+    m.num_users, m.num_items, m.emb_size, m.emb_pad, m.n_layers = U, I, D, D, args.layers
     m.lRate, m.regU, m.device = 0.001, 0.001, dev
-
-    class Adj(object):
-        def matmul(self, Xin, out, acc=None, acc_scale=0.0):
-            return E.spmm_csr(rowptr, cols, vals, Xin, out, acc=acc, acc_scale=acc_scale, rowsplit=not args.zipf)
-
-        def matmul_sparse_rows(self, Xin, src_rows, out, acc=None, acc_scale=0.0):
-            return E.spmm_csr_scatter_rows(rowptr, cols, vals, src_rows, Xin, out, acc=acc, acc_scale=acc_scale)
-    m.norm_adj = Adj()
+    m.norm_adj = DeviceCSR.from_tensors((N, N), rowptr, cols, vals)
+    m.norm_adj.rowsplit = not args.zipf
     m.ego = X.clone()
     m.user_embeddings, m.item_embeddings = m.ego[:U], m.ego[U:]
     m._buf = [torch.empty(N, D, device=dev) for _ in range(2)]

@@ -76,19 +76,16 @@ def parity(args, build, rank, world, dev, D, DEG, E, torch):
     # ---------------- parity on a small graph (every rank also runs the 1-GPU step)
     U, I = 16000, 1600
     data, (rp, co, va), ego, part, mine, m = build(U, I)
+    from qrec_b200.base.graphRecommender import DeviceCSR
     from qrec_b200.model.ranking.LightGCN import LightGCN
 
     class Shell(LightGCN):
         def __init__(self):
             pass
-
-    class Adj(object):
-        def matmul(self, X, out, acc=None, acc_scale=0.0):
-            return E.spmm_csr(rp, co, va, X, out, acc=acc, acc_scale=acc_scale)
     ref = Shell()
     ref.num_users, ref.num_items, ref.emb_size, ref.emb_pad, ref.n_layers, ref.lRate, ref.regU, ref.device = U, I, D, D, args.layers, 0.001, 0.001, dev
-    ref.norm_adj, ref.ego = Adj(), ego.clone()
     N = U + I
+    ref.norm_adj, ref.ego = DeviceCSR.from_tensors((N, N), rp, co, va), ego.clone()
     ref._buf = [torch.empty(N, D, device=dev) for _ in range(2)]
     ref._mean, ref._grad, ref._total = (torch.zeros(N, D, device=dev) for _ in range(3))
     ref._adam_m, ref._adam_v = torch.zeros(N, D, device=dev), torch.zeros(N, D, device=dev)

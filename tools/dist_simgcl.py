@@ -50,20 +50,17 @@ def main():
         A_ui, A_iu, (lo, hi) = parallel.shard_bipartite_by_user(rp, co, va, U, I, rank, world)
         m = parallel.UserShardedSimGCL(A_ui, A_iu, ego[lo:hi].clone(), ego[U:].clone(), args.layers, 0.001, 0.001, lo, U, CL, EPS,
                                        noise_seed=0x5151, d_valid=D)
+        from qrec_b200.base.graphRecommender import DeviceCSR
         from qrec_b200.model.ranking.SimGCL import SimGCL
 
         class Shell(SimGCL):
             def __init__(self):
                 pass
-
-        class Adj(object):
-            def matmul(self, X, out, acc=None, acc_scale=0.0):
-                return E.spmm_csr(rp, co, va, X, out, acc=acc, acc_scale=acc_scale)
         ref = Shell()
         ref.num_users, ref.num_items, ref.emb_size, ref.emb_pad, ref.n_layers = U, I, D, D, args.layers
         ref.lRate, ref.regU, ref.device, ref.cl_rate, ref.eps = 0.001, 0.001, dev, CL, EPS
-        ref.norm_adj, ref.ego = Adj(), ego.clone()
         N = U + I
+        ref.norm_adj, ref.ego = DeviceCSR.from_tensors((N, N), rp, co, va), ego.clone()
         ref._buf = [torch.empty(N, D, device=dev) for _ in range(2)]
         ref._main = torch.empty(N, D, device=dev)
         ref._pert = [torch.empty(N, D, device=dev) for _ in range(2)]
